@@ -18,6 +18,7 @@ static void load_locked() {
   Config c;
   memset(&c, 0, sizeof(c));
   c.no_fat = on("MSCNN_NO_FAT");
+  c.no_rowshare = on("MSCNN_NO_ROWSHARE");
   c.no_head_taps = on("MSCNN_NO_HEAD_TAPS");
   c.verbose_conv = on("MSCNN_VERBOSE_CONV");
   c.c3_swap = on("MSCNN_C3_SWAP");

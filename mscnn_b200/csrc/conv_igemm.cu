@@ -24,6 +24,9 @@
 //         the three products per K step in the order hi*lo, lo*hi, hi*hi;
 //       - BLOCK_N = 256 (or MSCNN_NO_FAT): term-major, every (tap, chunk) k-block once per term
 //         (all of hi*hi, then hi*lo, then lo*hi) -- four weight tiles per stage would leave room for one stage.
+//   * row-share (3x3, BLOCK_N <= 128, 64x2 or 128x1 boxes): the taps dx = 0..2 of a (term, dy, chunk) read ONE
+//     haloed activation tile ({64, bw + 2, bh, 1}) from a separate A ring, each MMA warpgroup's descriptor starting
+//     dx rows further in; only the weights are fetched per tap.  Same MMAs in the same order: bit-identical results.
 //   * optional fused 2x2 / stride-2 MAX pooling of the staged output tile (box_w, box_h even): bit-identical
 //     to conv -> store -> pool_kernel, since it pools the stored (hi, lo) values.
 //   * persistent CTAs (one per SM), static round-robin tile schedule, n-tile fastest so
@@ -59,8 +62,13 @@ struct IgemmParams {
   int has_lo_out;
   int pool;           // fused 2x2 / stride-2 MAX pooling of the output tile (box_w, box_h even)
   int store_full;     // also store the un-pooled tile (0 when only the pooling layer reads it)
-  int stages, epi_bufs;
+  int stages, epi_bufs;  // stages: depth of the ring that carries B (and, without row-share, A with it)
   int fat;            // split mode with all four operand tiles (A_hi, A_lo, B_hi, B_lo) in one stage
+  int rowshare;       // 3 horizontal taps read one haloed activation tile, delivered on its own ring of a_stages slots
+  int a_stages;       // row-share: A-ring depth (0 otherwise)
+  int a_slot;         // bytes of one A slot ([A_hi] or [A_hi][A_lo]); without row-share the A part of a stage
+  int a_plane;        // bytes from A_hi to A_lo inside a slot
+  int a_wg_row;       // activation-tile row where MMA warpgroup 1's 64 pixels start (tap dx = 0)
   const float* bias;  // [Cout_pad]
   const int* dyn_n;   // optional device count: process min(*dyn_n, out_n) images only (mscnn_conv_desc.dyn_n)
   float* out_f32;     // NCHW fp32 (out_mode 1)
@@ -99,17 +107,20 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
 
   const int S = p.stages;
-  const uint32_t a_stride = FAT ? 2u * kABytes : kABytes;  // one stage: [A_hi] or [A_hi][A_lo]
-  const uint32_t b_stride = FAT ? 2u * kBBytes : kBBytes;  //            [B_hi] or [B_hi][B_lo]
+  const int SA = p.rowshare ? p.a_stages : S;  // A slots: their own ring (row-share) or one per stage
+  const uint32_t a_stride = p.a_slot;                      // [A_hi] or [A_hi][A_lo]
+  const uint32_t b_stride = FAT ? 2u * kBBytes : kBBytes;  // [B_hi] or [B_hi][B_lo]
   const uint32_t sA = smem_base;
-  const uint32_t sB = sA + S * a_stride;
-  const uint32_t sEpi = sB + S * b_stride;  // 1024-aligned: kABytes, kBBytes are multiples of 1024
+  const uint32_t sB = sA + SA * a_stride;
+  const uint32_t sEpi = sB + S * b_stride;  // 1024-aligned: a_slot and kBBytes are multiples of 1024
   constexpr int kPoolBytes = kABytes / 4;  // pooled tile: 32 rows x 128 B
   const int epi_buf_bytes = (kABytes + (p.pool ? kPoolBytes : 0)) * (p.has_lo_out ? 2 : 1);
   const uint32_t sBar = sEpi + p.epi_bufs * epi_buf_bytes;
-  // barrier layout: full[S], empty[S]
+  // barrier layout: full[S], empty[S], then for row-share a_full[SA], a_empty[SA]
   auto full_bar = [&](int s) { return sBar + 8u * s; };
   auto empty_bar = [&](int s) { return sBar + 8u * (S + s); };
+  auto a_full_bar = [&](int s) { return sBar + 8u * (2 * S + s); };
+  auto a_empty_bar = [&](int s) { return sBar + 8u * (2 * S + SA + s); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -132,6 +143,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
     for (int s = 0; s < S; ++s) {
       ptx::mbar_init(full_bar(s), 1);
       ptx::mbar_init(empty_bar(s), 2);  // one arrival per MMA warpgroup
+    }
+    for (int s = 0; p.rowshare && s < SA; ++s) {
+      ptx::mbar_init(a_full_bar(s), 1);
+      ptx::mbar_init(a_empty_bar(s), 2);
     }
     ptx::fence_mbar_init();
   }
@@ -166,6 +181,58 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
     // The whole warp walks the loops (warp-uniform control flow); one elected lane issues.
     int stage = 0;
     uint32_t phase = 0;
+    if (p.rowshare) {
+      // Row-share: the activation rows of one (term, dy, channel chunk) are fetched ONCE with a one-pixel halo on each
+      // side ({64, box_w + 2, box_h, 1} from column w0 - pad: TMA zero fill is still the padding) and serve the taps
+      // dx = 0, 1, 2; only the weight tiles are fetched per tap.
+      int sa = 0;
+      uint32_t pa = 0;
+      const uint32_t a_tx = (FAT ? 2u : 1u) * static_cast<uint32_t>((p.box_w + 2) * p.box_h) * kBlockK * 2;
+      const uint32_t b_tx = (FAT ? 2u : 1u) * kBBytes;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int n_tile = tile % p.n_tiles;
+        int tw, th, tn;
+        m_coords(tile / p.n_tiles, tw, th, tn);
+        const int w0 = tw * p.box_w - p.pad_w, h0 = th * p.box_h - p.pad_h, n0 = tn * p.box_n;
+        for (int term = 0; term < terms; ++term) {
+          const CUtensorMap* mapA = (term == 2) ? &tmA_lo : &tmA_hi;
+          const CUtensorMap* mapB = (term == 1) ? &tmB_lo : &tmB_hi;
+          for (int dy = 0; dy < p.taps_h; ++dy) {
+            for (int cc = 0; cc < p.cin_chunks; ++cc) {
+              ptx::mbar_wait(a_empty_bar(sa), pa ^ 1u);
+              if (ptx::elect_one()) {
+                ptx::mbar_expect_tx(a_full_bar(sa), a_tx);
+                const uint32_t a0 = sA + sa * a_stride;
+                ptx::tma_load_4d(a0, mapA, a_full_bar(sa), cc * kBlockK, w0, h0 + dy, n0);
+                if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, a_full_bar(sa), cc * kBlockK, w0, h0 + dy, n0);
+              }
+              __syncwarp();
+              if (++sa == SA) {
+                sa = 0;
+                pa ^= 1u;
+              }
+              for (int dx = 0; dx < p.taps_w; ++dx) {
+                const int tap = dy * p.taps_w + dx;
+                ptx::mbar_wait(empty_bar(stage), phase ^ 1u);
+                if (ptx::elect_one()) {
+                  ptx::mbar_expect_tx(full_bar(stage), b_tx);
+                  const uint32_t b0 = sB + stage * b_stride;
+                  const int kcol = (tap * p.cin_chunks + cc) * kBlockK;
+                  ptx::tma_load_2d(b0, mapB, full_bar(stage), kcol, n_tile * BLOCK_N);
+                  if (FAT) ptx::tma_load_2d(b0 + kBBytes, &tmB_lo, full_bar(stage), kcol, n_tile * BLOCK_N);
+                }
+                __syncwarp();
+                if (++stage == S) {
+                  stage = 0;
+                  phase ^= 1u;
+                }
+              }
+            }
+          }
+        }
+      }
+      return;
+    }
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int n_tile = tile % p.n_tiles;
       int tw, th, tn;
@@ -210,24 +277,31 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
   const bool issuer = (et == 0);
   const int r0 = wg * 64 + (wl >> 5) * 16 + (lane >> 2);  // accumulator rows r0 and r0 + 8
   const int cq = 2 * (lane & 3);                          // column offset within an 8-column group
-  const uint32_t a_row_off = static_cast<uint32_t>(wg) * 64u * 128u;
+  const uint32_t a_row_off = static_cast<uint32_t>(wg * p.a_wg_row) * 128u;
+  // row-share: tap dx starts dx rows further into the haloed tile
+  const uint32_t a_dx_step = p.rowshare ? 128u : 0u;
   const int hw_box = p.box_w * p.box_h;
   const int box_rows = hw_box * p.box_n;
   int stage = 0;
   uint32_t phase = 0;
+  int sa = 0;  // A ring (row-share only)
+  uint32_t pa = 0;
   int ebuf = 0;
   float acc[kAcc];
 
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int n_tile = tile % p.n_tiles;
     const int n_base = n_tile * BLOCK_N;
-    int prev = -1;
+    int prev = -1, prev_a = -1;
+    int dx = 0;
     for (int kb = 0; kb < num_kb; ++kb) {
       // operands first, then the fence: between wgmma.fence and the MMAs nothing but the MMAs is issued
-      const uint32_t a0 = sA + stage * a_stride + a_row_off, b0 = sB + stage * b_stride;
+      const uint32_t a0 = sA + (p.rowshare ? sa : stage) * a_stride + a_row_off + dx * a_dx_step;
+      const uint32_t b0 = sB + stage * b_stride;
       const uint64_t ah = ptx::gmma_desc_sw128(a0), bh = ptx::gmma_desc_sw128(b0);
-      const uint64_t al = ptx::gmma_desc_sw128(a0 + kABytes), bl = ptx::gmma_desc_sw128(b0 + kBBytes);
+      const uint64_t al = ptx::gmma_desc_sw128(a0 + p.a_plane), bl = ptx::gmma_desc_sw128(b0 + kBBytes);
       const uint32_t accumulate = kb != 0 ? 1u : 0u;  // the tile's first K step overwrites the accumulators
+      if (p.rowshare && dx == 0) ptx::mbar_wait(a_full_bar(sa), pa);
       ptx::mbar_wait(full_bar(stage), phase);
       ptx::fence_regs(acc);  // keep the accumulators in place across the asynchronous MMAs
       ptx::wgmma_fence();
@@ -249,15 +323,29 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
       // the previous k-block's MMAs have finished reading their stage: hand it back to the producer
       ptx::wgmma_wait<1>();
       if (prev >= 0 && wg_leader) ptx::mbar_arrive(empty_bar(prev));
+      if (prev_a >= 0 && wg_leader) ptx::mbar_arrive(a_empty_bar(prev_a));
       prev = stage;
+      prev_a = -1;
       if (++stage == S) {
         stage = 0;
         phase ^= 1u;
+      }
+      // k-blocks run (term, dy, chunk, dx) with dx innermost: after the last dx the A slot is done with
+      if (++dx == p.taps_w) {
+        dx = 0;
+        if (p.rowshare) {
+          prev_a = sa;
+          if (++sa == SA) {
+            sa = 0;
+            pa ^= 1u;
+          }
+        }
       }
     }
     ptx::wgmma_wait<0>();
     ptx::fence_regs(acc);
     if (prev >= 0 && wg_leader) ptx::mbar_arrive(empty_bar(prev));
+    if (prev_a >= 0 && wg_leader) ptx::mbar_arrive(a_empty_bar(prev_a));
 
     int tw, th, tn;
     m_coords(tile / p.n_tiles, tw, th, tn);
@@ -613,12 +701,53 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
   if (stages < 2) return MSCNN_ERR_INVALID;
   p.stages = stages;
   p.epi_bufs = epi_bufs;  // 0 in fp32-output mode: no staging region is carved
-  const size_t smem = (size_t)stages * stage_bytes + (size_t)epi_bufs * epi_unit + misc;
+  p.a_slot = kABytes * (p.fat ? 2 : 1);
+  p.a_plane = kABytes;
+  p.a_wg_row = 64;
+  size_t smem = (size_t)stages * stage_bytes + (size_t)epi_bufs * epi_unit + misc;
+
+  // Row-share (3 horizontal taps, one image row per MMA warpgroup: 64x2 and 128x1 boxes, BLOCK_N <= 128).  The three
+  // taps dx of a (term, dy, chunk) are the same activation rows shifted by one pixel: fetch them once with a one-pixel
+  // halo per side into an A ring, and deliver only the weight tiles per tap on the B ring.  The MMAs, their order and
+  // hence the results are those of the per-tap plan; L2->SM bytes per k-block drop from A + B to A / 3 + B.  The B ring
+  // has to be at least as deep (in taps) as the per-tap ring it replaces, else the per-tap plan stays.
+  const bool rs_box = p.box_n == 1 && ((p.box_w == 64 && p.box_h == 2) || (p.box_w == 128 && p.box_h == 1));
+  if (!cfg.no_rowshare && d->KW == 3 && BN <= 128 && rs_box) {
+    const int planes = p.fat ? 2 : 1;
+    const int a_plane = ((p.box_w + 2) * p.box_h * 128 + 1023) / 1024 * 1024;  // each plane 1024-aligned (swizzle)
+    const int a_slot = a_plane * planes;
+    const int b_stage = b_bytes * planes;
+    const int rs_misc = 8 * 2 * (8 + 4) + 1024 /*alignment slack*/;
+    // a second epilogue buffer only overlaps the two 64-channel chunks of a BLOCK_N = 128 tile
+    int rs_epi = (epi_unit == 0) ? 0 : (BN > 64 ? 2 : 1);
+    int a_stages = 2;
+    auto fit = [&](int eb, int sa) { return (kSmemBudget - rs_misc - sa * a_slot - eb * epi_unit) / b_stage; };
+    int rs_stages = fit(rs_epi, a_stages);
+    if (rs_stages < 4 && rs_epi == 2) {
+      rs_epi = 1;
+      rs_stages = fit(rs_epi, a_stages);
+    }
+    // Room left with the B ring at its cap deepens the A ring (up to 4): with short k-blocks (plain bf16) two slots
+    // leave only one group of three taps to cover the L2 latency of the next activation tile.
+    while (a_stages < 4 && fit(rs_epi, a_stages + 1) >= 8) ++a_stages;
+    rs_stages = fit(rs_epi, a_stages);
+    if (rs_stages > 8) rs_stages = 8;
+    if (rs_stages >= stages) {
+      p.rowshare = 1;
+      p.a_stages = a_stages;
+      p.a_slot = a_slot;
+      p.a_plane = a_plane;
+      p.a_wg_row = 64 / p.box_w * (p.box_w + 2) + 64 % p.box_w;  // halo-tile row of output pixel 64
+      p.stages = rs_stages;
+      p.epi_bufs = rs_epi;
+      smem = (size_t)a_stages * a_slot + (size_t)rs_stages * b_stage + (size_t)rs_epi * epi_unit + rs_misc;
+    }
+  }
   const int total_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_tiles;
   if (cfg.verbose_conv)
-    fprintf(stderr, "conv plan: N=%d H=%d W=%d C=%d Cout_pad=%d k=%dx%d BN=%d box=%dx%dx%d fat=%d terms=%d stages=%d epi_bufs=%d smem=%zu tiles=%d\n",
-            d->N, d->H, d->W, d->C, d->Cout_pad, d->KH, d->KW, BN, p.box_w, p.box_h, p.box_n, p.fat, p.num_terms, stages,
-            epi_bufs, smem, total_tiles);
+    fprintf(stderr, "conv plan: N=%d H=%d W=%d C=%d Cout_pad=%d k=%dx%d BN=%d box=%dx%dx%d fat=%d terms=%d rowshare=%d a_stages=%d stages=%d epi_bufs=%d smem=%zu tiles=%d\n",
+            d->N, d->H, d->W, d->C, d->Cout_pad, d->KH, d->KW, BN, p.box_w, p.box_h, p.box_n, p.fat, p.num_terms,
+            p.rowshare, p.a_stages, p.stages, p.epi_bufs, smem, total_tiles);
 
   plan->BN = BN;
   plan->smem = smem;
@@ -629,11 +758,12 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
     return MSCNN_OK;
   }
   const uint32_t obox[4] = {64u, (uint32_t)p.box_w, (uint32_t)p.box_h, (uint32_t)p.box_n};
+  const uint32_t abox[4] = {64u, (uint32_t)(p.box_w + (p.rowshare ? 2 : 0)), (uint32_t)p.box_h, (uint32_t)p.box_n};
   const uint64_t adim[4] = {(uint64_t)d->C, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->N};
-  int rc = tmap_nhwc_bf16(&maps[0], d->x_hi, adim, obox);
+  int rc = tmap_nhwc_bf16(&maps[0], d->x_hi, adim, abox);
   if (rc) return rc;
   if (split) {
-    rc = tmap_nhwc_bf16(&maps[1], d->x_lo, adim, obox);
+    rc = tmap_nhwc_bf16(&maps[1], d->x_lo, adim, abox);
     if (rc) return rc;
   } else {
     maps[1] = maps[0];
@@ -690,7 +820,8 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
 
 // The launch plan mscnn_conv_forward would use for `d`, as text, WITHOUT touching the device (no tensor map is encoded,
 // the pointers in `d` only have to be non-NULL where the call would require them): which instantiation, pixel box,
-// operand staging and pipeline depth.  Host-side tests pin the variant every full-size layer takes.
+// operand staging and pipeline depth (`stages` = depth of the ring carrying the weights; with rowshare=1 the
+// activation tiles have their own ring of a_stages slots).  Host-side tests pin the variant every full-size layer takes.
 extern "C" int mscnn_conv_plan_describe(const mscnn_conv_desc* d, char* buf, int cap) {
   if (!d || !buf || cap <= 0) return MSCNN_ERR_INVALID;
   mscnn::ConvPlan plan;
@@ -699,8 +830,8 @@ extern "C" int mscnn_conv_plan_describe(const mscnn_conv_desc* d, char* buf, int
   const mscnn::IgemmParams& p = plan.p;
   const int n = snprintf(buf, (size_t)cap,
                          "kernel=conv_igemm_kernel<%d, %s> box=%dx%dx%d terms=%d fat=%d pool=%d stages=%d epi_bufs=%d "
-                         "smem=%zu dyn=%d",
+                         "smem=%zu dyn=%d rowshare=%d a_stages=%d",
                          plan.BN, p.fat ? "true" : "false", p.box_w, p.box_h, p.box_n, p.num_terms, p.fat, p.pool, p.stages, p.epi_bufs,
-                         plan.smem, p.dyn_n ? 1 : 0);
+                         plan.smem, p.dyn_n ? 1 : 0, p.rowshare, p.a_stages);
   return (n > 0 && n < cap) ? MSCNN_OK : MSCNN_ERR_INVALID;
 }

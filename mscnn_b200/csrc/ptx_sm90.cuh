@@ -119,11 +119,15 @@ __device__ __forceinline__ void setmaxnreg_inc() {
 //   bits [0,14)  start address >> 4
 //   bits [16,30) leading byte offset >> 4
 //   bits [32,46) stride byte offset >> 4
-//   bits [49,52) base offset (0: every tile here starts 1024-aligned, or is not swizzled)
+//   bits [49,52) base offset (0: the tiles here are written by TMA from 1024-aligned bases, see below)
 //   bits [62,64) layout: 0 = no swizzle (core matrices of 8 rows x 16 B), 1 = SWIZZLE_128B
 // K-major bf16 tile whose rows are 128 B (64 bf16) written by TMA with CU_TENSOR_MAP_SWIZZLE_128B:
 // LBO unused (1), SBO = 8 rows * 128 B = 1024 B.  Advancing by one K step (16 bf16 = 32 B) inside
 // the 128 B swizzle atom adds 2 to the start-address field.
+// The operand may also start at any 128 B row of such a tile, with the base offset left at 0 (the row-share halo of
+// conv_igemm.cu: tap dx reads the tile dx rows further in).  wgmma takes the swizzle phase from the address bits
+// [7,10) as TMA wrote them; measured on H100 for starts 0..15 rows in, where a base offset of (addr >> 7) & 7 instead
+// reads the rows with the wrong phase.
 __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
