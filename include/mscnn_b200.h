@@ -120,14 +120,6 @@ MSCNN_API int mscnn_pack_conv_weights(const float* w_f32, void* w_hi, void* w_lo
 MSCNN_API int mscnn_pack_fc_weights(const float* w_f32, void* w_hi, void* w_lo, int Nout, int C, int H, int W,
                           int Nout_pad, int Cpad, void* stream);
 
-/* First trunk convolution (3 input channels, 3x3, pad 1, stride 1) in exact fp32 on the CUDA cores,
- * fused bias + ReLU, planes out.  x: fp32 NCHW [N][3][H][W] (the net input blob), w: fp32
- * [Cout][3][3][3] (layer blob 0 as is), y planes [N][H][W][Cout_pad].  Replaces
- * ConvolutionLayer::Forward_gpu for conv1_1 (conv_layer.cu:8-23); K = 27 is too short for a
- * tensor-core k-block, the layer is bound by its output traffic. */
-MSCNN_API int mscnn_conv3x3_c3_forward(const float* x, const float* w, const float* bias, void* y_hi, void* y_lo,
-                             int N, int H, int W, int Cout, int Cout_pad, int relu, void* stream);
-
 /* conv1_1 as one tensor-core kernel (mscnn_b200/csrc/conv_c3_tc.cu): 3 -> 64 channels, 3x3, pad 1, straight
  * from the fp32 NCHW input blob to NHWC bf16 planes [N][H][W][64] (+ReLU).  Same reference call sites as
  * mscnn_conv_forward (conv_layer.cpp:25-40, relu_layer.cpp:9-19).  The horizontal taps are overlapping views
@@ -160,19 +152,6 @@ MSCNN_API int mscnn_nchw_f32_to_planes(const float* x, void* hi, void* lo, int N
                              int Cpad, void* stream);
 MSCNN_API int mscnn_planes_to_nchw_f32(const void* hi, const void* lo, float* y, int N, int C, int H, int W,
                              int Cpad, void* stream);
-/* conv1_1 operand: 3x3 / pad 1 patches of a 3-channel NCHW fp32 image as 64-channel planes,
- * channel k = c*9 + dy*3 + dx for k < 27 (Caffe's own weight order), zero above. */
-MSCNN_API int mscnn_im2col3x3_c3_to_planes(const float* x, void* hi, void* lo, int N, int H, int W,
-                                 void* stream);
-
-/* conv1_1 on the tensor cores with the 64-wide k-block fully used: one GEMM row = two horizontally
- * adjacent pixels (54 of 64 channels = 2 x 27 taps); with the block-diagonal weights
- * [2*Cout_pad][64] from mscnn_pack_conv1_pair_weights, mscnn_conv_forward (1x1, Cout = 2*Cout_pad) on
- * the [N][H][W/2][64] patch planes writes exactly the NHWC tensor [N][H][W][Cout_pad].  W must be even. */
-MSCNN_API int mscnn_im2col3x3_c3_pair_to_planes(const float* x, void* hi, void* lo, int N, int H, int W,
-                                      void* stream);
-MSCNN_API int mscnn_pack_conv1_pair_weights(const float* w_f32 /*[Cout][3][3][3]*/, void* w_hi, void* w_lo, int Cout,
-                                  int Cout_pad, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * Pooling, pad 0, ceil-mode output size.  Replaces PoolingLayer::Forward_gpu

@@ -111,10 +111,6 @@ def _declare(L: C.CDLL) -> None:
     L.mscnn_nchw_f32_to_planes.argtypes = [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]
     L.mscnn_planes_to_nchw_f32.restype = c_int
     L.mscnn_planes_to_nchw_f32.argtypes = [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]
-    L.mscnn_im2col3x3_c3_to_planes.restype = c_int
-    L.mscnn_im2col3x3_c3_to_planes.argtypes = [c_void_p, c_void_p, c_void_p] + [c_int] * 3 + [c_void_p]
-    L.mscnn_conv3x3_c3_forward.restype = c_int
-    L.mscnn_conv3x3_c3_forward.argtypes = [c_void_p] * 5 + [c_int] * 6 + [c_void_p]
     L.mscnn_pool_forward.restype = c_int
     L.mscnn_pool_forward.argtypes = [c_void_p] * 4 + [c_int] * 7 + [c_void_p]
     L.mscnn_deconv2x_forward.restype = c_int

@@ -73,7 +73,6 @@ class CAFFE_API ConvolutionLayer : public Layer<Dtype> {
   int num_output_, channels_, kernel_h_, kernel_w_, pad_h_, pad_w_;
   bool bias_term_, fuse_relu_;
   PackedParam packed_;
-  PlaneStore patches_;  // conv1_1: 27-tap patch planes
   float* head_bias_ = nullptr;        // narrow k x k heads: bias applied by the tap gather
   unsigned long head_bias_version_ = ~0ul;
  public:

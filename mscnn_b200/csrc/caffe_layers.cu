@@ -120,9 +120,9 @@ void ConvolutionLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const 
 
 // (re)pack weights when the fp32 blobs or the precision changed
 static void ensure_packed_conv(PackedParam* pk, Blob<float>* w, Blob<float>* b, bool split, int cout, int cin,
-                               int kh, int kw, int cin_pad_override) {
+                               int kh, int kw) {
   const int cout_pad = out_pad(cout);
-  const int cin_pad = cin_pad_override > 0 ? cin_pad_override : pad64(cin);
+  const int cin_pad = pad64(cin);
   const bool stale_w = pk->w_version != w->version() || pk->split != split || pk->cout_pad != cout_pad ||
                        pk->cin_pad != cin_pad;
   if (stale_w) {
@@ -205,22 +205,15 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
                                   Caffe::stream()));
     return;
   }
-  // conv1_1-style layer (3 input channels, 3x3, pad 1): K = 27 is far below one 64-channel
-  // tensor-core k-block; it runs as a direct exact-fp32 kernel straight from the NCHW input blob.
-  const bool first_path = (channels_ == 3 && kernel_h_ == 3 && kernel_w_ == 3 && pad_h_ == 1 && pad_w_ == 1);
-  const int conv1_mode = mscnn::config().conv1_mode;  // MSCNN_CONV1: 1 "pair" | 2 "direct" | 3 "patch" | 0 default = single tensor-core kernel
-  if (first_path && num_output_ == 64 && !conv1_mode) {
-    // One kernel from the fp32 NCHW blob to planes: pixel rows staged once, the horizontal taps are
-    // descriptor-shifted views of them (mscnn_conv1_tc_forward, conv_c3_tc.cu).
+  // conv1_1 (3 -> 64 channels, 3x3, pad 1): K = 27 is far below one 64-channel tensor-core k-block.
+  // One kernel from the fp32 NCHW blob to planes: pixel rows staged once, the horizontal taps are
+  // descriptor-shifted views of them (mscnn_conv1_tc_forward, conv_c3_tc.cu).
+  if (channels_ == 3 && kernel_h_ == 3 && kernel_w_ == 3 && pad_h_ == 1 && pad_w_ == 1 && num_output_ == 64) {
     Blob<Dtype>* wb = this->blobs_[0].get();
-    constexpr long kTcKey = -64;
-    if (packed_.w_version != wb->version() || packed_.key != kTcKey) {
+    if (packed_.w_version != wb->version()) {
       packed_.w.reserve((size_t)mscnn_conv1_tc_packed_bytes(), false);
       MSCNN_CHECK(mscnn_pack_conv1_tc_weights(wb->gpu_data(), packed_.w.hi, 1, Caffe::stream()));
       packed_.w_version = wb->version();
-      packed_.key = kTcKey;
-      packed_.b_version = ~0ul;
-      if (packed_.bias) { CUDA_CHECK(cudaFree(packed_.bias)); packed_.bias = nullptr; }
     }
     const unsigned long bver = bias ? bias->version() : 0;
     if (!packed_.bias || packed_.b_version != bver) {
@@ -237,87 +230,15 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
                                        N, H, W, fuse_relu_ ? 1 : 0, Caffe::stream()));
     return;
   }
-  if (first_path && (W % 2 == 0) && num_output_ % 64 == 0 && conv1_mode == 1) {
-    // Pixel-pair GEMM: rows = two adjacent pixels (K = 54 of 64), block-diagonal weights, the output
-    // [N][H][W/2][2*Cout] is the NHWC tensor [N][H][W][Cout] (see mscnn_im2col3x3_c3_pair_to_planes).
-    const int cp = num_output_;  // multiple of 64
-    Blob<Dtype>* wb = this->blobs_[0].get();
-    if (packed_.w_version != wb->version() || packed_.split != split || packed_.cout_pad != 2 * cp || packed_.key != -2) {
-      packed_.key = -2;
-      packed_.w.reserve((size_t)2 * cp * 64 * 2, split);
-      MSCNN_CHECK(mscnn_pack_conv1_pair_weights(wb->gpu_data(), packed_.w.hi, split ? packed_.w.lo : nullptr,
-                                                num_output_, cp, Caffe::stream()));
-      packed_.w_version = wb->version();
-      packed_.split = split;
-      packed_.b_version = ~0ul;
-      if (packed_.bias) { CUDA_CHECK(cudaFree(packed_.bias)); packed_.bias = nullptr; }
-    }
-    const unsigned long bver = bias ? bias->version() : 0;
-    if (!packed_.bias || packed_.b_version != bver) {
-      if (!packed_.bias) CUDA_CHECK(cudaMalloc(&packed_.bias, sizeof(float) * 2 * cp));
-      CUDA_CHECK(cudaMemsetAsync(packed_.bias, 0, sizeof(float) * 2 * cp, Caffe::stream()));
-      if (bias) {
-        CUDA_CHECK(cudaMemcpyAsync(packed_.bias, bias->gpu_data(), sizeof(float) * num_output_,
-                                   cudaMemcpyDeviceToDevice, Caffe::stream()));
-        CUDA_CHECK(cudaMemcpyAsync(packed_.bias + cp, bias->gpu_data(), sizeof(float) * num_output_,
-                                   cudaMemcpyDeviceToDevice, Caffe::stream()));
-      }
-      packed_.b_version = bver;
-    }
-    packed_.cout_pad = 2 * cp;
-    const size_t bytes = (size_t)N * H * (W / 2) * 64 * 2;
-    patches_.reserve(bytes, split);
-    MSCNN_CHECK(mscnn_im2col3x3_c3_pair_to_planes(bottom[0]->gpu_data(), patches_.hi,
-                                                  split ? patches_.lo : nullptr, N, H, W, Caffe::stream()));
-    typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
-    d.x_hi = patches_.hi;
-    d.x_lo = split ? patches_.lo : nullptr;
-    d.N = N; d.H = H; d.W = W / 2; d.C = 64;
-    d.w_hi = packed_.w.hi;
-    d.w_lo = split ? packed_.w.lo : nullptr;
-    d.bias = packed_.bias;
-    d.Cout = 2 * cp; d.Cout_pad = 2 * cp;
-    d.KH = d.KW = 1;
-    d.relu = fuse_relu_ ? 1 : 0;
-    d.out_mode = MSCNN_OUT_NHWC_BF16;
-    d.y_hi = y.hi;
-    d.y_lo = y.lo;
-    d.dyn_n = this->dyn_rows_device();
-  MSCNN_CHECK(mscnn_conv_forward(&d, Caffe::stream()));
-    return;
-  }
-  if (first_path && conv1_mode != 3) {
-    typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
-    MSCNN_CHECK(mscnn_conv3x3_c3_forward(bottom[0]->gpu_data(), this->blobs_[0]->gpu_data(),
-                                         bias ? bias->gpu_data() : nullptr, y.hi, y.lo, N, H, W, num_output_,
-                                         y.cpad, fuse_relu_ ? 1 : 0, Caffe::stream()));
-    return;
-  }
-  // (MSCNN_CONV1=patch: the same layer as a 1x1 GEMM over single-pixel 27-tap patch planes, kept for comparison)
-  const bool patch_path = first_path;
-  if (patch_path) {
-    ensure_packed_conv(&packed_, this->blobs_[0].get(), bias, split, num_output_, 27, 1, 1, 64);
-    const size_t bytes = (size_t)N * H * W * 64 * 2;
-    patches_.reserve(bytes, split);
-    MSCNN_CHECK(mscnn_im2col3x3_c3_to_planes(bottom[0]->gpu_data(), patches_.hi, split ? patches_.lo : nullptr, N,
-                                             H, W, Caffe::stream()));
-    d.x_hi = patches_.hi;
-    d.x_lo = split ? patches_.lo : nullptr;
-    d.C = 64;
-    d.KH = d.KW = 1;
-    d.pad_h = d.pad_w = 0;
-  } else {
-    ensure_packed_conv(&packed_, this->blobs_[0].get(), bias, split, num_output_, channels_, kernel_h_, kernel_w_,
-                       0);
-    typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
-    d.x_hi = x.hi;
-    d.x_lo = x.lo;
-    d.C = x.cpad;
-    d.KH = kernel_h_;
-    d.KW = kernel_w_;
-    d.pad_h = pad_h_;
-    d.pad_w = pad_w_;
-  }
+  ensure_packed_conv(&packed_, this->blobs_[0].get(), bias, split, num_output_, channels_, kernel_h_, kernel_w_);
+  typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
+  d.x_hi = x.hi;
+  d.x_lo = x.lo;
+  d.C = x.cpad;
+  d.KH = kernel_h_;
+  d.KW = kernel_w_;
+  d.pad_h = pad_h_;
+  d.pad_w = pad_w_;
   d.N = N; d.H = H; d.W = W;
   d.w_hi = packed_.w.hi;
   d.w_lo = split ? packed_.w.lo : nullptr;
@@ -328,7 +249,7 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
   if (packed_.cout_pad % 64 == 0) {
     d.out_mode = MSCNN_OUT_NHWC_BF16;
     const int ho = top[0]->height(), wo = top[0]->width();
-    const bool pool_here = fused_pool_ && !patch_path && (ho % 2 == 0) && (wo % 2 == 0);
+    const bool pool_here = fused_pool_ && (ho % 2 == 0) && (wo % 2 == 0);
     if (!pool_here || fused_keep_full_) {
       typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
       d.y_hi = y.hi;

@@ -21,10 +21,6 @@ static void load_locked() {
   c.no_rowshare = on("MSCNN_NO_ROWSHARE");
   c.no_head_taps = on("MSCNN_NO_HEAD_TAPS");
   c.verbose_conv = on("MSCNN_VERBOSE_CONV");
-  c.c3_swap = on("MSCNN_C3_SWAP");
-  if (const char* e = std::getenv("MSCNN_CONV1")) {
-    c.conv1_mode = !strcmp(e, "pair") ? 1 : !strcmp(e, "direct") ? 2 : 3;
-  }
   c.epoch = g_cfg.epoch + 1;
   g_cfg = c;
   g_loaded.store(true, std::memory_order_release);

@@ -9,8 +9,7 @@ struct Config {
   bool no_fat;      // MSCNN_NO_FAT: term-major k-blocks for every fp32-faithful layer
   bool no_rowshare; // MSCNN_NO_ROWSHARE: one activation tile per tap, also where three horizontal taps could share one
   bool no_head_taps;
-  bool verbose_conv, c3_swap;
-  int conv1_mode;  // MSCNN_CONV1: 0 = tensor-core kernel (default), 1 = pair, 2 = direct, 3 = patch
+  bool verbose_conv;
   unsigned epoch;  // bumped by every reload: cached plans carry the epoch they were built under
 };
 

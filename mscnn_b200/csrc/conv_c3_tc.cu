@@ -4,8 +4,8 @@
 // (src/caffe/layers/conv_layer.cpp:25-40, base_conv_layer.cpp:257-280; the reference builds a
 // 27 x (H*W) im2col buffer per image and calls sgemm).  The layer is HBM-bound (K = 27): per pixel it
 // must read 12 B and write 64 channels x 2 B (x2 for the (hi, lo) pair) = 256 B: 4.2 GB for 8 x 768 x 2560
-// pixels, about 1.3 ms at the H100's 3.35 TB/s.  The alternative formulation (im2col3x3_c3_pair_kernel + the generic
-// implicit-GEMM kernel, MSCNN_CONV1=pair) writes and re-reads a 2 GB patch tensor.  Here:
+// pixels, about 1.3 ms at the H100's 3.35 TB/s.  An im2col patch tensor feeding a GEMM (27 taps padded to
+// 64 bf16 channels) would add 128 B per pixel and plane, 2 GB per plane at that size, written and read again.  Here:
 //   * producer warps read the fp32 image rows themselves (coalesced along x, zero padding by predication),
 //     split to bf16 (hi, lo) and write them to shared memory as PIXEL ROWS of 8 channels (3 real) = 16 B per
 //     pixel.  Nothing else is staged: no im2col tensor, no padded copy of the image.
@@ -28,7 +28,6 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include "config.h"
 #include "mscnn_b200.h"
 #include "ptx_sm90.cuh"
 #include "tmap.h"
@@ -59,7 +58,6 @@ struct Params {
   const float* bias;  // [64]
   int N, H, W, tiles_w;
   int split, relu;
-  int swap;  // debug (MSCNN_C3_SWAP=1): exchange the LBO / SBO fields of the operand descriptors
 };
 
 // SPLIT is a template parameter so that the MMA sequence has no runtime branch (see conv_igemm.cu).
@@ -193,9 +191,8 @@ conv_c3_tc_kernel(const __grid_constant__ CUtensorMap tmO_hi, const __grid_const
         for (int m = 0; m < 2; ++m) {  // K chunks (2m, 2m+1) = pixels r + 2m, r + 2m + 1
           const uint32_t aoff = dy * kRowBytes + m * 32;
           const uint32_t boff = (dy * 4 + 2 * m) * 1024;
-          const uint32_t a_l = p.swap ? 128 : 16, a_s = p.swap ? 16 : 128, b_l = p.swap ? 128 : 1024, b_s = p.swap ? 1024 : 128;
-          const uint64_t ah = ptx::gmma_desc_nosw(a_hi + aoff, a_l, a_s), al = ptx::gmma_desc_nosw(a_lo + aoff, a_l, a_s);
-          const uint64_t bh = ptx::gmma_desc_nosw(w_hi + boff, b_l, b_s), bl = ptx::gmma_desc_nosw(w_lo + boff, b_l, b_s);
+          const uint64_t ah = ptx::gmma_desc_nosw(a_hi + aoff, 16, 128), al = ptx::gmma_desc_nosw(a_lo + aoff, 16, 128);
+          const uint64_t bh = ptx::gmma_desc_nosw(w_hi + boff, 1024, 128), bl = ptx::gmma_desc_nosw(w_lo + boff, 1024, 128);
           if constexpr (SPLIT) {
             ptx::wgmma_bf16<kCout>(acc, ah, bl, accum);
             ptx::wgmma_bf16<kCout>(acc, al, bh, 1u);
@@ -295,7 +292,6 @@ extern "C" int mscnn_conv1_tc_forward(const float* x, const void* packed_w, cons
   p.tiles_w = (W + c3::kTileW - 1) / c3::kTileW;
   p.split = y_lo ? 1 : 0;
   p.relu = relu ? 1 : 0;
-  p.swap = mscnn::config().c3_swap ? 1 : 0;
   CUtensorMap maps[2];
   memset(maps, 0, sizeof(maps));
   const uint64_t odim[4] = {64u, (uint64_t)W, (uint64_t)H, (uint64_t)N};

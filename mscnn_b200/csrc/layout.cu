@@ -90,118 +90,6 @@ __global__ void planes_to_nchw_kernel(const __nv_bfloat16* __restrict__ hi,
   }
 }
 
-// One thread per pixel; 27 taps gathered from the 3-channel image, written as one 128 B row
-// per plane (eight 16 B stores).
-__global__ void im2col3x3_c3_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ hi,
-                                    __nv_bfloat16* __restrict__ lo, int N, int H, int W) {
-  const size_t total = (size_t)N * H * W;
-  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const int w = idx % W;
-  const int h = (idx / W) % H;
-  const int n = idx / ((size_t)W * H);
-  __align__(16) __nv_bfloat16 vh[64];
-  __align__(16) __nv_bfloat16 vl[64];
-#pragma unroll
-  for (int k = 0; k < 64; ++k) {
-    vh[k] = __float2bfloat16_rn(0.f);
-    vl[k] = vh[k];
-  }
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-#pragma unroll
-    for (int dy = 0; dy < 3; ++dy) {
-#pragma unroll
-      for (int dx = 0; dx < 3; ++dx) {
-        const int hh = h + dy - 1, ww = w + dx - 1;
-        float v = 0.f;
-        if (hh >= 0 && hh < H && ww >= 0 && ww < W) v = x[((size_t)(n * 3 + c) * H + hh) * W + ww];
-        split_bf16(v, vh[c * 9 + dy * 3 + dx], vl[c * 9 + dy * 3 + dx]);
-      }
-    }
-  }
-  uint4* oh = reinterpret_cast<uint4*>(hi + idx * 64);
-  const uint4* sh = reinterpret_cast<const uint4*>(vh);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) oh[j] = sh[j];
-  if (lo) {
-    uint4* ol = reinterpret_cast<uint4*>(lo + idx * 64);
-    const uint4* sl = reinterpret_cast<const uint4*>(vl);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) ol[j] = sl[j];
-  }
-}
-
-// conv1_1 as a tensor-core GEMM with K = 64 fully used: one GEMM row = TWO horizontally adjacent
-// pixels.  Channels [0,27) hold the 27 taps (c*9 + dy*3 + dx) of pixel 2j, [27,54) those of pixel
-// 2j+1, [54,64) zero.  With block-diagonal weights [2*Cout][64] the 1x1 GEMM emits
-// [pixel 2j: Cout ch][pixel 2j+1: Cout ch] per row, which in memory IS the NHWC tensor [N][H][W][Cout].
-// One thread per pixel pair; one 128-byte row per plane.
-__global__ void im2col3x3_c3_pair_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ hi,
-                                         __nv_bfloat16* __restrict__ lo, int N, int H, int W) {
-  const int W2 = W / 2;
-  const size_t total = (size_t)N * H * W2;
-  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const int j = idx % W2;
-  const int h = (idx / W2) % H;
-  const int n = idx / ((size_t)W2 * H);
-  __align__(16) __nv_bfloat16 vh[64];
-  __align__(16) __nv_bfloat16 vl[64];
-#pragma unroll
-  for (int k = 54; k < 64; ++k) {
-    vh[k] = __float2bfloat16_rn(0.f);
-    vl[k] = vh[k];
-  }
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-#pragma unroll
-    for (int dy = 0; dy < 3; ++dy) {
-      const int hh = h + dy - 1;
-      float col[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int ww = 2 * j + q - 1;
-        col[q] = (hh >= 0 && hh < H && ww >= 0 && ww < W) ? x[((size_t)(n * 3 + c) * H + hh) * W + ww] : 0.f;
-      }
-#pragma unroll
-      for (int dx = 0; dx < 3; ++dx) {
-        split_bf16(col[dx], vh[c * 9 + dy * 3 + dx], vl[c * 9 + dy * 3 + dx]);
-        split_bf16(col[dx + 1], vh[27 + c * 9 + dy * 3 + dx], vl[27 + c * 9 + dy * 3 + dx]);
-      }
-    }
-  }
-  uint4* oh = reinterpret_cast<uint4*>(hi + idx * 64);
-  const uint4* sh = reinterpret_cast<const uint4*>(vh);
-#pragma unroll
-  for (int q = 0; q < 8; ++q) oh[q] = sh[q];
-  if (lo) {
-    uint4* ol = reinterpret_cast<uint4*>(lo + idx * 64);
-    const uint4* sl = reinterpret_cast<const uint4*>(vl);
-#pragma unroll
-    for (int q = 0; q < 8; ++q) ol[q] = sl[q];
-  }
-}
-
-// block-diagonal weights for the pixel-pair GEMM: out[r][k], r < 2*Cout_pad, k < 64
-//   r <  Cout_pad: out[r][k]      = w[r][k]              for k < 27
-//   r >= Cout_pad: out[r][27 + k] = w[r - Cout_pad][k]   for k < 27
-__global__ void pack_conv1_pair_w_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ hi,
-                                         __nv_bfloat16* __restrict__ lo, int Cout, int Cout_pad) {
-  const int total = 2 * Cout_pad * 64;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int k = i % 64, r = i / 64;
-    const int half = r / Cout_pad, co = r % Cout_pad;
-    const int t = k - 27 * half;
-    float v = 0.f;
-    if (co < Cout && t >= 0 && t < 27) v = w[co * 27 + t];
-    __nv_bfloat16 h, l;
-    split_bf16(v, h, l);
-    hi[i] = h;
-    if (lo) lo[i] = l;
-  }
-}
-
 // out[(co*KH*KW + tap)*Cin_pad + ci] = w[((co*Cin + ci)*KH*KW) + tap]
 __global__ void pack_conv_w_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ hi,
                                    __nv_bfloat16* __restrict__ lo, int Cout, int Cin, int taps,
@@ -329,17 +217,6 @@ extern "C" int mscnn_planes_to_nchw_f32(const void* hi, const void* lo, float* y
   return check_launch("planes_to_nchw");
 }
 
-extern "C" int mscnn_im2col3x3_c3_to_planes(const float* x, void* hi, void* lo, int N, int H, int W,
-                                            void* stream) {
-  if (!x || !hi || N <= 0 || H <= 0 || W <= 0) return MSCNN_ERR_INVALID;
-  const size_t total = (size_t)N * H * W;
-  const int threads = 128;
-  mscnn::note_launch();
-  im2col3x3_c3_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0,
-                        (cudaStream_t)stream>>>(x, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, N, H, W);
-  return check_launch("im2col3x3_c3");
-}
-
 extern "C" int mscnn_pack_conv_weights(const float* w, void* hi, void* lo, int Cout, int Cin, int KH,
                                        int KW, int Cout_pad, int Cin_pad, void* stream) {
   if (!w || !hi || Cout <= 0 || Cin <= 0 || Cout_pad < Cout || Cin_pad < Cin || Cin_pad % 64)
@@ -388,24 +265,4 @@ extern "C" int mscnn_head_gather(const float* P, int ld, const float* bias, floa
     default: return MSCNN_ERR_INVALID;  // the MS-CNN heads have cls_num + 4 = 6 or 9 channels
   }
   return check_launch("head_gather");
-}
-
-extern "C" int mscnn_im2col3x3_c3_pair_to_planes(const float* x, void* hi, void* lo, int N, int H, int W,
-                                                 void* stream) {
-  if (!x || !hi || N <= 0 || H <= 0 || W <= 0 || (W & 1)) return MSCNN_ERR_INVALID;
-  const size_t total = (size_t)N * H * (W / 2);
-  const int threads = 128;
-  mscnn::note_launch();
-  im2col3x3_c3_pair_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0, (cudaStream_t)stream>>>(
-      x, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, N, H, W);
-  return check_launch("im2col3x3_c3_pair");
-}
-
-extern "C" int mscnn_pack_conv1_pair_weights(const float* w, void* hi, void* lo, int Cout, int Cout_pad,
-                                             void* stream) {
-  if (!w || !hi || Cout <= 0 || Cout_pad < Cout || Cout_pad % 32) return MSCNN_ERR_INVALID;
-  mscnn::note_launch();
-  pack_conv1_pair_w_kernel<<<(2 * Cout_pad * 64 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
-      w, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, Cout, Cout_pad);
-  return check_launch("pack_conv1_pair_w");
 }

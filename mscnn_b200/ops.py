@@ -73,16 +73,6 @@ def planes_to_nchw(p: Planes) -> torch.Tensor:
     return y
 
 
-def im2col3x3_c3(x: torch.Tensor, split: bool) -> Planes:
-    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.shape[1] == 3
-    n, _, h, w = x.shape
-    hi = torch.empty((n, h, w, 64), dtype=torch.bfloat16, device=x.device)
-    lo = torch.empty_like(hi) if split else None
-    capi.check(capi.lib().mscnn_im2col3x3_c3_to_planes(capi.ptr(x), capi.ptr(hi), capi.ptr(lo),
-                                                       n, h, w, _stream()), "im2col3x3_c3")
-    return Planes(hi, lo, 27)
-
-
 def pack_conv_weights(w: torch.Tensor, b: torch.Tensor | None, split: bool,
                       cout_pad: int | None = None, cin_pad: int | None = None) -> PackedWeights:
     """w: [Cout][Cin][KH][KW] fp32 (Caffe blob 0), b: [Cout] fp32 (blob 1) or None."""
@@ -313,19 +303,6 @@ def detect_postprocess(cfg: capi.DetectCfg, n: int, proposals_score, cls_pred, b
                                                    nbytes.value, capi.ptr(dets), capi.ptr(counts), _stream()),
                "detect_postprocess")
     return dets, counts
-
-
-def conv3x3_c3_forward(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None, relu: bool, split: bool) -> Planes:
-    """conv1_1 shape: x [N,3,H,W] fp32 NCHW, w [Cout,3,3,3] fp32 -> planes (direct fp32 kernel)."""
-    n, _, h, wd = x.shape
-    cout = w.shape[0]
-    cp = pad64(cout)
-    y_hi = torch.empty((n, h, wd, cp), dtype=torch.bfloat16, device=x.device)
-    y_lo = torch.empty_like(y_hi) if split else None
-    capi.check(capi.lib().mscnn_conv3x3_c3_forward(capi.ptr(x), capi.ptr(w), capi.ptr(b), capi.ptr(y_hi),
-                                                   capi.ptr(y_lo), n, h, wd, cout, cp, int(relu), _stream()),
-               "conv3x3_c3_forward")
-    return Planes(y_hi, y_lo, cout)
 
 
 def conv1_tc_forward(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None, relu: bool, split: bool) -> Planes:

@@ -53,6 +53,9 @@ CASES = [
     ("roi_c1_like",    7, 128, 7, 7, 128, 3, 0),
     ("conv1x1",        1, 64, 8, 24, 64, 1, 0),
     ("deepK",          1, 512, 6, 40, 128, 3, 1),
+    # 3 input channels padded to one 64-channel chunk: conv1_1-like layers with Cout != 64
+    ("c3_n48",         2, 3, 21, 150, 48, 3, 1),
+    ("c3_n128",        1, 3, 20, 36, 128, 3, 1),
     # many more M tiles than SMs: every persistent CTA walks several tiles through the ring
     ("mt_n64",         2, 64, 128, 160, 64, 3, 1),
     ("mt_n128",        2, 64, 128, 320, 128, 3, 1),
@@ -202,50 +205,6 @@ def test_inner_product(cuda, split):
         _report("fc6", got, ref, 2.0 ** -8, 1e-5 * rms)
         ref2 = got.double() @ wt2.bfloat16().double().t() + b2.double()
         _report("fc_narrow", got2, ref2, 1e-5, 1e-5 * float(ref2.pow(2).mean().sqrt()))
-
-
-@pytest.mark.parametrize("split", [True, False], ids=["split", "bf16"])
-def test_conv1_1_im2col(cuda, split):
-    """conv1_1: 3 -> 64, 3x3 pad 1 as a 1x1 GEMM over the 27-tap patch planes."""
-    from mscnn_b200 import ops
-    g = torch.Generator(device="cpu").manual_seed(3)
-    n, h, w = 2, 20, 36
-    x = (torch.randint(0, 256, (n, 3, h, w), generator=g).float()
-         - torch.tensor([104.0, 117.0, 123.0]).view(1, 3, 1, 1)).to(cuda).contiguous()
-    wt = (torch.randn((64, 3, 3, 3), generator=g) * (2.0 / 27) ** 0.5).to(cuda)
-    b = (torch.randn((64,), generator=g) * 0.1).to(cuda)
-    patches = ops.im2col3x3_c3(x, split)
-    wp = ops.pack_conv_weights(wt.view(64, 27, 1, 1).contiguous(), b, split)
-    yp = ops.conv_forward(patches, wp, 0, relu=True)
-    got = ops.planes_to_nchw(yp)
-    torch.cuda.synchronize()
-    if split:
-        ref = _ref_conv(x, wt, b, 1, True)
-        _report("conv1_1", got, ref, 1e-4, 1e-4 * float(ref.pow(2).mean().sqrt()))
-    else:
-        ref = _ref_conv(x.bfloat16().float(), wt.bfloat16().float(), b, 1, True)
-        _report("conv1_1", got, ref, 2.0 ** -8, 1e-5 * float(ref.pow(2).mean().sqrt()))
-
-
-@pytest.mark.parametrize("split", [True, False], ids=["split", "bf16"])
-def test_conv1_1_direct(cuda, split):
-    """conv1_1 as the direct exact-fp32 kernel (the path the Net uses)."""
-    from mscnn_b200 import ops
-    g = torch.Generator(device="cpu").manual_seed(4)
-    n, h, w = 2, 21, 150        # W crosses a 128-pixel tile boundary
-    x = (torch.randint(0, 256, (n, 3, h, w), generator=g).float()
-         - torch.tensor([104.0, 117.0, 123.0]).view(1, 3, 1, 1)).to(cuda).contiguous()
-    wt = (torch.randn((64, 3, 3, 3), generator=g) * (2.0 / 27) ** 0.5 / 64).to(cuda)
-    b = (torch.randn((64,), generator=g) * 0.1).to(cuda)
-    yp = ops.conv3x3_c3_forward(x, wt, b, relu=True, split=split)
-    got = ops.planes_to_nchw(yp)
-    torch.cuda.synchronize()
-    ref = _ref_conv(x, wt, b, 1, True)
-    rms = float(ref.pow(2).mean().sqrt())
-    if split:
-        _report("conv1_1_direct", got, ref, 2e-5, 2e-5 * rms)      # fp32 FMA + 2^-18 split of the output
-    else:
-        _report("conv1_1_direct", got, ref, 2.0 ** -8, 1e-5 * rms)
 
 
 @pytest.mark.parametrize("split", [True, False], ids=["split", "bf16"])

@@ -26,19 +26,6 @@ def timeit(fn, iters=5):
 def main():
     dev = torch.device("cuda:0")
     B = 8
-    x = (torch.randint(0, 256, (B, 3, 768, 2560), device=dev).float() - 110.0).contiguous()
-    wt = torch.randn((64, 3, 3, 3), device=dev) * 0.01
-    b = torch.zeros(64, device=dev)
-    for split in (True, False):
-        t = timeit(lambda: ops.conv3x3_c3_forward(x, wt, b, True, split))
-        wp = ops.pack_conv_weights(wt.view(64, 27, 1, 1).contiguous(), b, split)
-
-        def gemm_path():
-            p = ops.im2col3x3_c3(x, split)
-            return ops.conv_forward(p, wp, 0, relu=True)
-        t2 = timeit(gemm_path)
-        print(f"conv1_1 split={split}: direct {t:.3f} ms, patch-GEMM {t2:.3f} ms", flush=True)
-    del x
     for name, cin, h, w, cout in [("conv1_2", 64, 768, 2560, 64), ("conv2_1", 64, 384, 1280, 128), ("conv2_2", 128, 384, 1280, 128)]:
         xin = torch.randn((B, cin, h, w), device=dev)
         wt = torch.randn((cout, cin, 3, 3), device=dev) * (2.0 / (cin * 9)) ** 0.5
