@@ -292,6 +292,20 @@ MSCNN_API int mscnn_detect_postprocess(const mscnn_detect_cfg* cfg, int N, const
                              const float* cls_pred, const float* bbox_pred, const int* num_rois,
                              void* workspace, size_t workspace_bytes, float* dets, int* det_counts,
                              void* stream);
+/* Batches of images with different ORIGINAL sizes (all resized to the one net input).  The reference drivers handle
+ * one frame at a time and rescale / clip its detections with that frame's own ratios
+ * (examples/kitti_car/run_mscnn_detection.m:64-65 and :111-116, run_cascademscnn.m:77-80 and :101-105); the *_sized
+ * entries take them per image instead of from the cfg:
+ *   geom: HOST float [N][4] = ratio_h, ratio_w, org_h, org_w of each image (every value > 0, finite); the cfg's four
+ *   geometry fields are ignored.  Image n's result equals bit for bit the cfg entry's with image n's four values.
+ * mscnn_detect_image_geometry (host-only, no CUDA call): geom from the net input size and the original sizes
+ *   org_hw [N][2] = h, w: ratio = (float)((double)net / (double)org), org = (float)org, the values the MATLAB drivers
+ *   compute (run_mscnn_detection.m:65). */
+MSCNN_API int mscnn_detect_image_geometry(int net_h, int net_w, int N, const int* org_hw, float* geom);
+MSCNN_API int mscnn_detect_postprocess_sized(const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
+                                             const float* cls_pred, const float* bbox_pred, const int* num_rois,
+                                             void* workspace, size_t workspace_bytes, float* dets, int* det_counts,
+                                             const float* geom, void* stream);
 
 /* Packed output of the same post-process, for the multi-GPU exchange below: `payload` (device,
  * mscnn_detect_payload_floats(N, max_rois_per_image) floats) = int32 header [N, total, counts[0..N)] padded to a
@@ -300,6 +314,11 @@ MSCNN_API size_t mscnn_detect_payload_floats(int N, int max_rois_per_image);
 MSCNN_API int mscnn_detect_postprocess_packed(const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
                                     const float* cls_pred, const float* bbox_pred, const int* num_rois,
                                     void* workspace, size_t workspace_bytes, float* payload, void* stream);
+/* Per-image geometry as in mscnn_detect_postprocess_sized (run_mscnn_detection.m:111-116). */
+MSCNN_API int mscnn_detect_postprocess_packed_sized(const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
+                                                    const float* cls_pred, const float* bbox_pred, const int* num_rois,
+                                                    void* workspace, size_t workspace_bytes, float* payload,
+                                                    const float* geom, void* stream);
 
 /* Cascade variant: replaces the MATLAB code after net.forward in examples/kitti_car/run_cascademscnn.m:99-126
  * (+ utils/bbNms.m:112-126).  The net already holds decoded boxes and probabilities:
@@ -311,6 +330,11 @@ MSCNN_API int mscnn_cascade_detect_postprocess(const mscnn_detect_cfg* cfg, int 
                                      const float* cls_prob, const float* output_bbox, const int* num_rois,
                                      void* workspace, size_t workspace_bytes, float* dets, int* det_counts,
                                      void* stream);
+/* Per-image geometry as in mscnn_detect_postprocess_sized (run_cascademscnn.m:77-80, :101-105). */
+MSCNN_API int mscnn_cascade_detect_postprocess_sized(const mscnn_detect_cfg* cfg, int N, const float* proposals,
+                                                     const float* cls_prob, const float* output_bbox,
+                                                     const int* num_rois, void* workspace, size_t workspace_bytes,
+                                                     float* dets, int* det_counts, const float* geom, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * Image pre-processing (the step in front of the path, SURVEY.md 8(f)-3).  Replaces the MATLAB code
@@ -320,7 +344,8 @@ MSCNN_API int mscnn_cascade_detect_postprocess(const mscnn_detect_cfg* cfg, int 
  *   (RGB -> BGR) -> single -> minus mean [104 117 123] -> W-fastest planes = the net's `data` blob.
  * images: uint8 [N][in_h][in_w][3] interleaved (what an image decoder returns), all N of one size;
  * data: fp32 [N][3][out_h][out_w].  mean[] is indexed by OUTPUT channel (after the swap).
- * A plan holds the fp64 tap tables of one (in, out) size pair on the device. */
+ * A plan has one output size, mean and channel order.  It caches the fp64 tap tables of every input size it has
+ * seen on the device (built once per distinct size); the size it was created with is the first. */
 typedef struct mscnn_preprocess_desc {
   int in_h, in_w;   /* original image */
   int out_h, out_w; /* net input */
@@ -336,6 +361,16 @@ MSCNN_API int mscnn_preprocess_forward(void* plan, int N, const unsigned char* i
  * the plan (pinned host memory makes it asynchronous), then the kernels. */
 MSCNN_API int mscnn_preprocess_forward_host(void* plan, int N, const unsigned char* host_images, float* data,
                                             void* stream);
+/* Images of different original sizes in one batch, all resized to the plan's output size.  The reference reads each
+ * frame's size inside its loop (examples/kitti_car/run_mscnn_detection.m:64-65, run_cascademscnn.m:77-80).
+ *   in_hw: HOST int [N][2] = h, w of each image (>= 1); images packed back to back in batch order, image n starting
+ *   at byte sum_{m<n} h_m * w_m * 3.  Each slot of `data` equals the result of a plan made for that image's size.
+ *   A size the plan has not seen yet builds and uploads its tap tables first (synchronous, once per size).
+ * _host: the same with HOST images, one async H2D copy into the plan's staging buffer. */
+MSCNN_API int mscnn_preprocess_forward_sized(void* plan, int N, const int* in_hw, const unsigned char* images,
+                                             float* data, void* stream);
+MSCNN_API int mscnn_preprocess_forward_sized_host(void* plan, int N, const int* in_hw,
+                                                  const unsigned char* host_images, float* data, void* stream);
 /* Host-only helpers (no CUDA call; usable on a GPU-less box):
  * imresize's tap tables for one dimension: returns the tap count P (<= cap_taps) and fills
  * host_weights / host_indices as [out_len][cap_taps] (0-based indices); mscnn_imresize_taps = P alone. */
@@ -414,6 +449,20 @@ MSCNN_API const float* mscnn_net_blob_device(void* net, const char* blob);
 /* uint8 host images -> pre-processing kernels -> the input blob (N, in size and out size from the plan / blob). */
 MSCNN_API int mscnn_net_set_input_images(void* net, const char* blob, void* preprocess_plan, int N,
                                          const unsigned char* host_images);
+/* Batches of frames with different original sizes (run_mscnn_detection.m:64-65 reads each frame's size; the frames
+ * are resized to the one net input size).
+ * mscnn_net_set_input_images_sized: mscnn_preprocess_forward_sized_host into the blob, and records in_hw [N][2] as
+ *   the original sizes of the images the NEXT forward consumes.
+ * mscnn_net_set_input_geometry: records org_hw [N][2] (host) alone, for hosts that resize themselves and fill the
+ *   input with mscnn_net_set_blob*; N = 0 or org_hw = NULL clears it.
+ * A forward from the first layer turns the recorded sizes into the per-image geometry of its outputs (net size = the
+ * input blob's H and W; N must match the input blob) and clears them; without recorded sizes its geometry is "none".
+ * mscnn_net_detect, _gather, _push and _cascade rescale and clip with the last forward's per-image geometry when it
+ * has one (run_mscnn_detection.m:111-116), with the cfg's ratio_* / org_* otherwise.  So the pipelined order "set
+ * batch k + 1, detect batch k" pairs each batch with its own sizes.  mscnn_net_set_input_images drops recorded sizes. */
+MSCNN_API int mscnn_net_set_input_images_sized(void* net, const char* blob, void* preprocess_plan, int N,
+                                               const int* in_hw, const unsigned char* host_images);
+MSCNN_API int mscnn_net_set_input_geometry(void* net, int N, const int* org_hw);
 MSCNN_API int mscnn_net_forward(void* net, int from_layer, int to_layer); /* inclusive; to < 0 = last */
 /* mscnn_net_forward returns with the forward QUEUED on the stream: no layer waits for the device, not even BoxOutput,
  * whose data-dependent row count R stays on the device for the layers behind it (mscnn_conv_desc.dyn_n and the *_dyn

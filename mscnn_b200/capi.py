@@ -140,6 +140,17 @@ def _declare(L: C.CDLL) -> None:
     L.mscnn_detect_postprocess.restype = c_int
     L.mscnn_detect_postprocess.argtypes = [C.POINTER(DetectCfg), c_int] + [c_void_p] * 5 + [C.c_size_t] + \
         [c_void_p] * 3
+    for f in ("mscnn_detect_postprocess_sized", "mscnn_cascade_detect_postprocess_sized"):
+        getattr(L, f).restype = c_int
+        getattr(L, f).argtypes = [C.POINTER(DetectCfg), c_int] + [c_void_p] * 5 + [C.c_size_t] + [c_void_p] * 4
+    L.mscnn_detect_postprocess_packed.restype = c_int
+    L.mscnn_detect_postprocess_packed.argtypes = [C.POINTER(DetectCfg), c_int] + [c_void_p] * 5 + [C.c_size_t] + \
+        [c_void_p] * 2
+    L.mscnn_detect_postprocess_packed_sized.restype = c_int
+    L.mscnn_detect_postprocess_packed_sized.argtypes = [C.POINTER(DetectCfg), c_int] + [c_void_p] * 5 + \
+        [C.c_size_t] + [c_void_p] * 3
+    L.mscnn_detect_image_geometry.restype = c_int
+    L.mscnn_detect_image_geometry.argtypes = [c_int, c_int, c_int, c_void_p, c_void_p]
 
 
     L.mscnn_preprocess_create.restype = c_int
@@ -150,6 +161,9 @@ def _declare(L: C.CDLL) -> None:
     L.mscnn_preprocess_forward.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p]
     L.mscnn_preprocess_forward_host.restype = c_int
     L.mscnn_preprocess_forward_host.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p]
+    for f in ("mscnn_preprocess_forward_sized", "mscnn_preprocess_forward_sized_host"):
+        getattr(L, f).restype = c_int
+        getattr(L, f).argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
     L.mscnn_imresize_taps.restype = c_int
     L.mscnn_imresize_taps.argtypes = [c_int, c_int]
     L.mscnn_imresize_contributions.restype = c_int

@@ -383,6 +383,15 @@ struct DetectParams {
   float proposal_thr, ratio_h, ratio_w, org_h, org_w;
 };
 
+// Per-image geometry [ratio_h, ratio_w, org_h, org_w] of the images n0 .. n0 + count - 1 of one launch, by value in
+// the kernel parameter block (1 KB); count = 0: every image of the launch uses DetectParams' four scalars.  The MATLAB
+// drivers read each frame's size inside their loop (run_mscnn_detection.m:64-65, run_cascademscnn.m:77-80).
+constexpr int kGeomPerLaunch = 64;
+struct DetectGeom {
+  int n0, count;
+  float4 g[kGeomPerLaunch];
+};
+
 // One CTA per image: decode every ROI of the image, rank by probability (MATLAB sort 'descend'
 // is stable: ties keep the lower row first), leave boxes sorted in `sboxes` / `sscores`.
 // CASCADE = false: MS-CNN driver (run_mscnn_detection.m:75-116): prop = proposals_score [R][6],
@@ -393,7 +402,7 @@ struct DetectParams {
 //   MATLAB "+1" width convention and nothing is thresholded (det_thr = -1).
 template <bool CASCADE>
 __global__ void __launch_bounds__(kTopkThreads)
-detect_decode_sort_kernel(const DetectParams p, const float* __restrict__ prop,
+detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const float* __restrict__ prop,
                           const float* __restrict__ cls,
                           const float* __restrict__ bbox,
                           const int* __restrict__ num_rois, int Kpad, float4* __restrict__ dboxes,
@@ -401,7 +410,12 @@ detect_decode_sort_kernel(const DetectParams p, const float* __restrict__ prop,
                           int* __restrict__ counts) {
   extern __shared__ unsigned long long sk[];
   __shared__ int s_valid;
-  const int n = blockIdx.x, tid = threadIdx.x;
+  const int n = geom.n0 + blockIdx.x, tid = threadIdx.x;
+  float ratio_h = p.ratio_h, ratio_w = p.ratio_w, org_h = p.org_h, org_w = p.org_w;
+  if (geom.count) {
+    const float4 q = geom.g[blockIdx.x];
+    ratio_h = q.x; ratio_w = q.y; org_h = q.z; org_w = q.w;
+  }
   int start = 0;
   for (int m = 0; m < n; ++m) start += num_rois[2 + m];
   int cnt = num_rois[2 + n];
@@ -416,9 +430,9 @@ detect_decode_sort_kernel(const DetectParams p, const float* __restrict__ prop,
       const float qw = q[3] - q[1] + 1.f, qh = q[4] - q[2] + 1.f;  // run_cascademscnn.m:113-117
       if (qw == 0.f || qh == 0.f) continue;
       const float* b = bbox + (size_t)(start + i) * 5;
-      float x1 = b[1] / p.ratio_w, y1 = b[2] / p.ratio_h, x2 = b[3] / p.ratio_w, y2 = b[4] / p.ratio_h;  // :101-102
-      x1 = fmaxf(0.f, x1); y1 = fmaxf(0.f, y1);                                                            // :104
-      x2 = fminf(x2, p.org_w); y2 = fminf(y2, p.org_h);                                                    // :105
+      float x1 = b[1] / ratio_w, y1 = b[2] / ratio_h, x2 = b[3] / ratio_w, y2 = b[4] / ratio_h;  // :101-102
+      x1 = fmaxf(0.f, x1); y1 = fmaxf(0.f, y1);                                                    // :104
+      x2 = fminf(x2, org_w); y2 = fminf(y2, org_h);                                                // :105
       const float w = x2 - x1 + 1.f, h = y2 - y1 + 1.f;                                                    // :106
       const float prob = cls[(size_t)(start + i) * p.num_cls + id];
       if (prob != prob) continue;  // bbNms: kp = bbs(:,5) > -inf drops NaN
@@ -445,10 +459,10 @@ detect_decode_sort_kernel(const DetectParams p, const float* __restrict__ prop,
     float tx = dx * pw + cx, ty = dy * ph + cy;
     float tw = pw * exp_ref(dw), th = ph * exp_ref(dh);
     tx = tx - tw / 2.f; ty = ty - th / 2.f;
-    tx = tx / p.ratio_w; tw = tw / p.ratio_w;
-    ty = ty / p.ratio_h; th = th / p.ratio_h;
+    tx = tx / ratio_w; tw = tw / ratio_w;
+    ty = ty / ratio_h; th = th / ratio_h;
     tx = fmaxf(0.f, tx); ty = fmaxf(0.f, ty);
-    tw = fminf(tw, p.org_w - tx); th = fminf(th, p.org_h - ty);
+    tw = fminf(tw, org_w - tx); th = fminf(th, org_h - ty);
     if (prob != prob) continue;  // bbNms: kp = bbs(:,5) > -inf drops NaN
     dboxes[(size_t)n * Kpad + i] = make_float4(tx, ty, tw, th);
     sk[i] = ((unsigned long long)float_orderable(prob) << 32) | (unsigned int)(0xFFFFFFFFu - (unsigned)i);
@@ -798,16 +812,21 @@ extern "C" int mscnn_detect_workspace_bytes(const mscnn_detect_cfg* cfg, int N, 
   return MSCNN_OK;
 }
 
+// geom: HOST [N][4] = ratio_h, ratio_w, org_h, org_w per image, or NULL for the cfg's four scalars.
 static int detect_run(bool cascade, const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
                       const float* cls_pred, const float* bbox_pred, const int* num_rois, void* workspace,
-                      size_t workspace_bytes, float* dets, int* det_counts, void* stream_v, float* payload = nullptr,
-                      const mscnn::PushTargets* push = nullptr, unsigned int seq = 0, unsigned int* done_counter = nullptr) {
+                      size_t workspace_bytes, float* dets, int* det_counts, const float* geom, void* stream_v,
+                      float* payload = nullptr, const mscnn::PushTargets* push = nullptr, unsigned int seq = 0,
+                      unsigned int* done_counter = nullptr) {
   cudaStream_t stream = (cudaStream_t)stream_v;
   int Kpad;
   const int rc = det_cfg_check(cfg, N, &Kpad);
   if (rc) return rc;
   if (!proposals_score || !cls_pred || !bbox_pred || !num_rois || !workspace || (!payload && !push && (!dets || !det_counts)))
     return MSCNN_ERR_INVALID;
+  if (geom)
+    for (int k = 0; k < 4 * N; ++k)
+      if (!(geom[k] > 0.f) || geom[k] == INFINITY) return MSCNN_ERR_INVALID;
   const DetWs w = plan_det_ws(N, Kpad);
   if (workspace_bytes < w.total) return MSCNN_ERR_NOMEM;
   char* ws = (char*)workspace;
@@ -832,13 +851,25 @@ static int detect_run(bool cascade, const mscnn_detect_cfg* cfg, int N, const fl
     e = cudaFuncSetAttribute(detect_decode_sort_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)smem);
   if (e != cudaSuccess) return MSCNN_ERR_CUDA;
-  mscnn::note_launch();
-  if (cascade)
-    detect_decode_sort_kernel<true><<<N, kTopkThreads, smem, stream>>>(p, proposals_score, cls_pred, bbox_pred,
-                                                                      num_rois, Kpad, dboxes, sboxes, sscores, counts);
-  else
-    detect_decode_sort_kernel<false><<<N, kTopkThreads, smem, stream>>>(p, proposals_score, cls_pred, bbox_pred,
-                                                                       num_rois, Kpad, dboxes, sboxes, sscores, counts);
+  // one launch for the whole batch without per-image geometry, one per kGeomPerLaunch images with it
+  const int per_launch = geom ? kGeomPerLaunch : N;
+  for (int n0 = 0; n0 < N; n0 += per_launch) {
+    DetectGeom g;
+    g.n0 = n0;
+    g.count = geom ? (N - n0 < kGeomPerLaunch ? N - n0 : kGeomPerLaunch) : 0;
+    for (int i = 0; i < g.count; ++i)
+      g.g[i] = make_float4(geom[4 * (n0 + i)], geom[4 * (n0 + i) + 1], geom[4 * (n0 + i) + 2], geom[4 * (n0 + i) + 3]);
+    const int blocks = geom ? g.count : N;
+    mscnn::note_launch();
+    if (cascade)
+      detect_decode_sort_kernel<true><<<blocks, kTopkThreads, smem, stream>>>(p, g, proposals_score, cls_pred, bbox_pred,
+                                                                             num_rois, Kpad, dboxes, sboxes, sscores,
+                                                                             counts);
+    else
+      detect_decode_sort_kernel<false><<<blocks, kTopkThreads, smem, stream>>>(p, g, proposals_score, cls_pred,
+                                                                              bbox_pred, num_rois, Kpad, dboxes, sboxes,
+                                                                              sscores, counts);
+  }
   const int words = Kpad / 64;
   mscnn::note_launch();
   bbnms_mask_kernel<<<dim3(words, words, N), 64, 0, stream>>>(sboxes, counts, Kpad, words,
@@ -871,7 +902,31 @@ extern "C" int mscnn_detect_postprocess(const mscnn_detect_cfg* cfg, int N, cons
                                         void* workspace, size_t workspace_bytes, float* dets,
                                         int* det_counts, void* stream) {
   return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
-                    dets, det_counts, stream);
+                    dets, det_counts, nullptr, stream);
+}
+
+extern "C" int mscnn_detect_postprocess_sized(const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
+                                              const float* cls_pred, const float* bbox_pred, const int* num_rois,
+                                              void* workspace, size_t workspace_bytes, float* dets, int* det_counts,
+                                              const float* geom, void* stream) {
+  if (!geom) return MSCNN_ERR_INVALID;
+  return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+                    dets, det_counts, geom, stream);
+}
+
+extern "C" int mscnn_detect_image_geometry(int net_h, int net_w, int N, const int* org_hw, float* geom) {
+  if (net_h < 1 || net_w < 1 || N < 1 || !org_hw || !geom) return MSCNN_ERR_INVALID;
+  for (int n = 0; n < N; ++n)
+    if (org_hw[2 * n] < 1 || org_hw[2 * n + 1] < 1) return MSCNN_ERR_INVALID;
+  for (int n = 0; n < N; ++n) {
+    const int oh = org_hw[2 * n], ow = org_hw[2 * n + 1];
+    // ratios = [imgH imgW] ./ [orgH orgW] (run_mscnn_detection.m:65), in double, rounded once to the fp32 fields
+    geom[4 * n + 0] = (float)((double)net_h / (double)oh);
+    geom[4 * n + 1] = (float)((double)net_w / (double)ow);
+    geom[4 * n + 2] = (float)oh;
+    geom[4 * n + 3] = (float)ow;
+  }
+  return MSCNN_OK;
 }
 
 extern "C" size_t mscnn_detect_payload_floats(int N, int max_rois_per_image) {
@@ -885,16 +940,26 @@ extern "C" int mscnn_detect_postprocess_packed(const mscnn_detect_cfg* cfg, int 
                                                void* workspace, size_t workspace_bytes, float* payload, void* stream) {
   if (!payload) return MSCNN_ERR_INVALID;
   return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
-                    nullptr, nullptr, stream, payload);
+                    nullptr, nullptr, nullptr, stream, payload);
+}
+
+extern "C" int mscnn_detect_postprocess_packed_sized(const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
+                                                     const float* cls_pred, const float* bbox_pred,
+                                                     const int* num_rois, void* workspace, size_t workspace_bytes,
+                                                     float* payload, const float* geom, void* stream) {
+  if (!payload || !geom) return MSCNN_ERR_INVALID;
+  return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+                    nullptr, nullptr, geom, stream, payload);
 }
 
 // internal entry of the peer-memory exchange (xchg.cu): post-process + fused push
 int mscnn::detect_postprocess_push(const mscnn_detect_cfg* cfg, int N, const float* proposals_score, const float* cls_pred,
                                    const float* bbox_pred, const int* num_rois, void* workspace, size_t workspace_bytes,
-                                   const PushTargets* push, unsigned int seq, unsigned int* done_counter, void* stream) {
+                                   const PushTargets* push, unsigned int seq, unsigned int* done_counter,
+                                   const float* geom, void* stream) {
   if (!push || push->count < 1 || push->count > kMaxPushRanks || !done_counter) return MSCNN_ERR_INVALID;
   return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes, nullptr,
-                    nullptr, stream, nullptr, push, seq, done_counter);
+                    nullptr, geom, stream, nullptr, push, seq, done_counter);
 }
 
 extern "C" int mscnn_cascade_detect_postprocess(const mscnn_detect_cfg* cfg, int N, const float* proposals,
@@ -902,5 +967,14 @@ extern "C" int mscnn_cascade_detect_postprocess(const mscnn_detect_cfg* cfg, int
                                                 const int* num_rois, void* workspace, size_t workspace_bytes,
                                                 float* dets, int* det_counts, void* stream) {
   return detect_run(true, cfg, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes, dets,
-                    det_counts, stream);
+                    det_counts, nullptr, stream);
+}
+
+extern "C" int mscnn_cascade_detect_postprocess_sized(const mscnn_detect_cfg* cfg, int N, const float* proposals,
+                                                      const float* cls_prob, const float* output_bbox,
+                                                      const int* num_rois, void* workspace, size_t workspace_bytes,
+                                                      float* dets, int* det_counts, const float* geom, void* stream) {
+  if (!geom) return MSCNN_ERR_INVALID;
+  return detect_run(true, cfg, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes, dets,
+                    det_counts, geom, stream);
 }

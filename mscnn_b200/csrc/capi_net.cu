@@ -9,6 +9,7 @@
 #include "caffe/layers/mscnn_layers.hpp"
 #include "caffe/net.hpp"
 #include "mscnn_b200.h"
+#include "xchg.h"
 
 using caffe::Blob;
 using caffe::Caffe;
@@ -26,6 +27,11 @@ struct NetHandle {
   cudaEvent_t input_ready = nullptr, inputs_consumed = nullptr;
   bool pending_input = false, consumed_valid = false, graph_mode = false;
   int pending_consumer = -1;
+  // Original image sizes: recorded for the next forward ([N][2], empty = none), and the per-image geometry of the
+  // last forward's outputs ([N][4] = ratio_h, ratio_w, org_h, org_w; empty = the detect cfg's scalars).  The
+  // geometry belongs to the forward, so "set batch k + 1, then detect batch k" pairs each batch with its own sizes.
+  std::vector<int> next_org_hw;
+  std::vector<float> geom;
   ~NetHandle() {
     if (det_ws) cudaFree(det_ws);
     if (input_ready) cudaEventDestroy(input_ready);
@@ -39,6 +45,14 @@ int settle_pending(NetHandle* nh) {
   if (!nh->pending_input) return MSCNN_OK;
   nh->pending_input = false;
   return cudaStreamWaitEvent(Caffe::stream(), nh->input_ready, 0) == cudaSuccess ? MSCNN_OK : MSCNN_ERR_CUDA;
+}
+// Per-image geometry of the last forward for a post-process over N images: NULL when that forward had none.
+int forward_geometry(const NetHandle* nh, int N, const float** geom) {
+  *geom = nullptr;
+  if (nh->geom.empty()) return MSCNN_OK;
+  if (nh->geom.size() != (size_t)4 * N) return MSCNN_ERR_INVALID;
+  *geom = nh->geom.data();
+  return MSCNN_OK;
 }
 int fill_shape(const std::vector<int>& s, int* shape4) {
   for (size_t d = 0; d < s.size() && d < 4; ++d) shape4[d] = s[d];
@@ -213,7 +227,38 @@ int mscnn_net_set_input_images(void* h, const char* name, void* plan, int N, con
   Blob<float>* b = H(h)->net->blob_by_name(name).get();
   if (b->count() != (long)N * 3 * d.out_h * d.out_w) return MSCNN_ERR_INVALID;
   if (settle_pending(H(h)) != MSCNN_OK) return MSCNN_ERR_CUDA;
+  H(h)->next_org_hw.clear();  // these images replace any sized batch set before them
   return mscnn_preprocess_forward_host(plan, N, host_images, b->mutable_gpu_data(), Caffe::stream());
+}
+// The same for images of different original sizes (run_mscnn_detection.m:64-65 reads each frame's size): records
+// them as the geometry of the next forward.
+int mscnn_net_set_input_images_sized(void* h, const char* name, void* plan, int N, const int* in_hw,
+                                     const unsigned char* host_images) {
+  if (N < 1 || !in_hw || !host_images) return MSCNN_ERR_INVALID;
+  for (int n = 0; n < N; ++n)
+    if (in_hw[2 * n] < 1 || in_hw[2 * n + 1] < 1) return MSCNN_ERR_INVALID;
+  H(h)->net->ResolveRowsFor(name);
+  if (!H(h)->net->has_blob(name)) return MSCNN_ERR_INVALID;
+  mscnn_preprocess_desc d;
+  if (mscnn_preprocess_get_desc(plan, &d) != MSCNN_OK) return MSCNN_ERR_INVALID;
+  Blob<float>* b = H(h)->net->blob_by_name(name).get();
+  if (b->count() != (long)N * 3 * d.out_h * d.out_w) return MSCNN_ERR_INVALID;
+  if (settle_pending(H(h)) != MSCNN_OK) return MSCNN_ERR_CUDA;
+  const int rc = mscnn_preprocess_forward_sized_host(plan, N, in_hw, host_images, b->mutable_gpu_data(), Caffe::stream());
+  if (rc != MSCNN_OK) return rc;
+  H(h)->next_org_hw.assign(in_hw, in_hw + 2 * N);
+  return MSCNN_OK;
+}
+int mscnn_net_set_input_geometry(void* h, int N, const int* org_hw) {
+  if (N < 0) return MSCNN_ERR_INVALID;
+  if (N == 0 || !org_hw) {
+    H(h)->next_org_hw.clear();
+    return MSCNN_OK;
+  }
+  for (int n = 0; n < N; ++n)
+    if (org_hw[2 * n] < 1 || org_hw[2 * n + 1] < 1) return MSCNN_ERR_INVALID;
+  H(h)->next_org_hw.assign(org_hw, org_hw + 2 * N);
+  return MSCNN_OK;
 }
 int mscnn_net_set_blob_device(void* h, const char* name, const float* dev, long count) {
   H(h)->net->ResolveRowsFor(name);
@@ -248,6 +293,19 @@ int mscnn_net_forward(void* h, int from, int to) {
   Net<float>* net = nh->net.get();
   if (to < 0) to = (int)net->layers().size() - 1;
   if (from < 0 || from > to || to >= (int)net->layers().size()) return MSCNN_ERR_INVALID;
+  if (from == 0) {
+    // a forward from the first layer consumes the sizes recorded for it; the net input's H and W are the net size
+    const int n = (int)nh->next_org_hw.size() / 2;
+    std::vector<float> geom((size_t)4 * n);
+    if (n > 0) {
+      if (net->input_blobs().empty() || net->input_blobs()[0]->num() != n) return MSCNN_ERR_INVALID;
+      const Blob<float>* in = net->input_blobs()[0];
+      if (mscnn_detect_image_geometry(in->height(), in->width(), n, nh->next_org_hw.data(), geom.data()) != MSCNN_OK)
+        return MSCNN_ERR_INVALID;
+    }
+    nh->geom.swap(geom);
+    nh->next_org_hw.clear();
+  }
   if (nh->pending_input) {
     // the upload issued by mscnn_net_set_blob_async must land before the first layer runs
     if (cudaStreamWaitEvent(Caffe::stream(), nh->input_ready, 0) != cudaSuccess) return MSCNN_ERR_CUDA;
@@ -376,6 +434,13 @@ int mscnn_net_detect(void* hv, const mscnn_detect_cfg* cfg, float* dets_dev, int
     if (cudaMalloc(&h->det_ws, need) != cudaSuccess) return MSCNN_ERR_NOMEM;
     h->det_ws_bytes = need;
   }
+  const float* geom = nullptr;
+  if (forward_geometry(h, N, &geom) != MSCNN_OK) return MSCNN_ERR_INVALID;
+  if (geom)
+    return mscnn_detect_postprocess_sized(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
+                                          h->net->blob_by_name("cls_pred")->gpu_data(),
+                                          h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(),
+                                          h->det_ws, h->det_ws_bytes, dets_dev, det_counts_dev, geom, Caffe::stream());
   return mscnn_detect_postprocess(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
                                   h->net->blob_by_name("cls_pred")->gpu_data(),
                                   h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(),
@@ -407,13 +472,22 @@ int mscnn_net_detect_gather(void* hv, const mscnn_detect_cfg* cfg, void* comm, f
     if (cudaMalloc(&h->det_ws, need) != cudaSuccess) return MSCNN_ERR_NOMEM;
     h->det_ws_bytes = need;
   }
+  const float* geom = nullptr;
+  if (forward_geometry(h, N, &geom) != MSCNN_OK) return MSCNN_ERR_INVALID;
   const size_t per = mscnn_detect_payload_floats(N, cfg->max_rois_per_image);
   rc = mscnn_comm_stream_wait(comm, Caffe::stream());
   if (rc) return rc;
-  rc = mscnn_detect_postprocess_packed(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
-                                       h->net->blob_by_name("cls_pred")->gpu_data(),
-                                       h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(),
-                                       h->det_ws, h->det_ws_bytes, payload_all + (size_t)rank * per, Caffe::stream());
+  if (geom)
+    rc = mscnn_detect_postprocess_packed_sized(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
+                                               h->net->blob_by_name("cls_pred")->gpu_data(),
+                                               h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(),
+                                               h->det_ws, h->det_ws_bytes, payload_all + (size_t)rank * per, geom,
+                                               Caffe::stream());
+  else
+    rc = mscnn_detect_postprocess_packed(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
+                                         h->net->blob_by_name("cls_pred")->gpu_data(),
+                                         h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(),
+                                         h->det_ws, h->det_ws_bytes, payload_all + (size_t)rank * per, Caffe::stream());
   if (rc) return rc;
   return mscnn_comm_all_gather(comm, payload_all, per, Caffe::stream());
 }
@@ -434,10 +508,12 @@ int mscnn_net_detect_push(void* hv, const mscnn_detect_cfg* cfg, void* xchg) {
     if (cudaMalloc(&h->det_ws, need) != cudaSuccess) return MSCNN_ERR_NOMEM;
     h->det_ws_bytes = need;
   }
-  return mscnn_detect_postprocess_push(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
-                                       h->net->blob_by_name("cls_pred")->gpu_data(),
-                                       h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(), h->det_ws,
-                                       h->det_ws_bytes, xchg, Caffe::stream());
+  const float* geom = nullptr;
+  if (forward_geometry(h, N, &geom) != MSCNN_OK) return MSCNN_ERR_INVALID;
+  return mscnn::xchg_detect_push(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
+                                 h->net->blob_by_name("cls_pred")->gpu_data(),
+                                 h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(), h->det_ws,
+                                 h->det_ws_bytes, xchg, geom, Caffe::stream());
 }
 int mscnn_net_detect_cascade(void* hv, const mscnn_detect_cfg* cfg, const char* proposals_blob,
                              const char* cls_prob_blob, const char* output_bbox_blob, float* dets_dev,
@@ -463,6 +539,14 @@ int mscnn_net_detect_cascade(void* hv, const mscnn_detect_cfg* cfg, const char* 
     h->det_ws_bytes = need;
   }
   if (h->net->blob_by_name(cls_prob_blob)->channels() != cfg->num_cls) return MSCNN_ERR_INVALID;
+  const float* geom = nullptr;
+  if (forward_geometry(h, N, &geom) != MSCNN_OK) return MSCNN_ERR_INVALID;
+  if (geom)
+    return mscnn_cascade_detect_postprocess_sized(cfg, N, h->net->blob_by_name(proposals_blob)->gpu_data(),
+                                                  h->net->blob_by_name(cls_prob_blob)->gpu_data(),
+                                                  h->net->blob_by_name(output_bbox_blob)->gpu_data(),
+                                                  h->box->num_out_device(), h->det_ws, h->det_ws_bytes, dets_dev,
+                                                  det_counts_dev, geom, Caffe::stream());
   return mscnn_cascade_detect_postprocess(cfg, N, h->net->blob_by_name(proposals_blob)->gpu_data(),
                                           h->net->blob_by_name(cls_prob_blob)->gpu_data(),
                                           h->net->blob_by_name(output_bbox_blob)->gpu_data(),

@@ -97,16 +97,39 @@ struct DevTable {
   int* idx = nullptr;
 };
 
+// The tap tables of one input size (the output size is the plan's), uploaded once.
+struct SizeTables {
+  int in_h, in_w;
+  int first_dim;  // 0: height pass first, 1: width pass first (ascending scale, ties -> height)
+  DevTable th, tw;
+};
+
 }  // namespace
 
 struct PreprocessPlan {
-  mscnn_preprocess_desc d;
-  int first_dim;  // 0: height pass first, 1: width pass first (ascending scale, ties -> height)
-  DevTable th, tw;
-  unsigned char* mid = nullptr;  // intermediate image after the first pass
+  mscnn_preprocess_desc d;         // in_h / in_w = sizes[0], the size the plan was created for
+  std::vector<SizeTables> sizes;   // one entry per distinct input size seen so far
+  unsigned char* mid = nullptr;    // intermediate images after the first pass
   size_t mid_cap = 0;
-  unsigned char* stage = nullptr;  // device copy of host images (mscnn_preprocess_forward_host)
+  unsigned char* stage = nullptr;  // device copy of host images (mscnn_preprocess_forward*_host)
   size_t stage_cap = 0;
+};
+
+// One image of a batch as both passes see it.  The descriptors of a launch travel by value in the kernel parameter
+// block, so a later call can never overwrite them before the kernels have read them.
+struct ImageDesc {
+  size_t src, mid;  // byte offsets of the image in the input batch and of its intermediate image
+  int in_h, in_w;   // original size
+  int mid_h, mid_w; // size after the first pass
+  int first_dim;    // the first pass resizes along this dimension (0: height), the second along the other
+  DevTable t1, t2;  // tap tables of the first and the second pass
+};
+
+// 32 descriptors = 2.8 KB of parameters; larger batches take several launches of both kernels.
+constexpr int kImagesPerLaunch = 32;
+struct ImageBatch {
+  int n0;  // batch index of d[0]
+  ImageDesc d[kImagesPerLaunch];
 };
 
 // uint8 conversion of an fp64 accumulator: saturate, round half away from zero.
@@ -115,23 +138,25 @@ __device__ __forceinline__ double round_u8(double v) {
   return round(v);
 }
 
-// First pass: resize along one dimension, uint8 [N][H][W][3] -> uint8.  One thread per output byte
-// (the three channels of a pixel are adjacent bytes, so a warp writes 32 consecutive bytes and reads
-// `taps` rows or pixel neighbourhoods that its lanes share).
-//   along = 0: out[n][y][x][c] = sum_k w[y][k] * in[n][idx[y][k]][x][c]   (out_h x in_w)
-//   along = 1: out[n][y][x][c] = sum_k w[x][k] * in[n][y][idx[x][k]][c]   (in_h x out_w)
-__global__ void imresize_pass_u8_kernel(const unsigned char* __restrict__ in, unsigned char* __restrict__ out,
-                                        int N, int in_h, int in_w, int out_h, int out_w, int along, int taps,
-                                        const double* __restrict__ w, const int* __restrict__ idx) {
-  const size_t total = (size_t)N * out_h * out_w * 3;
+// First pass: resize image d[blockIdx.y] of the launch along one dimension, uint8 [h][w][3] -> uint8 [mid_h][mid_w][3].
+// One thread per output byte (the three channels of a pixel are adjacent bytes, so a warp writes 32 consecutive bytes
+// and reads `taps` rows or pixel neighbourhoods that its lanes share).
+//   along = 0: out[y][x][c] = sum_k w[y][k] * in[idx[y][k]][x][c]   (out_h x in_w)
+//   along = 1: out[y][x][c] = sum_k w[x][k] * in[y][idx[x][k]][c]   (in_h x out_w)
+__global__ void imresize_pass_u8_kernel(const unsigned char* __restrict__ images, unsigned char* __restrict__ mid,
+                                        const ImageBatch b) {
+  const ImageDesc& D = b.d[blockIdx.y];
+  const int in_w = D.in_w, out_w = D.mid_w, along = D.first_dim, taps = D.t1.taps;
+  const double* __restrict__ w = D.t1.w;
+  const int* __restrict__ idx = D.t1.idx;
+  const unsigned char* img = images + D.src;
+  unsigned char* out = mid + D.mid;
+  const size_t total = (size_t)D.mid_h * out_w * 3;
   for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(e % 3);
-    size_t p = e / 3;
+    const size_t p = e / 3;
     const int x = (int)(p % out_w);
-    p /= out_w;
-    const int y = (int)(p % out_h);
-    const int n = (int)(p / out_h);
-    const unsigned char* img = in + (size_t)n * in_h * in_w * 3;
+    const int y = (int)(p / out_w);
     const int o = along == 0 ? y : x;
     const double* wr = w + (size_t)o * taps;
     const int* ir = idx + (size_t)o * taps;
@@ -145,20 +170,21 @@ __global__ void imresize_pass_u8_kernel(const unsigned char* __restrict__ in, un
   }
 }
 
-// Second pass + channel swap + mean subtraction + HWC -> CHW.  One thread per output pixel; a warp
-// writes 32 consecutive floats of each of the three output planes.
-__global__ void imresize_pass_to_blob_kernel(const unsigned char* __restrict__ in, float* __restrict__ out, int N,
-                                             int in_h, int in_w, int out_h, int out_w, int along, int taps,
-                                             const double* __restrict__ w, const int* __restrict__ idx,
-                                             float mean0, float mean1, float mean2, int swap_rb) {
-  const size_t total = (size_t)N * out_h * out_w;
+// Second pass + channel swap + mean subtraction + HWC -> CHW, into slot b.n0 + blockIdx.y of the blob.  One thread
+// per output pixel; a warp writes 32 consecutive floats of each of the three output planes.
+__global__ void imresize_pass_to_blob_kernel(const unsigned char* __restrict__ mid, float* __restrict__ data,
+                                             int out_h, int out_w, const ImageBatch b, float mean0, float mean1,
+                                             float mean2, int swap_rb) {
+  const ImageDesc& D = b.d[blockIdx.y];
+  const int in_w = D.mid_w, along = 1 - D.first_dim, taps = D.t2.taps;
+  const double* __restrict__ w = D.t2.w;
+  const int* __restrict__ idx = D.t2.idx;
+  const unsigned char* img = mid + D.mid;
   const size_t plane = (size_t)out_h * out_w;
-  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+  float* out = data + (size_t)(b.n0 + blockIdx.y) * 3 * plane;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < plane; e += (size_t)gridDim.x * blockDim.x) {
     const int x = (int)(e % out_w);
-    size_t p = e / out_w;
-    const int y = (int)(p % out_h);
-    const int n = (int)(p / out_h);
-    const unsigned char* img = in + (size_t)n * in_h * in_w * 3;
+    const int y = (int)(e / out_w);
     const int o = along == 0 ? y : x;
     const double* wr = w + (size_t)o * taps;
     const int* ir = idx + (size_t)o * taps;
@@ -172,7 +198,7 @@ __global__ void imresize_pass_to_blob_kernel(const unsigned char* __restrict__ i
       a2 = __dadd_rn(a2, __dmul_rn(wk, (double)q[2]));
     }
     const float v0 = (float)round_u8(a0), v1 = (float)round_u8(a1), v2 = (float)round_u8(a2);
-    float* dst = out + (size_t)n * 3 * plane + (size_t)y * out_w + x;
+    float* dst = out + (size_t)y * out_w + x;
     // output channel order after test_image(:,:,[3 2 1]): plane 0 = input channel 2 when swapping
     dst[0] = (swap_rb ? v2 : v0) - mean0;
     dst[plane] = v1 - mean1;
@@ -201,6 +227,106 @@ static int grow(unsigned char** buf, size_t* cap, size_t need) {
   if (cudaMalloc(buf, need) != cudaSuccess) return MSCNN_ERR_NOMEM;
   *cap = need;
   return MSCNN_OK;
+}
+
+static void free_tables(SizeTables* s) {
+  cudaFree(s->th.w);
+  cudaFree(s->th.idx);
+  cudaFree(s->tw.w);
+  cudaFree(s->tw.idx);
+}
+
+// Index of the tap tables of input size (in_h, in_w) in the plan's cache; built in fp64 and uploaded on first use.
+static int tables_for(PreprocessPlan* p, int in_h, int in_w, int* index) {
+  for (size_t i = 0; i < p->sizes.size(); ++i)
+    if (p->sizes[i].in_h == in_h && p->sizes[i].in_w == in_w) {
+      *index = (int)i;
+      return MSCNN_OK;
+    }
+  SizeTables s;
+  s.in_h = in_h;
+  s.in_w = in_w;
+  const double sh = (double)p->d.out_h / in_h, sw = (double)p->d.out_w / in_w;
+  s.first_dim = sw < sh ? 1 : 0;  // ascending scale, stable: height first on ties (imresize.m sort(scale))
+  int rc = upload(contributions(in_h, p->d.out_h), &s.th);
+  if (rc == MSCNN_OK) rc = upload(contributions(in_w, p->d.out_w), &s.tw);
+  if (rc != MSCNN_OK) {
+    free_tables(&s);
+    return rc;
+  }
+  p->sizes.push_back(s);
+  *index = (int)p->sizes.size() - 1;
+  return MSCNN_OK;
+}
+
+static bool sizes_valid(int N, const int* in_hw) {
+  if (N < 1 || !in_hw) return false;
+  for (int n = 0; n < N; ++n)
+    if (in_hw[2 * n] < 1 || in_hw[2 * n + 1] < 1) return false;
+  return true;
+}
+
+static std::vector<int> uniform_sizes(const PreprocessPlan* p, int N) {
+  std::vector<int> hw((size_t)2 * N);
+  for (int n = 0; n < N; ++n) {
+    hw[2 * n] = p->d.in_h;
+    hw[2 * n + 1] = p->d.in_w;
+  }
+  return hw;
+}
+
+static unsigned grid_x(size_t work, unsigned cap) {
+  const size_t blocks = (work + 255) / 256;
+  return (unsigned)(blocks > cap ? cap : blocks);
+}
+
+// Images packed back to back in batch order (image n starts at byte sum_{m<n} h_m w_m 3) -> data [N][3][out_h][out_w].
+// Both passes cover up to kImagesPerLaunch images per launch, image = blockIdx.y.
+static int forward_sized(PreprocessPlan* p, int N, const int* in_hw, const unsigned char* images, float* data,
+                         cudaStream_t st) {
+  const mscnn_preprocess_desc& d = p->d;
+  std::vector<ImageDesc> desc(N);
+  size_t src = 0, mid = 0;
+  for (int n = 0; n < N; ++n) {
+    int t;
+    const int rc = tables_for(p, in_hw[2 * n], in_hw[2 * n + 1], &t);
+    if (rc != MSCNN_OK) return rc;
+    const SizeTables& s = p->sizes[t];
+    ImageDesc& D = desc[n];
+    D.src = src;
+    D.mid = mid;
+    D.in_h = s.in_h;
+    D.in_w = s.in_w;
+    D.first_dim = s.first_dim;
+    D.mid_h = s.first_dim == 0 ? d.out_h : s.in_h;
+    D.mid_w = s.first_dim == 0 ? s.in_w : d.out_w;
+    D.t1 = s.first_dim == 0 ? s.th : s.tw;
+    D.t2 = s.first_dim == 0 ? s.tw : s.th;
+    src += (size_t)s.in_h * s.in_w * 3;
+    mid += (size_t)D.mid_h * D.mid_w * 3;
+  }
+  const int rc = grow(&p->mid, &p->mid_cap, mid);
+  if (rc != MSCNN_OK) return rc;
+  const size_t px = (size_t)d.out_h * d.out_w;
+  for (int n0 = 0; n0 < N; n0 += kImagesPerLaunch) {
+    const int count = N - n0 < kImagesPerLaunch ? N - n0 : kImagesPerLaunch;
+    ImageBatch b;
+    b.n0 = n0;
+    size_t mid_max = 0;
+    for (int i = 0; i < count; ++i) {
+      b.d[i] = desc[n0 + i];
+      const size_t m = (size_t)b.d[i].mid_h * b.d[i].mid_w * 3;
+      if (m > mid_max) mid_max = m;
+    }
+    const unsigned cap = 132u * 64 / count;  // at most 132 x 64 blocks per launch, as before
+    imresize_pass_u8_kernel<<<dim3(grid_x(mid_max, cap), count), 256, 0, st>>>(images, p->mid, b);
+    note_launch();
+    imresize_pass_to_blob_kernel<<<dim3(grid_x(px, cap), count), 256, 0, st>>>(p->mid, data, d.out_h, d.out_w, b,
+                                                                               d.mean[0], d.mean[1], d.mean[2],
+                                                                               d.swap_rb);
+    note_launch();
+  }
+  return cudaPeekAtLastError() == cudaSuccess ? MSCNN_OK : MSCNN_ERR_CUDA;
 }
 
 }  // namespace mscnn
@@ -246,10 +372,8 @@ int mscnn_preprocess_create(const mscnn_preprocess_desc* d, void** plan) {
   if (!d || !plan || d->in_h < 1 || d->in_w < 1 || d->out_h < 1 || d->out_w < 1) return MSCNN_ERR_INVALID;
   PreprocessPlan* p = new PreprocessPlan();
   p->d = *d;
-  const double sh = (double)d->out_h / d->in_h, sw = (double)d->out_w / d->in_w;
-  p->first_dim = sw < sh ? 1 : 0;  // ascending scale, stable: height first on ties (imresize.m sort(scale))
-  int rc = upload(contributions(d->in_h, d->out_h), &p->th);
-  if (rc == MSCNN_OK) rc = upload(contributions(d->in_w, d->out_w), &p->tw);
+  int first;
+  const int rc = tables_for(p, d->in_h, d->in_w, &first);
   if (rc != MSCNN_OK) {
     mscnn_preprocess_destroy(p);
     return rc;
@@ -267,56 +391,44 @@ int mscnn_preprocess_get_desc(void* plan, mscnn_preprocess_desc* d) {
 int mscnn_preprocess_destroy(void* plan) {
   PreprocessPlan* p = static_cast<PreprocessPlan*>(plan);
   if (!p) return MSCNN_OK;
-  cudaFree(p->th.w);
-  cudaFree(p->th.idx);
-  cudaFree(p->tw.w);
-  cudaFree(p->tw.idx);
+  for (SizeTables& s : p->sizes) free_tables(&s);
   cudaFree(p->mid);
   cudaFree(p->stage);
   delete p;
   return MSCNN_OK;
 }
 
+int mscnn_preprocess_forward_sized(void* plan, int N, const int* in_hw, const unsigned char* images, float* data,
+                                   void* stream) {
+  PreprocessPlan* p = static_cast<PreprocessPlan*>(plan);
+  if (!p || !sizes_valid(N, in_hw) || !images || !data) return MSCNN_ERR_INVALID;
+  return forward_sized(p, N, in_hw, images, data, (cudaStream_t)stream);
+}
+
+int mscnn_preprocess_forward_sized_host(void* plan, int N, const int* in_hw, const unsigned char* host_images,
+                                        float* data, void* stream) {
+  PreprocessPlan* p = static_cast<PreprocessPlan*>(plan);
+  if (!p || !sizes_valid(N, in_hw) || !host_images || !data) return MSCNN_ERR_INVALID;
+  size_t bytes = 0;
+  for (int n = 0; n < N; ++n) bytes += (size_t)in_hw[2 * n] * in_hw[2 * n + 1] * 3;
+  int rc = grow(&p->stage, &p->stage_cap, bytes);
+  if (rc != MSCNN_OK) return rc;
+  if (cudaMemcpyAsync(p->stage, host_images, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream) != cudaSuccess)
+    return MSCNN_ERR_CUDA;
+  return forward_sized(p, N, in_hw, p->stage, data, (cudaStream_t)stream);
+}
+
+// The uniform batch: every image has the plan's own input size.
 int mscnn_preprocess_forward(void* plan, int N, const unsigned char* images, float* data, void* stream) {
   PreprocessPlan* p = static_cast<PreprocessPlan*>(plan);
   if (!p || N < 1 || !images || !data) return MSCNN_ERR_INVALID;
-  const mscnn_preprocess_desc& d = p->d;
-  cudaStream_t st = (cudaStream_t)stream;
-  // sizes after the first pass
-  const int mid_h = p->first_dim == 0 ? d.out_h : d.in_h;
-  const int mid_w = p->first_dim == 0 ? d.in_w : d.out_w;
-  const size_t mid_bytes = (size_t)N * mid_h * mid_w * 3;
-  int rc = grow(&p->mid, &p->mid_cap, mid_bytes);
-  if (rc != MSCNN_OK) return rc;
-  const int threads = 256;
-  const DevTable& t1 = p->first_dim == 0 ? p->th : p->tw;
-  const DevTable& t2 = p->first_dim == 0 ? p->tw : p->th;
-  {
-    const size_t blocks = (mid_bytes + threads - 1) / threads;
-    imresize_pass_u8_kernel<<<(unsigned)(blocks > 132u * 64 ? 132u * 64 : blocks), threads, 0, st>>>(
-        images, p->mid, N, d.in_h, d.in_w, mid_h, mid_w, p->first_dim, t1.taps, t1.w, t1.idx);
-    note_launch();
-  }
-  {
-    const size_t px = (size_t)N * d.out_h * d.out_w;
-    const size_t blocks = (px + threads - 1) / threads;
-    imresize_pass_to_blob_kernel<<<(unsigned)(blocks > 132u * 64 ? 132u * 64 : blocks), threads, 0, st>>>(
-        p->mid, data, N, mid_h, mid_w, d.out_h, d.out_w, 1 - p->first_dim, t2.taps, t2.w, t2.idx, d.mean[0],
-        d.mean[1], d.mean[2], d.swap_rb);
-    note_launch();
-  }
-  return cudaPeekAtLastError() == cudaSuccess ? MSCNN_OK : MSCNN_ERR_CUDA;
+  return mscnn_preprocess_forward_sized(plan, N, uniform_sizes(p, N).data(), images, data, stream);
 }
 
 int mscnn_preprocess_forward_host(void* plan, int N, const unsigned char* host_images, float* data, void* stream) {
   PreprocessPlan* p = static_cast<PreprocessPlan*>(plan);
   if (!p || N < 1 || !host_images || !data) return MSCNN_ERR_INVALID;
-  const size_t bytes = (size_t)N * p->d.in_h * p->d.in_w * 3;
-  int rc = grow(&p->stage, &p->stage_cap, bytes);
-  if (rc != MSCNN_OK) return rc;
-  if (cudaMemcpyAsync(p->stage, host_images, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream) != cudaSuccess)
-    return MSCNN_ERR_CUDA;
-  return mscnn_preprocess_forward(plan, N, p->stage, data, stream);
+  return mscnn_preprocess_forward_sized_host(plan, N, uniform_sizes(p, N).data(), host_images, data, stream);
 }
 
 }  // extern "C"

@@ -200,6 +200,15 @@ int mscnn_xchg_wait(void* xv, void* stream) {
 int mscnn_detect_postprocess_push(const mscnn_detect_cfg* cfg, int N, const float* proposals_score, const float* cls_pred,
                                   const float* bbox_pred, const int* num_rois, void* workspace, size_t workspace_bytes,
                                   void* xv, void* stream) {
+  return mscnn::xchg_detect_push(cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes, xv,
+                                 nullptr, stream);
+}
+
+}  // extern "C"
+
+int mscnn::xchg_detect_push(const mscnn_detect_cfg* cfg, int N, const float* proposals_score, const float* cls_pred,
+                            const float* bbox_pred, const int* num_rois, void* workspace, size_t workspace_bytes,
+                            void* xv, const float* geom, void* stream) {
   Xchg* x = static_cast<Xchg*>(xv);
   if (!x || !cfg) return MSCNN_ERR_INVALID;
   if (mscnn_detect_payload_floats(N, cfg->max_rois_per_image) != x->per) return MSCNN_ERR_INVALID;
@@ -220,9 +229,7 @@ int mscnn_detect_postprocess_push(const mscnn_detect_cfg* cfg, int N, const floa
   }
   unsigned int* counter = reinterpret_cast<unsigned int*>(x->local + (size_t)x->gens * x->gen_bytes);
   const int rc = mscnn::detect_postprocess_push(cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace,
-                                                workspace_bytes, &t, seq, counter, stream);
+                                                workspace_bytes, &t, seq, counter, geom, stream);
   if (rc == MSCNN_OK) x->seq = seq;
   return rc;
 }
-
-}  // extern "C"

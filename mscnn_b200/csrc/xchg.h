@@ -19,6 +19,13 @@ struct PushTargets {
 
 int detect_postprocess_push(const mscnn_detect_cfg* cfg, int N, const float* proposals_score, const float* cls_pred,
                             const float* bbox_pred, const int* num_rois, void* workspace, size_t workspace_bytes,
-                            const PushTargets* push, unsigned int seq, unsigned int* done_counter, void* stream);
+                            const PushTargets* push, unsigned int seq, unsigned int* done_counter, const float* geom,
+                            void* stream);
+
+// mscnn_detect_postprocess_push with optional per-image geometry (HOST [N][4], NULL = the cfg's scalars): the Net
+// facade's entry.
+int xchg_detect_push(const mscnn_detect_cfg* cfg, int N, const float* proposals_score, const float* cls_pred,
+                     const float* bbox_pred, const int* num_rois, void* workspace, size_t workspace_bytes, void* xchg,
+                     const float* geom, void* stream);
 
 }  // namespace mscnn

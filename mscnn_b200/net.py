@@ -43,6 +43,8 @@ def _declare(L):
     L.mscnn_net_reshape_blob.argtypes = [C.c_void_p, C.c_char_p] + [C.c_int] * 4
     L.mscnn_net_set_blob.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long]
     L.mscnn_net_set_input_images.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_void_p]
+    L.mscnn_net_set_input_images_sized.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    L.mscnn_net_set_input_geometry.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.mscnn_net_set_blob_async.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long]
     L.mscnn_net_set_blob_device.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long]
     L.mscnn_net_get_blob.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long]
@@ -75,10 +77,20 @@ def set_precision(mode: str) -> None:
     capi.check(L.mscnn_set_precision(1 if mode.lower() == "bf16" else 0), "set_precision")
 
 
+_net_stream_ptr = None   # the stream the nets of this process run on (mscnn_set_stream); None = the default stream
+
+
 def set_stream(stream_ptr: int | None) -> None:
+    global _net_stream_ptr
     L = capi.lib()
     _declare(L)
     capi.check(L.mscnn_set_stream(stream_ptr), "set_stream")
+    _net_stream_ptr = stream_ptr
+
+
+def _net_stream():
+    import torch
+    return torch.cuda.ExternalStream(_net_stream_ptr) if _net_stream_ptr else torch.cuda.default_stream()
 
 
 def set_device(device: int) -> None:
@@ -204,13 +216,33 @@ class Net:
 
     def set_input_images(self, name: str, pre, images) -> None:
         """uint8 host images [N][h][w][3] (numpy or pinned CPU tensor) -> device pre-processing (`pre` = an
-        ops.Preprocess plan) -> the input blob; the MATLAB code before net.forward, run_mscnn_detection.m:64-69."""
-        n = images.shape[0]
+        ops.Preprocess plan) -> the input blob; the MATLAB code before net.forward, run_mscnn_detection.m:64-69.
+        A list of host uint8 [h][w][3] frames may mix original sizes: their sizes become the geometry of the next
+        forward, whose detections are then rescaled and clipped per frame (run_mscnn_detection.m:64-65, 111-116)."""
+        from . import ops
+        sized = isinstance(images, (list, tuple))
+        hw = ops.image_sizes(images) if sized else None
+        n = len(hw) if sized else images.shape[0]
         shp = (n, 3, *pre.out_hw)
         if self.blob_shape(name) != shp:
             capi.check(self._L.mscnn_net_reshape_blob(self._h, name.encode(), *shp), "reshape_blob")
-        capi.check(self._L.mscnn_net_set_input_images(self._h, name.encode(), pre.handle, n, capi.ptr(images)),
-                   "set_input_images")
+        if not sized:
+            capi.check(self._L.mscnn_net_set_input_images(self._h, name.encode(), pre.handle, n, capi.ptr(images)),
+                       "set_input_images")
+            return
+        packed = pre.pack_host(images)
+        capi.check(self._L.mscnn_net_set_input_images_sized(self._h, name.encode(), pre.handle, n, hw.ctypes.data,
+                                                            capi.ptr(packed)), "set_input_images_sized")
+        pre.host_copy_issued(_net_stream())
+
+    def set_input_geometry(self, org_hw_list) -> None:
+        """Original (h, w) of each image the NEXT forward consumes, for inputs resized by the caller and set with
+        set_input*; None or [] clears them.  The detections of that forward are rescaled and clipped per image."""
+        if not org_hw_list:
+            capi.check(self._L.mscnn_net_set_input_geometry(self._h, 0, None), "set_input_geometry")
+            return
+        hw = np.ascontiguousarray(org_hw_list, dtype=np.int32).reshape(-1, 2)
+        capi.check(self._L.mscnn_net_set_input_geometry(self._h, len(hw), hw.ctypes.data), "set_input_geometry")
 
     def forward_only(self, start: str | None = None, end: str | None = None) -> None:
         i0 = self.layer_names.index(start) if start else 0
@@ -288,3 +320,14 @@ def kitti_detect_cfg(net_h: int, net_w: int, max_rois: int = 2000, num_cls: int 
     cfg.org_h, cfg.org_w = float(oh), float(ow)
     cfg.max_rois_per_image = max_rois
     return cfg
+
+
+def image_geometry(net_hw: tuple[int, int], org_hw_list) -> np.ndarray:
+    """float32 [N][4] = ratio_h, ratio_w, org_h, org_w per image (mscnn_detect_image_geometry, host only): the
+    `geometry=` of ops.detect_postprocess, with the same values kitti_detect_cfg(*net_hw, org_hw=...) stores."""
+    L = capi.lib()
+    hw = np.ascontiguousarray(org_hw_list, dtype=np.int32).reshape(-1, 2)
+    out = np.zeros((len(hw), 4), dtype=np.float32)
+    capi.check(L.mscnn_detect_image_geometry(int(net_hw[0]), int(net_hw[1]), len(hw), hw.ctypes.data, out.ctypes.data),
+               "detect_image_geometry")
+    return out

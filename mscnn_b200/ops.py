@@ -275,7 +275,15 @@ def eltwise_forward(bottoms: list[torch.Tensor], op: int, coeffs=None) -> torch.
     return y
 
 
-def cascade_detect_postprocess(cfg: capi.DetectCfg, n: int, proposals, cls_prob, output_bbox, num_out):
+def _geometry(geometry, n: int) -> np.ndarray:
+    """Host float32 [n][4] = ratio_h, ratio_w, org_h, org_w per image (see mscnn_detect_image_geometry)."""
+    g = np.ascontiguousarray(geometry, dtype=np.float32)
+    assert g.shape == (n, 4), (g.shape, n)
+    return g
+
+
+def cascade_detect_postprocess(cfg: capi.DetectCfg, n: int, proposals, cls_prob, output_bbox, num_out, geometry=None):
+    """geometry: None (the cfg's ratio_* / org_*) or per-image [n][4] = ratio_h, ratio_w, org_h, org_w."""
     import ctypes as C
     dev = proposals.device
     nbytes = C.c_size_t(0)
@@ -283,14 +291,19 @@ def cascade_detect_postprocess(cfg: capi.DetectCfg, n: int, proposals, cls_prob,
     ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
     dets = torch.zeros((n, cfg.max_rois_per_image, 5), dtype=torch.float32, device=dev)
     counts = torch.zeros(n, dtype=torch.int32, device=dev)
-    capi.check(capi.lib().mscnn_cascade_detect_postprocess(cfg, n, capi.ptr(proposals), capi.ptr(cls_prob),
-                                                           capi.ptr(output_bbox), capi.ptr(num_out), capi.ptr(ws),
-                                                           nbytes.value, capi.ptr(dets), capi.ptr(counts), _stream()),
-               "cascade_detect_postprocess")
+    args = (cfg, n, capi.ptr(proposals), capi.ptr(cls_prob), capi.ptr(output_bbox), capi.ptr(num_out), capi.ptr(ws),
+            nbytes.value, capi.ptr(dets), capi.ptr(counts))
+    if geometry is None:
+        capi.check(capi.lib().mscnn_cascade_detect_postprocess(*args, _stream()), "cascade_detect_postprocess")
+    else:
+        g = _geometry(geometry, n)
+        capi.check(capi.lib().mscnn_cascade_detect_postprocess_sized(*args, g.ctypes.data, _stream()),
+                   "cascade_detect_postprocess_sized")
     return dets, counts
 
 
-def detect_postprocess(cfg: capi.DetectCfg, n: int, proposals_score, cls_pred, bbox_pred, num_out):
+def detect_postprocess(cfg: capi.DetectCfg, n: int, proposals_score, cls_pred, bbox_pred, num_out, geometry=None):
+    """geometry: None (the cfg's ratio_* / org_*) or per-image [n][4] = ratio_h, ratio_w, org_h, org_w."""
     import ctypes as C
     dev = proposals_score.device
     nbytes = C.c_size_t(0)
@@ -298,10 +311,14 @@ def detect_postprocess(cfg: capi.DetectCfg, n: int, proposals_score, cls_pred, b
     ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
     dets = torch.zeros((n, cfg.max_rois_per_image, 5), dtype=torch.float32, device=dev)
     counts = torch.zeros(n, dtype=torch.int32, device=dev)
-    capi.check(capi.lib().mscnn_detect_postprocess(cfg, n, capi.ptr(proposals_score), capi.ptr(cls_pred),
-                                                   capi.ptr(bbox_pred), capi.ptr(num_out), capi.ptr(ws),
-                                                   nbytes.value, capi.ptr(dets), capi.ptr(counts), _stream()),
-               "detect_postprocess")
+    args = (cfg, n, capi.ptr(proposals_score), capi.ptr(cls_pred), capi.ptr(bbox_pred), capi.ptr(num_out),
+            capi.ptr(ws), nbytes.value, capi.ptr(dets), capi.ptr(counts))
+    if geometry is None:
+        capi.check(capi.lib().mscnn_detect_postprocess(*args, _stream()), "detect_postprocess")
+    else:
+        g = _geometry(geometry, n)
+        capi.check(capi.lib().mscnn_detect_postprocess_sized(*args, g.ctypes.data, _stream()),
+                   "detect_postprocess_sized")
     return dets, counts
 
 
@@ -342,8 +359,8 @@ def widerface_net_size(org_h: int, org_w: int, img_h: int = 0, img_w: int = 0, m
 
 
 class Preprocess:
-    """imresize + BGR + mean subtraction + CHW on the device for images of one size
-    (examples/kitti_car/run_mscnn_detection.m:64-69)."""
+    """imresize + BGR + mean subtraction + CHW on the device (examples/kitti_car/run_mscnn_detection.m:64-69), into
+    one output size.  ``in_hw`` is the size of an array batch; a list of images may mix any sizes."""
 
     def __init__(self, in_hw, out_hw, mean=(104.0, 117.0, 123.0), swap_rb=True):
         import ctypes as C
@@ -351,6 +368,8 @@ class Preprocess:
         h = C.c_void_p()
         capi.check(capi.lib().mscnn_preprocess_create(C.byref(d), C.byref(h)), "preprocess_create")
         self.handle, self.in_hw, self.out_hw = h, tuple(in_hw), tuple(out_hw)
+        self._pinned = None    # host images of a list, packed back to back for the one H2D copy
+        self._copied = None    # event behind the last H2D copy from _pinned
 
     def __del__(self):
         if getattr(self, "handle", None):
@@ -358,7 +377,10 @@ class Preprocess:
             self.handle = None
 
     def __call__(self, images, out: torch.Tensor | None = None) -> torch.Tensor:
-        """images: uint8 [N][h][w][3], a torch.cuda tensor, or a host numpy array / CPU tensor (H2D inside)."""
+        """images: uint8 [N][h][w][3], a torch.cuda tensor, or a host numpy array / CPU tensor (H2D inside); or a
+        list of uint8 [h][w][3] images of any sizes, all torch.cuda tensors or all on the host."""
+        if isinstance(images, (list, tuple)):
+            return self._call_sized(images, out)
         n = images.shape[0]
         assert tuple(images.shape[1:]) == (*self.in_hw, 3) and images.dtype in (torch.uint8, np.uint8)
         if out is None:
@@ -372,3 +394,51 @@ class Preprocess:
             capi.check(L.mscnn_preprocess_forward_host(self.handle, n, capi.ptr(images), capi.ptr(out), _stream()),
                        "preprocess_forward_host")
         return out
+
+    def _call_sized(self, images, out):
+        n, hw = len(images), image_sizes(images)
+        if out is None:
+            out = torch.empty((n, 3, *self.out_hw), dtype=torch.float32, device="cuda")
+        L = capi.lib()
+        on_device = [isinstance(im, torch.Tensor) and im.is_cuda for im in images]
+        if all(on_device):
+            packed = torch.cat([im.reshape(-1) for im in images])
+            capi.check(L.mscnn_preprocess_forward_sized(self.handle, n, hw.ctypes.data, capi.ptr(packed),
+                                                        capi.ptr(out), _stream()), "preprocess_forward_sized")
+        elif not any(on_device):
+            packed = self.pack_host(images)
+            capi.check(L.mscnn_preprocess_forward_sized_host(self.handle, n, hw.ctypes.data, capi.ptr(packed),
+                                                             capi.ptr(out), _stream()),
+                       "preprocess_forward_sized_host")
+            self.host_copy_issued(torch.cuda.current_stream())
+        else:
+            raise ValueError("a list of images must be all on the device or all on the host")
+        return out
+
+    def pack_host(self, images) -> torch.Tensor:
+        """Host images back to back in one pinned buffer owned by the plan, so that their H2D copy is asynchronous.
+        The buffer is refilled only once the copy issued from it last time has run (`host_copy_issued`)."""
+        total = sum(int(np.prod(im.shape)) for im in images)
+        if self._copied is not None:
+            self._copied.synchronize()
+        if self._pinned is None or self._pinned.numel() < total:
+            self._pinned = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+        off = 0
+        for im in images:
+            t = torch.as_tensor(im).reshape(-1)
+            self._pinned[off:off + t.numel()].copy_(t)
+            off += t.numel()
+        return self._pinned
+
+    def host_copy_issued(self, stream: torch.cuda.Stream) -> None:
+        """Mark the H2D copy from the packed buffer, just issued on `stream`."""
+        self._copied = torch.cuda.Event()
+        self._copied.record(stream)
+
+
+def image_sizes(images) -> np.ndarray:
+    """int32 [N][2] = h, w of a list of uint8 [h][w][3] images."""
+    assert len(images) >= 1
+    for im in images:
+        assert len(im.shape) == 3 and im.shape[2] == 3 and im.dtype in (torch.uint8, np.uint8), (im.shape, im.dtype)
+    return np.ascontiguousarray([im.shape[:2] for im in images], dtype=np.int32)
