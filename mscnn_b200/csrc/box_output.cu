@@ -113,6 +113,24 @@ __global__ void box_decode_kernel(const DecodeParams p, int N, unsigned long lon
 // shared memory, bitonic sort.  box_output_layer.cpp:166-179.
 constexpr int kTopkThreads = 1024;
 
+// Bitonic sort of the shared keys sk[0 .. Kpad) into descending order (Kpad a power of two) by all kTopkThreads threads
+// of the CTA, which have filled sk and synchronised before the call; it ends synchronised.
+__device__ __forceinline__ void bitonic_sort_desc(unsigned long long* sk, int Kpad) {
+  const int tid = threadIdx.x;
+  for (int size = 2; size <= Kpad; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int i = tid; i < (Kpad >> 1); i += kTopkThreads) {
+        const int lo = 2 * i - (i & (stride - 1));
+        const int hi = lo + stride;
+        const bool desc = ((lo & size) == 0);
+        const unsigned long long a = sk[lo], b = sk[hi];
+        if ((a < b) == desc) { sk[lo] = b; sk[hi] = a; }
+      }
+      __syncthreads();
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kTopkThreads)
 box_topk_kernel(const unsigned long long* __restrict__ keys, const float4* __restrict__ boxes,
                 int A, int K, int Kpad, float4* __restrict__ sorted_boxes,
@@ -171,19 +189,7 @@ box_topk_kernel(const unsigned long long* __restrict__ keys, const float4* __res
     }
   }
   __syncthreads();
-  // bitonic sort, descending
-  for (int size = 2; size <= Kpad; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int i = tid; i < (Kpad >> 1); i += kTopkThreads) {
-        const int lo = 2 * i - (i & (stride - 1));
-        const int hi = lo + stride;
-        const bool desc = ((lo & size) == 0);
-        const unsigned long long a = sk[lo], b = sk[hi];
-        if ((a < b) == desc) { sk[lo] = b; sk[hi] = a; }
-      }
-      __syncthreads();
-    }
-  }
+  bitonic_sort_desc(sk, Kpad);
   for (int i = tid; i < M; i += kTopkThreads) {
     const unsigned long long k = sk[i];
     const unsigned int a = (unsigned int)(k & 0xFFFFFFFFull);
@@ -217,9 +223,35 @@ __device__ __forceinline__ float box_iou_ref(const float4 a, const float4 b, int
   return over / u;
 }
 
-// mask[n][i][cb] bit t  <=>  IoU(box i, box cb*64+t) > thr  and  cb*64+t > i
+// bbNms.m:112-126 overlap test in double ('union' denominator).
+__device__ __forceinline__ bool bbnms_overlaps(const float4 a, const float4 b, double overlap) {
+  const double axs = a.x, axe = (double)a.x + (double)a.z, ays = a.y, aye = (double)a.y + (double)a.w;
+  const double bxs = b.x, bxe = (double)b.x + (double)b.z, bys = b.y, bye = (double)b.y + (double)b.w;
+  const double iw = fmin(axe, bxe) - fmax(axs, bxs);
+  if (iw <= 0) return false;
+  const double ih = fmin(aye, bye) - fmax(ays, bys);
+  if (ih <= 0) return false;
+  double o = iw * ih;
+  const double u = (double)a.z * (double)a.w + (double)b.z * (double)b.w - o;
+  o = o / u;
+  return o > overlap;
+}
+
+// The suppression test of each NMS: BoxOutput's BoxIOU in fp32, the post-process's bbNms overlap in fp64.
+struct BoxIouTest {
+  float thr;
+  int mode;
+  __device__ __forceinline__ bool operator()(const float4 a, const float4 b) const { return box_iou_ref(a, b, mode) > thr; }
+};
+struct BbNmsTest {
+  double overlap;
+  __device__ __forceinline__ bool operator()(const float4 a, const float4 b) const { return bbnms_overlaps(a, b, overlap); }
+};
+
+// mask[n][i][cb] bit t  <=>  suppresses(box i, box cb*64+t)  and  cb*64+t > i
+template <class Test>
 __global__ void nms_mask_kernel(const float4* __restrict__ boxes, const int* __restrict__ counts,
-                                int Kpad, int words, float thr, int mode,
+                                int Kpad, int words, const Test suppresses,
                                 unsigned long long* __restrict__ mask) {
   const int n = blockIdx.z, rb = blockIdx.y, cb = blockIdx.x;
   const int M = counts[n];
@@ -236,7 +268,7 @@ __global__ void nms_mask_kernel(const float4* __restrict__ boxes, const int* __r
   unsigned long long bits = 0ull;
   const int start = (rb == cb) ? t + 1 : 0;
   for (int c = start; c < ncol; ++c)
-    if (box_iou_ref(me, cbox[c], mode) > thr) bits |= (1ull << c);
+    if (suppresses(me, cbox[c])) bits |= (1ull << c);
   mask[((size_t)n * Kpad + i) * words + cb] = bits;
 }
 
@@ -380,15 +412,15 @@ __global__ void box_finalize_kernel(const float4* __restrict__ boxes, const floa
 struct DetectParams {
   int num_cls, cls_id;  // cls_id is 1-based like the MATLAB script
   float mean[4], stdv[4];
-  float proposal_thr, ratio_h, ratio_w, org_h, org_w;
+  float proposal_thr;
 };
 
-// Per-image geometry [ratio_h, ratio_w, org_h, org_w] of the images n0 .. n0 + count - 1 of one launch, by value in
-// the kernel parameter block (1 KB); count = 0: every image of the launch uses DetectParams' four scalars.  The MATLAB
-// drivers read each frame's size inside their loop (run_mscnn_detection.m:64-65, run_cascademscnn.m:77-80).
+// Per-image geometry [ratio_h, ratio_w, org_h, org_w] of the images n0, n0 + 1, ... of one launch (one CTA each), by
+// value in the kernel parameter block (1 KB).  The MATLAB drivers read each frame's size inside their loop
+// (run_mscnn_detection.m:64-65, run_cascademscnn.m:77-80); a batch without per-image sizes repeats the cfg's four.
 constexpr int kGeomPerLaunch = 64;
 struct DetectGeom {
-  int n0, count;
+  int n0;
   float4 g[kGeomPerLaunch];
 };
 
@@ -411,11 +443,8 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
   extern __shared__ unsigned long long sk[];
   __shared__ int s_valid;
   const int n = geom.n0 + blockIdx.x, tid = threadIdx.x;
-  float ratio_h = p.ratio_h, ratio_w = p.ratio_w, org_h = p.org_h, org_w = p.org_w;
-  if (geom.count) {
-    const float4 q = geom.g[blockIdx.x];
-    ratio_h = q.x; ratio_w = q.y; org_h = q.z; org_w = q.w;
-  }
+  const float4 gn = geom.g[blockIdx.x];
+  const float ratio_h = gn.x, ratio_w = gn.y, org_h = gn.z, org_w = gn.w;
   int start = 0;
   for (int m = 0; m < n; ++m) start += num_rois[2 + m];
   int cnt = num_rois[2 + n];
@@ -469,18 +498,7 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
     atomicAdd(&s_valid, 1);
   }
   __syncthreads();
-  for (int size = 2; size <= Kpad; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int i = tid; i < (Kpad >> 1); i += kTopkThreads) {
-        const int lo = 2 * i - (i & (stride - 1));
-        const int hi = lo + stride;
-        const bool desc = ((lo & size) == 0);
-        const unsigned long long a = sk[lo], b = sk[hi];
-        if ((a < b) == desc) { sk[lo] = b; sk[hi] = a; }
-      }
-      __syncthreads();
-    }
-  }
+  bitonic_sort_desc(sk, Kpad);
   const int M = s_valid;
   for (int i = tid; i < M; i += kTopkThreads) {
     const unsigned long long k = sk[i];
@@ -489,42 +507,6 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
     sscores[(size_t)n * Kpad + i] = orderable_float((uint32_t)(k >> 32));
   }
   if (tid == 0) counts[n] = M;
-}
-
-// bbNms.m:112-126 overlap test in double ('union' denominator).
-__device__ __forceinline__ bool bbnms_overlaps(const float4 a, const float4 b, double overlap) {
-  const double axs = a.x, axe = (double)a.x + (double)a.z, ays = a.y, aye = (double)a.y + (double)a.w;
-  const double bxs = b.x, bxe = (double)b.x + (double)b.z, bys = b.y, bye = (double)b.y + (double)b.w;
-  const double iw = fmin(axe, bxe) - fmax(axs, bxs);
-  if (iw <= 0) return false;
-  const double ih = fmin(aye, bye) - fmax(ays, bys);
-  if (ih <= 0) return false;
-  double o = iw * ih;
-  const double u = (double)a.z * (double)a.w + (double)b.z * (double)b.w - o;
-  o = o / u;
-  return o > overlap;
-}
-
-__global__ void bbnms_mask_kernel(const float4* __restrict__ boxes, const int* __restrict__ counts,
-                                  int Kpad, int words, double overlap,
-                                  unsigned long long* __restrict__ mask) {
-  const int n = blockIdx.z, rb = blockIdx.y, cb = blockIdx.x;
-  const int M = counts[n];
-  if (cb < rb || rb * 64 >= M || cb * 64 >= M) return;
-  __shared__ float4 cbox[64];
-  const int t = threadIdx.x;
-  const float4* bx = boxes + (size_t)n * Kpad;
-  if (cb * 64 + t < M) cbox[t] = bx[cb * 64 + t];
-  __syncthreads();
-  const int i = rb * 64 + t;
-  if (i >= M) return;
-  const float4 me = bx[i];
-  const int ncol = min(64, M - cb * 64);
-  unsigned long long bits = 0ull;
-  const int start = (rb == cb) ? t + 1 : 0;
-  for (int c = start; c < ncol; ++c)
-    if (bbnms_overlaps(me, cbox[c], overlap)) bits |= (1ull << c);
-  mask[((size_t)n * Kpad + i) * words + cb] = bits;
 }
 
 // dets[n][r] = [x y w h prob], r < det_counts[n], in kept (score-descending) order.
@@ -547,9 +529,11 @@ __global__ void detect_write_kernel(const float4* __restrict__ sboxes, const flo
 // buffer with the post-process kernel"): payload = int32 header [N, total, counts[0..N)] padded to a multiple of 4
 // words, then the kept rows of all images back to back, [total][5] = [x y w h prob] in image order.  One block per
 // image; its row offset is the sum of the (capped) counts of the images before it.
-__global__ void detect_write_packed_kernel(const float4* __restrict__ sboxes, const float* __restrict__ sscores,
-                                           const int* __restrict__ keep_idx, const int* __restrict__ keep_count,
-                                           int Kpad, int cap, int N, float* __restrict__ payload) {
+struct PackedRows {
+  int hdr, off, cnt;  // header words of the payload; this image's first row and row count
+};
+__device__ __forceinline__ PackedRows pack_image_rows(const float4* sboxes, const float* sscores, const int* keep_idx,
+                                                      const int* keep_count, int Kpad, int cap, int N, float* payload) {
   const int n = blockIdx.x;
   int off = 0;
   for (int m = 0; m < n; ++m) off += min(keep_count[m], cap);
@@ -570,6 +554,13 @@ __global__ void detect_write_packed_kernel(const float4* __restrict__ sboxes, co
       head[1] = off + cnt;
     }
   }
+  return PackedRows{hdr, off, cnt};
+}
+
+__global__ void detect_write_packed_kernel(const float4* __restrict__ sboxes, const float* __restrict__ sscores,
+                                           const int* __restrict__ keep_idx, const int* __restrict__ keep_count,
+                                           int Kpad, int cap, int N, float* __restrict__ payload) {
+  pack_image_rows(sboxes, sscores, keep_idx, keep_count, Kpad, cap, N, payload);
 }
 
 // The same packing with the EXCHANGE FUSED IN (mscnn_net_detect_push): block n packs image n's rows into this rank's slot
@@ -583,26 +574,10 @@ __global__ void detect_push_packed_kernel(const float4* __restrict__ sboxes, con
                                           const int* __restrict__ keep_idx, const int* __restrict__ keep_count,
                                           int Kpad, int cap, int N, mscnn::PushTargets t, unsigned int seq,
                                           unsigned int* __restrict__ done_counter) {
-  const int n = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
-  int off = 0;
-  for (int m = 0; m < n; ++m) off += min(keep_count[m], cap);
-  const int cnt = min(keep_count[n], cap);
-  const int hdr = (2 + N + 3) & ~3;
+  const int tid = threadIdx.x, nt = blockDim.x;
   float* lbase = t.data[t.self];
-  for (int r = tid; r < cnt; r += nt) {
-    const int src = keep_idx[(size_t)n * Kpad + r];
-    const float4 b = sboxes[(size_t)n * Kpad + src];
-    float* o = lbase + hdr + (size_t)(off + r) * 5;
-    o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = b.w; o[4] = sscores[(size_t)n * Kpad + src];
-  }
-  if (tid == 0) {
-    int* head = reinterpret_cast<int*>(lbase);
-    head[2 + n] = cnt;
-    if (n == N - 1) {
-      head[0] = N;
-      head[1] = off + cnt;
-    }
-  }
+  const PackedRows pr = pack_image_rows(sboxes, sscores, keep_idx, keep_count, Kpad, cap, N, lbase);
+  const int hdr = pr.hdr, off = pr.off, cnt = pr.cnt;
   __syncthreads();
   // this block's rows = floats [f0, f1) of the slot; [a0, a1) is the 16-byte aligned middle (slot bases are aligned)
   const size_t f0 = (size_t)hdr + (size_t)off * 5, f1 = f0 + (size_t)cnt * 5;
@@ -755,8 +730,8 @@ extern "C" int mscnn_box_output_forward(const mscnn_box_output_cfg* cfg, int N, 
                                                          sscores, counts);
   const int words = Kpad / 64;
   mscnn::note_launch();
-  nms_mask_kernel<<<dim3(words, words, N), 64, 0, stream>>>(sboxes, counts, Kpad, words, cfg->iou_thr,
-                                                           cfg->nms_type, mask);
+  nms_mask_kernel<<<dim3(words, words, N), 64, 0, stream>>>(sboxes, counts, Kpad, words,
+                                                           BoxIouTest{cfg->iou_thr, cfg->nms_type}, mask);
   const size_t scan_smem = (size_t)2 * 64 * words * 8;
   e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_smem);
   if (e != cudaSuccess) return MSCNN_ERR_CUDA;
@@ -812,18 +787,19 @@ extern "C" int mscnn_detect_workspace_bytes(const mscnn_detect_cfg* cfg, int N, 
   return MSCNN_OK;
 }
 
-// geom: HOST [N][4] = ratio_h, ratio_w, org_h, org_w per image, or NULL for the cfg's four scalars.
-static int detect_run(bool cascade, const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
-                      const float* cls_pred, const float* bbox_pred, const int* num_rois, void* workspace,
-                      size_t workspace_bytes, float* dets, int* det_counts, const float* geom, void* stream_v,
-                      float* payload = nullptr, const mscnn::PushTargets* push = nullptr, unsigned int seq = 0,
-                      unsigned int* done_counter = nullptr) {
+int mscnn::detect_postprocess(bool cascade, const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
+                              const float* cls_pred, const float* bbox_pred, const int* num_rois, void* workspace,
+                              size_t workspace_bytes, const float* geom, const DetectOut& out, void* stream_v) {
   cudaStream_t stream = (cudaStream_t)stream_v;
   int Kpad;
   const int rc = det_cfg_check(cfg, N, &Kpad);
   if (rc) return rc;
-  if (!proposals_score || !cls_pred || !bbox_pred || !num_rois || !workspace || (!payload && !push && (!dets || !det_counts)))
+  if (!proposals_score || !cls_pred || !bbox_pred || !num_rois || !workspace) return MSCNN_ERR_INVALID;
+  if (out.push) {
+    if (out.push->count < 1 || out.push->count > kMaxPushRanks || !out.done_counter) return MSCNN_ERR_INVALID;
+  } else if (!out.payload && (!out.dets || !out.det_counts)) {
     return MSCNN_ERR_INVALID;
+  }
   if (geom)
     for (int k = 0; k < 4 * N; ++k)
       if (!(geom[k] > 0.f) || geom[k] == INFINITY) return MSCNN_ERR_INVALID;
@@ -835,8 +811,6 @@ static int detect_run(bool cascade, const mscnn_detect_cfg* cfg, int N, const fl
   p.cls_id = cfg->cls_id;
   for (int k = 0; k < 4; ++k) { p.mean[k] = cfg->bbox_mean[k]; p.stdv[k] = cfg->bbox_std[k]; }
   p.proposal_thr = cfg->proposal_thr;
-  p.ratio_h = cfg->ratio_h; p.ratio_w = cfg->ratio_w;
-  p.org_h = cfg->org_h; p.org_w = cfg->org_w;
   float4* dboxes = (float4*)(ws + w.dboxes);
   float4* sboxes = (float4*)(ws + w.sboxes);
   float* sscores = (float*)(ws + w.sscores);
@@ -851,15 +825,14 @@ static int detect_run(bool cascade, const mscnn_detect_cfg* cfg, int N, const fl
     e = cudaFuncSetAttribute(detect_decode_sort_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)smem);
   if (e != cudaSuccess) return MSCNN_ERR_CUDA;
-  // one launch for the whole batch without per-image geometry, one per kGeomPerLaunch images with it
-  const int per_launch = geom ? kGeomPerLaunch : N;
-  for (int n0 = 0; n0 < N; n0 += per_launch) {
+  for (int n0 = 0; n0 < N; n0 += kGeomPerLaunch) {
+    const int blocks = N - n0 < kGeomPerLaunch ? N - n0 : kGeomPerLaunch;
     DetectGeom g;
     g.n0 = n0;
-    g.count = geom ? (N - n0 < kGeomPerLaunch ? N - n0 : kGeomPerLaunch) : 0;
-    for (int i = 0; i < g.count; ++i)
-      g.g[i] = make_float4(geom[4 * (n0 + i)], geom[4 * (n0 + i) + 1], geom[4 * (n0 + i) + 2], geom[4 * (n0 + i) + 3]);
-    const int blocks = geom ? g.count : N;
+    for (int i = 0; i < blocks; ++i)
+      g.g[i] = geom ? make_float4(geom[4 * (n0 + i)], geom[4 * (n0 + i) + 1], geom[4 * (n0 + i) + 2],
+                                  geom[4 * (n0 + i) + 3])
+                    : make_float4(cfg->ratio_h, cfg->ratio_w, cfg->org_h, cfg->org_w);
     mscnn::note_launch();
     if (cascade)
       detect_decode_sort_kernel<true><<<blocks, kTopkThreads, smem, stream>>>(p, g, proposals_score, cls_pred, bbox_pred,
@@ -872,23 +845,23 @@ static int detect_run(bool cascade, const mscnn_detect_cfg* cfg, int N, const fl
   }
   const int words = Kpad / 64;
   mscnn::note_launch();
-  bbnms_mask_kernel<<<dim3(words, words, N), 64, 0, stream>>>(sboxes, counts, Kpad, words,
-                                                             (double)cfg->nms_overlap, mask);
+  nms_mask_kernel<<<dim3(words, words, N), 64, 0, stream>>>(sboxes, counts, Kpad, words,
+                                                           BbNmsTest{(double)cfg->nms_overlap}, mask);
   const size_t scan_smem = (size_t)2 * 64 * words * 8;
   e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_smem);
   if (e != cudaSuccess) return MSCNN_ERR_CUDA;
   mscnn::note_launch();
   nms_scan_kernel<<<N, kScanThreads, scan_smem, stream>>>(mask, counts, Kpad, words, 0, keep_idx, keep_count);
   mscnn::note_launch();
-  if (push)
+  if (out.push)
     detect_push_packed_kernel<<<N, 256, 0, stream>>>(sboxes, sscores, keep_idx, keep_count, Kpad,
-                                                    cfg->max_rois_per_image, N, *push, seq, done_counter);
-  else if (payload)
+                                                    cfg->max_rois_per_image, N, *out.push, out.seq, out.done_counter);
+  else if (out.payload)
     detect_write_packed_kernel<<<N, 256, 0, stream>>>(sboxes, sscores, keep_idx, keep_count, Kpad,
-                                                     cfg->max_rois_per_image, N, payload);
+                                                     cfg->max_rois_per_image, N, out.payload);
   else
     detect_write_kernel<<<N, 256, 0, stream>>>(sboxes, sscores, keep_idx, keep_count, Kpad,
-                                              cfg->max_rois_per_image, dets, det_counts);
+                                              cfg->max_rois_per_image, out.dets, out.det_counts);
   e = cudaGetLastError();
   if (e != cudaSuccess) {
     fprintf(stderr, "mscnn_detect_postprocess: %s\n", cudaGetErrorString(e));
@@ -901,8 +874,8 @@ extern "C" int mscnn_detect_postprocess(const mscnn_detect_cfg* cfg, int N, cons
                                         const float* cls_pred, const float* bbox_pred, const int* num_rois,
                                         void* workspace, size_t workspace_bytes, float* dets,
                                         int* det_counts, void* stream) {
-  return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
-                    dets, det_counts, nullptr, stream);
+  return detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+                            nullptr, DetectOut::padded(dets, det_counts), stream);
 }
 
 extern "C" int mscnn_detect_postprocess_sized(const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
@@ -910,8 +883,8 @@ extern "C" int mscnn_detect_postprocess_sized(const mscnn_detect_cfg* cfg, int N
                                               void* workspace, size_t workspace_bytes, float* dets, int* det_counts,
                                               const float* geom, void* stream) {
   if (!geom) return MSCNN_ERR_INVALID;
-  return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
-                    dets, det_counts, geom, stream);
+  return detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+                            geom, DetectOut::padded(dets, det_counts), stream);
 }
 
 extern "C" int mscnn_detect_image_geometry(int net_h, int net_w, int N, const int* org_hw, float* geom) {
@@ -939,8 +912,8 @@ extern "C" int mscnn_detect_postprocess_packed(const mscnn_detect_cfg* cfg, int 
                                                const float* cls_pred, const float* bbox_pred, const int* num_rois,
                                                void* workspace, size_t workspace_bytes, float* payload, void* stream) {
   if (!payload) return MSCNN_ERR_INVALID;
-  return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
-                    nullptr, nullptr, nullptr, stream, payload);
+  return detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+                            nullptr, DetectOut::packed(payload), stream);
 }
 
 extern "C" int mscnn_detect_postprocess_packed_sized(const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
@@ -948,26 +921,16 @@ extern "C" int mscnn_detect_postprocess_packed_sized(const mscnn_detect_cfg* cfg
                                                      const int* num_rois, void* workspace, size_t workspace_bytes,
                                                      float* payload, const float* geom, void* stream) {
   if (!payload || !geom) return MSCNN_ERR_INVALID;
-  return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
-                    nullptr, nullptr, geom, stream, payload);
-}
-
-// internal entry of the peer-memory exchange (xchg.cu): post-process + fused push
-int mscnn::detect_postprocess_push(const mscnn_detect_cfg* cfg, int N, const float* proposals_score, const float* cls_pred,
-                                   const float* bbox_pred, const int* num_rois, void* workspace, size_t workspace_bytes,
-                                   const PushTargets* push, unsigned int seq, unsigned int* done_counter,
-                                   const float* geom, void* stream) {
-  if (!push || push->count < 1 || push->count > kMaxPushRanks || !done_counter) return MSCNN_ERR_INVALID;
-  return detect_run(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes, nullptr,
-                    nullptr, geom, stream, nullptr, push, seq, done_counter);
+  return detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+                            geom, DetectOut::packed(payload), stream);
 }
 
 extern "C" int mscnn_cascade_detect_postprocess(const mscnn_detect_cfg* cfg, int N, const float* proposals,
                                                 const float* cls_prob, const float* output_bbox,
                                                 const int* num_rois, void* workspace, size_t workspace_bytes,
                                                 float* dets, int* det_counts, void* stream) {
-  return detect_run(true, cfg, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes, dets,
-                    det_counts, nullptr, stream);
+  return detect_postprocess(true, cfg, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes,
+                            nullptr, DetectOut::padded(dets, det_counts), stream);
 }
 
 extern "C" int mscnn_cascade_detect_postprocess_sized(const mscnn_detect_cfg* cfg, int N, const float* proposals,
@@ -975,6 +938,6 @@ extern "C" int mscnn_cascade_detect_postprocess_sized(const mscnn_detect_cfg* cf
                                                       const int* num_rois, void* workspace, size_t workspace_bytes,
                                                       float* dets, int* det_counts, const float* geom, void* stream) {
   if (!geom) return MSCNN_ERR_INVALID;
-  return detect_run(true, cfg, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes, dets,
-                    det_counts, geom, stream);
+  return detect_postprocess(true, cfg, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes,
+                            geom, DetectOut::padded(dets, det_counts), stream);
 }

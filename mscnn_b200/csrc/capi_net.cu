@@ -46,12 +46,54 @@ int settle_pending(NetHandle* nh) {
   nh->pending_input = false;
   return cudaStreamWaitEvent(Caffe::stream(), nh->input_ready, 0) == cudaSuccess ? MSCNN_OK : MSCNN_ERR_CUDA;
 }
-// Per-image geometry of the last forward for a post-process over N images: NULL when that forward had none.
-int forward_geometry(const NetHandle* nh, int N, const float** geom) {
-  *geom = nullptr;
-  if (nh->geom.empty()) return MSCNN_OK;
-  if (nh->geom.size() != (size_t)4 * N) return MSCNN_ERR_INVALID;
-  *geom = nh->geom.data();
+// The input blob `name` as the destination of plan's pre-processing of N images: it must hold exactly N images of the
+// plan's output size.  A pending asynchronous upload is settled first.
+int preprocess_target(NetHandle* nh, const char* name, void* plan, int N, float** dst) {
+  nh->net->ResolveRowsFor(name);
+  if (!nh->net->has_blob(name)) return MSCNN_ERR_INVALID;
+  mscnn_preprocess_desc d;
+  if (mscnn_preprocess_get_desc(plan, &d) != MSCNN_OK) return MSCNN_ERR_INVALID;
+  Blob<float>* b = nh->net->blob_by_name(name).get();
+  if (b->count() != (long)N * 3 * d.out_h * d.out_w) return MSCNN_ERR_INVALID;
+  if (settle_pending(nh) != MSCNN_OK) return MSCNN_ERR_CUDA;
+  *dst = b->mutable_gpu_data();
+  return MSCNN_OK;
+}
+// The post-process inputs of the last forward, as every mscnn_net_detect* entry needs them.
+struct DetectInputs {
+  int N;
+  const float *prop, *cls, *bbox;
+  const float* geom;  // per-image geometry of the last forward, NULL when it had none (= the cfg's scalars)
+};
+// Checks that the box layer and the three input blobs exist and that cfg keeps every proposal, grows the workspace and
+// looks up the last forward's geometry.
+int detect_inputs(NetHandle* h, const mscnn_detect_cfg* cfg, const char* prop, const char* cls, const char* bbox,
+                  DetectInputs* in) {
+  if (!h->box || !cfg || !prop || !cls || !bbox || !h->net->has_blob(prop) || !h->net->has_blob(cls) ||
+      !h->net->has_blob(bbox))
+    return MSCNN_ERR_INVALID;
+  const int N = h->net->input_blobs()[0]->num();
+  // The post-process keeps every proposal of an image (run_mscnn_detection.m:75-120 has no cap): a cfg whose
+  // max_rois_per_image is below what BoxOutput can emit would silently drop rows, so it is refused instead.
+  if (cfg->max_rois_per_image < h->box->max_rows_per_image()) {
+    fprintf(stderr, "mscnn_net_detect: max_rois_per_image = %d < %d proposals an image can carry (BoxOutput max_nms_num / "
+            "max_post_nms_num)\n", cfg->max_rois_per_image, h->box->max_rows_per_image());
+    return MSCNN_ERR_INVALID;
+  }
+  size_t need = 0;
+  const int rc = mscnn_detect_workspace_bytes(cfg, N, &need);
+  if (rc) return rc;
+  if (need > h->det_ws_bytes) {
+    if (h->det_ws) cudaFree(h->det_ws);
+    if (cudaMalloc(&h->det_ws, need) != cudaSuccess) return MSCNN_ERR_NOMEM;
+    h->det_ws_bytes = need;
+  }
+  if (!h->geom.empty() && h->geom.size() != (size_t)4 * N) return MSCNN_ERR_INVALID;
+  in->N = N;
+  in->prop = h->net->blob_by_name(prop)->gpu_data();
+  in->cls = h->net->blob_by_name(cls)->gpu_data();
+  in->bbox = h->net->blob_by_name(bbox)->gpu_data();
+  in->geom = h->geom.empty() ? nullptr : h->geom.data();
   return MSCNN_OK;
 }
 int fill_shape(const std::vector<int>& s, int* shape4) {
@@ -220,15 +262,11 @@ int mscnn_net_set_blob(void* h, const char* name, const float* host, long count)
 }
 // uint8 host images -> device pre-processing -> input blob (run_mscnn_detection.m:64-69 on the device)
 int mscnn_net_set_input_images(void* h, const char* name, void* plan, int N, const unsigned char* host_images) {
-  H(h)->net->ResolveRowsFor(name);
-  if (!H(h)->net->has_blob(name)) return MSCNN_ERR_INVALID;
-  mscnn_preprocess_desc d;
-  if (mscnn_preprocess_get_desc(plan, &d) != MSCNN_OK) return MSCNN_ERR_INVALID;
-  Blob<float>* b = H(h)->net->blob_by_name(name).get();
-  if (b->count() != (long)N * 3 * d.out_h * d.out_w) return MSCNN_ERR_INVALID;
-  if (settle_pending(H(h)) != MSCNN_OK) return MSCNN_ERR_CUDA;
+  float* dst = nullptr;
+  const int rc = preprocess_target(H(h), name, plan, N, &dst);
+  if (rc) return rc;
   H(h)->next_org_hw.clear();  // these images replace any sized batch set before them
-  return mscnn_preprocess_forward_host(plan, N, host_images, b->mutable_gpu_data(), Caffe::stream());
+  return mscnn_preprocess_forward_host(plan, N, host_images, dst, Caffe::stream());
 }
 // The same for images of different original sizes (run_mscnn_detection.m:64-65 reads each frame's size): records
 // them as the geometry of the next forward.
@@ -237,14 +275,10 @@ int mscnn_net_set_input_images_sized(void* h, const char* name, void* plan, int 
   if (N < 1 || !in_hw || !host_images) return MSCNN_ERR_INVALID;
   for (int n = 0; n < N; ++n)
     if (in_hw[2 * n] < 1 || in_hw[2 * n + 1] < 1) return MSCNN_ERR_INVALID;
-  H(h)->net->ResolveRowsFor(name);
-  if (!H(h)->net->has_blob(name)) return MSCNN_ERR_INVALID;
-  mscnn_preprocess_desc d;
-  if (mscnn_preprocess_get_desc(plan, &d) != MSCNN_OK) return MSCNN_ERR_INVALID;
-  Blob<float>* b = H(h)->net->blob_by_name(name).get();
-  if (b->count() != (long)N * 3 * d.out_h * d.out_w) return MSCNN_ERR_INVALID;
-  if (settle_pending(H(h)) != MSCNN_OK) return MSCNN_ERR_CUDA;
-  const int rc = mscnn_preprocess_forward_sized_host(plan, N, in_hw, host_images, b->mutable_gpu_data(), Caffe::stream());
+  float* dst = nullptr;
+  int rc = preprocess_target(H(h), name, plan, N, &dst);
+  if (rc) return rc;
+  rc = mscnn_preprocess_forward_sized_host(plan, N, in_hw, host_images, dst, Caffe::stream());
   if (rc != MSCNN_OK) return rc;
   H(h)->next_org_hw.assign(in_hw, in_hw + 2 * N);
   return MSCNN_OK;
@@ -415,79 +449,30 @@ int mscnn_net_num_proposals(void* h, int image) {
 // net's proposals_score / cls_pred / bbox_pred blobs.
 int mscnn_net_detect(void* hv, const mscnn_detect_cfg* cfg, float* dets_dev, int* det_counts_dev) {
   NetHandle* h = H(hv);
-  if (!h->box || !h->net->has_blob("proposals_score") || !h->net->has_blob("cls_pred") ||
-      !h->net->has_blob("bbox_pred"))
-    return MSCNN_ERR_INVALID;
-  const int N = h->net->input_blobs()[0]->num();
-  // The post-process keeps every proposal of an image (run_mscnn_detection.m:75-120 has no cap): a cfg whose
-  // max_rois_per_image is below what BoxOutput can emit would silently drop rows, so it is refused instead.
-  if (cfg->max_rois_per_image < h->box->max_rows_per_image()) {
-    fprintf(stderr, "mscnn_net_detect: max_rois_per_image = %d < %d proposals an image can carry (BoxOutput max_nms_num / "
-            "max_post_nms_num)\n", cfg->max_rois_per_image, h->box->max_rows_per_image());
-    return MSCNN_ERR_INVALID;
-  }
-  size_t need = 0;
-  int rc = mscnn_detect_workspace_bytes(cfg, N, &need);
+  DetectInputs in;
+  const int rc = detect_inputs(h, cfg, "proposals_score", "cls_pred", "bbox_pred", &in);
   if (rc) return rc;
-  if (need > h->det_ws_bytes) {
-    if (h->det_ws) cudaFree(h->det_ws);
-    if (cudaMalloc(&h->det_ws, need) != cudaSuccess) return MSCNN_ERR_NOMEM;
-    h->det_ws_bytes = need;
-  }
-  const float* geom = nullptr;
-  if (forward_geometry(h, N, &geom) != MSCNN_OK) return MSCNN_ERR_INVALID;
-  if (geom)
-    return mscnn_detect_postprocess_sized(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
-                                          h->net->blob_by_name("cls_pred")->gpu_data(),
-                                          h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(),
-                                          h->det_ws, h->det_ws_bytes, dets_dev, det_counts_dev, geom, Caffe::stream());
-  return mscnn_detect_postprocess(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
-                                  h->net->blob_by_name("cls_pred")->gpu_data(),
-                                  h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(),
-                                  h->det_ws, h->det_ws_bytes, dets_dev, det_counts_dev, Caffe::stream());
+  return mscnn::detect_postprocess(false, cfg, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
+                                   h->det_ws_bytes, in.geom, mscnn::DetectOut::padded(dets_dev, det_counts_dev),
+                                   Caffe::stream());
 }
 // Final detections of this rank's images, packed (header + compacted rows), then ONE all-gather on the communicator's
 // stream.  The producer stream first waits for the previous gather (it still reads / writes payload_all).
 int mscnn_net_detect_gather(void* hv, const mscnn_detect_cfg* cfg, void* comm, float* payload_all) {
   NetHandle* h = H(hv);
-  if (!h->box || !comm || !payload_all || !h->net->has_blob("proposals_score") || !h->net->has_blob("cls_pred") ||
-      !h->net->has_blob("bbox_pred"))
-    return MSCNN_ERR_INVALID;
-  const int N = h->net->input_blobs()[0]->num();
-  // The post-process keeps every proposal of an image (run_mscnn_detection.m:75-120 has no cap): a cfg whose
-  // max_rois_per_image is below what BoxOutput can emit would silently drop rows, so it is refused instead.
-  if (cfg->max_rois_per_image < h->box->max_rows_per_image()) {
-    fprintf(stderr, "mscnn_net_detect: max_rois_per_image = %d < %d proposals an image can carry (BoxOutput max_nms_num / "
-            "max_post_nms_num)\n", cfg->max_rois_per_image, h->box->max_rows_per_image());
-    return MSCNN_ERR_INVALID;
-  }
+  if (!comm || !payload_all) return MSCNN_ERR_INVALID;
+  DetectInputs in;
+  int rc = detect_inputs(h, cfg, "proposals_score", "cls_pred", "bbox_pred", &in);
+  if (rc) return rc;
   int nranks = 0, rank = 0;
-  int rc = mscnn_comm_info(comm, &nranks, &rank, nullptr);
+  rc = mscnn_comm_info(comm, &nranks, &rank, nullptr);
   if (rc) return rc;
-  size_t need = 0;
-  rc = mscnn_detect_workspace_bytes(cfg, N, &need);
-  if (rc) return rc;
-  if (need > h->det_ws_bytes) {
-    if (h->det_ws) cudaFree(h->det_ws);
-    if (cudaMalloc(&h->det_ws, need) != cudaSuccess) return MSCNN_ERR_NOMEM;
-    h->det_ws_bytes = need;
-  }
-  const float* geom = nullptr;
-  if (forward_geometry(h, N, &geom) != MSCNN_OK) return MSCNN_ERR_INVALID;
-  const size_t per = mscnn_detect_payload_floats(N, cfg->max_rois_per_image);
+  const size_t per = mscnn_detect_payload_floats(in.N, cfg->max_rois_per_image);
   rc = mscnn_comm_stream_wait(comm, Caffe::stream());
   if (rc) return rc;
-  if (geom)
-    rc = mscnn_detect_postprocess_packed_sized(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
-                                               h->net->blob_by_name("cls_pred")->gpu_data(),
-                                               h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(),
-                                               h->det_ws, h->det_ws_bytes, payload_all + (size_t)rank * per, geom,
-                                               Caffe::stream());
-  else
-    rc = mscnn_detect_postprocess_packed(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
-                                         h->net->blob_by_name("cls_pred")->gpu_data(),
-                                         h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(),
-                                         h->det_ws, h->det_ws_bytes, payload_all + (size_t)rank * per, Caffe::stream());
+  rc = mscnn::detect_postprocess(false, cfg, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
+                                 h->det_ws_bytes, in.geom, mscnn::DetectOut::packed(payload_all + (size_t)rank * per),
+                                 Caffe::stream());
   if (rc) return rc;
   return mscnn_comm_all_gather(comm, payload_all, per, Caffe::stream());
 }
@@ -495,62 +480,23 @@ int mscnn_net_detect_gather(void* hv, const mscnn_detect_cfg* cfg, void* comm, f
 // (peer-memory exchange, xchg.cu): no collective, nothing else to launch.
 int mscnn_net_detect_push(void* hv, const mscnn_detect_cfg* cfg, void* xchg) {
   NetHandle* h = H(hv);
-  if (!h->box || !xchg || !h->net->has_blob("proposals_score") || !h->net->has_blob("cls_pred") ||
-      !h->net->has_blob("bbox_pred"))
-    return MSCNN_ERR_INVALID;
-  const int N = h->net->input_blobs()[0]->num();
-  if (cfg->max_rois_per_image < h->box->max_rows_per_image()) return MSCNN_ERR_INVALID;
-  size_t need = 0;
-  int rc = mscnn_detect_workspace_bytes(cfg, N, &need);
+  if (!xchg) return MSCNN_ERR_INVALID;
+  DetectInputs in;
+  const int rc = detect_inputs(h, cfg, "proposals_score", "cls_pred", "bbox_pred", &in);
   if (rc) return rc;
-  if (need > h->det_ws_bytes) {
-    if (h->det_ws) cudaFree(h->det_ws);
-    if (cudaMalloc(&h->det_ws, need) != cudaSuccess) return MSCNN_ERR_NOMEM;
-    h->det_ws_bytes = need;
-  }
-  const float* geom = nullptr;
-  if (forward_geometry(h, N, &geom) != MSCNN_OK) return MSCNN_ERR_INVALID;
-  return mscnn::xchg_detect_push(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
-                                 h->net->blob_by_name("cls_pred")->gpu_data(),
-                                 h->net->blob_by_name("bbox_pred")->gpu_data(), h->box->num_out_device(), h->det_ws,
-                                 h->det_ws_bytes, xchg, geom, Caffe::stream());
+  return mscnn::xchg_detect_push(cfg, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
+                                 h->det_ws_bytes, xchg, in.geom, Caffe::stream());
 }
 int mscnn_net_detect_cascade(void* hv, const mscnn_detect_cfg* cfg, const char* proposals_blob,
                              const char* cls_prob_blob, const char* output_bbox_blob, float* dets_dev,
                              int* det_counts_dev) {
   NetHandle* h = H(hv);
-  if (!h->box || !proposals_blob || !cls_prob_blob || !output_bbox_blob || !h->net->has_blob(proposals_blob) ||
-      !h->net->has_blob(cls_prob_blob) || !h->net->has_blob(output_bbox_blob))
-    return MSCNN_ERR_INVALID;
-  const int N = h->net->input_blobs()[0]->num();
-  // The post-process keeps every proposal of an image (run_mscnn_detection.m:75-120 has no cap): a cfg whose
-  // max_rois_per_image is below what BoxOutput can emit would silently drop rows, so it is refused instead.
-  if (cfg->max_rois_per_image < h->box->max_rows_per_image()) {
-    fprintf(stderr, "mscnn_net_detect: max_rois_per_image = %d < %d proposals an image can carry (BoxOutput max_nms_num / "
-            "max_post_nms_num)\n", cfg->max_rois_per_image, h->box->max_rows_per_image());
-    return MSCNN_ERR_INVALID;
-  }
-  size_t need = 0;
-  int rc = mscnn_detect_workspace_bytes(cfg, N, &need);
+  DetectInputs in;
+  const int rc = detect_inputs(h, cfg, proposals_blob, cls_prob_blob, output_bbox_blob, &in);
   if (rc) return rc;
-  if (need > h->det_ws_bytes) {
-    if (h->det_ws) cudaFree(h->det_ws);
-    if (cudaMalloc(&h->det_ws, need) != cudaSuccess) return MSCNN_ERR_NOMEM;
-    h->det_ws_bytes = need;
-  }
   if (h->net->blob_by_name(cls_prob_blob)->channels() != cfg->num_cls) return MSCNN_ERR_INVALID;
-  const float* geom = nullptr;
-  if (forward_geometry(h, N, &geom) != MSCNN_OK) return MSCNN_ERR_INVALID;
-  if (geom)
-    return mscnn_cascade_detect_postprocess_sized(cfg, N, h->net->blob_by_name(proposals_blob)->gpu_data(),
-                                                  h->net->blob_by_name(cls_prob_blob)->gpu_data(),
-                                                  h->net->blob_by_name(output_bbox_blob)->gpu_data(),
-                                                  h->box->num_out_device(), h->det_ws, h->det_ws_bytes, dets_dev,
-                                                  det_counts_dev, geom, Caffe::stream());
-  return mscnn_cascade_detect_postprocess(cfg, N, h->net->blob_by_name(proposals_blob)->gpu_data(),
-                                          h->net->blob_by_name(cls_prob_blob)->gpu_data(),
-                                          h->net->blob_by_name(output_bbox_blob)->gpu_data(),
-                                          h->box->num_out_device(), h->det_ws, h->det_ws_bytes, dets_dev,
-                                          det_counts_dev, Caffe::stream());
+  return mscnn::detect_postprocess(true, cfg, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
+                                   h->det_ws_bytes, in.geom, mscnn::DetectOut::padded(dets_dev, det_counts_dev),
+                                   Caffe::stream());
 }
 }

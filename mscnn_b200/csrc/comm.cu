@@ -7,7 +7,7 @@
 // (mscnn_comm_init_all) or per process (mscnn_comm_init_rank).
 //
 // ONE ncclAllGather per step: each rank's payload carries its per-image counts in a header in front of the compacted
-// rows (detect_write_packed_kernel, box_output.cu), so no second collective for the counts.  The collective runs on
+// rows (pack_image_rows, box_output.cu), so no second collective for the counts.  The collective runs on
 // the communicator's own stream: it waits (on the device) for the producer stream's tail and the producer goes on
 // with the next step's trunk, so step k's gather overlaps step k + 1's convolutions.
 //

@@ -228,8 +228,8 @@ int mscnn::xchg_detect_push(const mscnn_detect_cfg* cfg, int N, const float* pro
     t.flag[p] = gen_flags(x->peer[p], x, gen) + x->rank;
   }
   unsigned int* counter = reinterpret_cast<unsigned int*>(x->local + (size_t)x->gens * x->gen_bytes);
-  const int rc = mscnn::detect_postprocess_push(cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace,
-                                                workspace_bytes, &t, seq, counter, geom, stream);
+  const int rc = mscnn::detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace,
+                                           workspace_bytes, geom, mscnn::DetectOut::pushed(&t, seq, counter), stream);
   if (rc == MSCNN_OK) x->seq = seq;
   return rc;
 }

@@ -275,51 +275,34 @@ def eltwise_forward(bottoms: list[torch.Tensor], op: int, coeffs=None) -> torch.
     return y
 
 
-def _geometry(geometry, n: int) -> np.ndarray:
-    """Host float32 [n][4] = ratio_h, ratio_w, org_h, org_w per image (see mscnn_detect_image_geometry)."""
-    g = np.ascontiguousarray(geometry, dtype=np.float32)
-    assert g.shape == (n, 4), (g.shape, n)
-    return g
+def _detect(entry: str, cfg: capi.DetectCfg, n: int, inputs, num_out, geometry):
+    """Post-process through mscnn_<entry> (geometry None) or mscnn_<entry>_sized: padded dets [n, cap, 5], counts [n]."""
+    import ctypes as C
+    dev = inputs[0].device
+    nbytes = C.c_size_t(0)
+    capi.check(capi.lib().mscnn_detect_workspace_bytes(cfg, n, C.byref(nbytes)), "detect_workspace")
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    dets = torch.zeros((n, cfg.max_rois_per_image, 5), dtype=torch.float32, device=dev)
+    counts = torch.zeros(n, dtype=torch.int32, device=dev)
+    args = (cfg, n, *map(capi.ptr, inputs), capi.ptr(num_out), capi.ptr(ws), nbytes.value, capi.ptr(dets),
+            capi.ptr(counts))
+    if geometry is None:
+        capi.check(getattr(capi.lib(), "mscnn_" + entry)(*args, _stream()), entry)
+    else:
+        g = np.ascontiguousarray(geometry, dtype=np.float32)
+        assert g.shape == (n, 4), (g.shape, n)
+        capi.check(getattr(capi.lib(), f"mscnn_{entry}_sized")(*args, g.ctypes.data, _stream()), entry + "_sized")
+    return dets, counts
 
 
 def cascade_detect_postprocess(cfg: capi.DetectCfg, n: int, proposals, cls_prob, output_bbox, num_out, geometry=None):
     """geometry: None (the cfg's ratio_* / org_*) or per-image [n][4] = ratio_h, ratio_w, org_h, org_w."""
-    import ctypes as C
-    dev = proposals.device
-    nbytes = C.c_size_t(0)
-    capi.check(capi.lib().mscnn_detect_workspace_bytes(cfg, n, C.byref(nbytes)), "detect_workspace")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-    dets = torch.zeros((n, cfg.max_rois_per_image, 5), dtype=torch.float32, device=dev)
-    counts = torch.zeros(n, dtype=torch.int32, device=dev)
-    args = (cfg, n, capi.ptr(proposals), capi.ptr(cls_prob), capi.ptr(output_bbox), capi.ptr(num_out), capi.ptr(ws),
-            nbytes.value, capi.ptr(dets), capi.ptr(counts))
-    if geometry is None:
-        capi.check(capi.lib().mscnn_cascade_detect_postprocess(*args, _stream()), "cascade_detect_postprocess")
-    else:
-        g = _geometry(geometry, n)
-        capi.check(capi.lib().mscnn_cascade_detect_postprocess_sized(*args, g.ctypes.data, _stream()),
-                   "cascade_detect_postprocess_sized")
-    return dets, counts
+    return _detect("cascade_detect_postprocess", cfg, n, (proposals, cls_prob, output_bbox), num_out, geometry)
 
 
 def detect_postprocess(cfg: capi.DetectCfg, n: int, proposals_score, cls_pred, bbox_pred, num_out, geometry=None):
     """geometry: None (the cfg's ratio_* / org_*) or per-image [n][4] = ratio_h, ratio_w, org_h, org_w."""
-    import ctypes as C
-    dev = proposals_score.device
-    nbytes = C.c_size_t(0)
-    capi.check(capi.lib().mscnn_detect_workspace_bytes(cfg, n, C.byref(nbytes)), "detect_workspace")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-    dets = torch.zeros((n, cfg.max_rois_per_image, 5), dtype=torch.float32, device=dev)
-    counts = torch.zeros(n, dtype=torch.int32, device=dev)
-    args = (cfg, n, capi.ptr(proposals_score), capi.ptr(cls_pred), capi.ptr(bbox_pred), capi.ptr(num_out),
-            capi.ptr(ws), nbytes.value, capi.ptr(dets), capi.ptr(counts))
-    if geometry is None:
-        capi.check(capi.lib().mscnn_detect_postprocess(*args, _stream()), "detect_postprocess")
-    else:
-        g = _geometry(geometry, n)
-        capi.check(capi.lib().mscnn_detect_postprocess_sized(*args, g.ctypes.data, _stream()),
-                   "detect_postprocess_sized")
-    return dets, counts
+    return _detect("detect_postprocess", cfg, n, (proposals_score, cls_pred, bbox_pred), num_out, geometry)
 
 
 def conv1_tc_forward(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None, relu: bool, split: bool) -> Planes:

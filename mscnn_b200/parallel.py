@@ -209,7 +209,7 @@ def _cuda_view(ptr: int, n_floats: int) -> torch.Tensor:
 
 
 def pack_payload(dets: np.ndarray, counts: np.ndarray, cap: int) -> np.ndarray:
-    """Host restatement of detect_write_packed_kernel (used by the CPU tests): dets [B, cap, 5], counts [B]."""
+    """Host restatement of pack_image_rows in box_output.cu (used by the CPU tests): dets [B, cap, 5], counts [B]."""
     b = len(counts)
     out = np.zeros(payload_floats(b, cap), dtype=np.float32)
     head = out.view(np.int32)

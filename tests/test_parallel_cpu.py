@@ -1,5 +1,5 @@
 """world_size-2 gloo test of the multi-GPU plumbing on CPU tensors: sharding, the packed detection payload (header with
-the per-image counts + compacted rows, the layout detect_write_packed_kernel writes) and its rank-major all-gather.  On
+the per-image counts + compacted rows, the layout pack_image_rows writes) and its rank-major all-gather.  On
 the GPU box the same payload is produced by the kernel and moved by ONE ncclAllGather inside libmscnn_b200.so
 (mscnn_net_detect_gather; tests/test_multigpu_gpu.py, bench.py --gpus N)."""
 import os
