@@ -19,6 +19,7 @@ ERR_NOMEM = -3
 
 OUT_NHWC_BF16 = 0
 OUT_NCHW_F32 = 1
+OUT_NHWC_F32 = 2
 POOL_MAX = 0
 POOL_AVE = 1
 NMS_IOU, NMS_IOMU, NMS_IOFU = 0, 1, 2
@@ -126,6 +127,27 @@ def _declare(L: C.CDLL) -> None:
                                          c_void_p]
     L.mscnn_roi_align_forward.restype = c_int
     L.mscnn_roi_align_forward.argtypes = L.mscnn_roi_pool_forward.argtypes
+    # data-dependent row counts: the same arguments plus a device int count before the stream
+    L.mscnn_pool_forward_dyn.restype = c_int
+    L.mscnn_pool_forward_dyn.argtypes = [c_void_p] * 4 + [c_int] * 7 + [c_void_p, c_void_p]
+    L.mscnn_roi_pool_multi_forward.restype = c_int
+    L.mscnn_roi_pool_multi_forward.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                                               c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                               c_int, c_void_p]
+    L.mscnn_roi_pool_multi_forward_dyn.restype = c_int
+    L.mscnn_roi_pool_multi_forward_dyn.argtypes = L.mscnn_roi_pool_multi_forward.argtypes[:-1] + [c_void_p, c_void_p]
+    L.mscnn_roi_align_forward_dyn.restype = c_int
+    L.mscnn_roi_align_forward_dyn.argtypes = L.mscnn_roi_align_forward.argtypes[:-1] + [c_void_p, c_void_p]
+    L.mscnn_pack_head_weights.restype = c_int
+    L.mscnn_pack_head_weights.argtypes = [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]
+    L.mscnn_head_gather.restype = c_int
+    L.mscnn_head_gather.argtypes = [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]
+    L.mscnn_relu_planes.restype = c_int
+    L.mscnn_relu_planes.argtypes = [c_void_p, c_void_p, C.c_size_t, c_void_p]
+    L.mscnn_relu_f32.restype = c_int
+    L.mscnn_relu_f32.argtypes = [c_void_p, C.c_size_t, c_void_p]
+    L.mscnn_concat_planes.restype = c_int
+    L.mscnn_concat_planes.argtypes = [c_void_p, c_void_p, C.c_size_t, c_int, c_int, c_int, c_void_p]
     L.mscnn_decode_bbox_forward.restype = c_int
     L.mscnn_decode_bbox_forward.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
     L.mscnn_softmax_forward.restype = c_int

@@ -435,6 +435,9 @@ extern "C" int mscnn_roi_pool_multi_forward_dyn(const void* x_hi, const void* x_
   if (!x_hi || !y_hi || !rois || !pad_ratios || !out_channel_offsets || N <= 0 || C % 8 || R < 0 ||
       pooled_h <= 0 || pooled_w <= 0 || out_channels_total % 8 || num_variants < 1 || num_variants > 4)
     return MSCNN_ERR_INVALID;
+  // split input and split output go together, as in every other plane entry: the kernel would otherwise store the
+  // rounded hi alone of an fp32-faithful input, or a lo plane of zeros
+  if ((x_lo == nullptr) != (y_lo == nullptr)) return MSCNN_ERR_INVALID;
   RoiVariants var;
   var.count = num_variants;
   for (int i = 0; i < num_variants; ++i) {

@@ -109,31 +109,50 @@ def pack_fc_weights(w: torch.Tensor, b: torch.Tensor | None, split: bool, c: int
     return PackedWeights(hi, lo, bias, nout, 1, 1)
 
 
-def conv_forward(x: Planes, w: PackedWeights, pad: int, relu: bool, out_f32: bool = False,
-                 out_split: bool | None = None, pool: str | None = None):
+def conv_forward(x: Planes, w: PackedWeights, pad, relu: bool, out_f32: bool = False,
+                 out_split: bool | None = None, pool: str | None = None, dyn: torch.Tensor | None = None,
+                 out_mode: int | None = None, out=None):
     """Convolution (stride 1) + bias (+ReLU).  Returns Planes, or an NCHW fp32 tensor when
-    ``out_f32``.  An InnerProduct is the KH=KW=H=W=1 case."""
+    ``out_f32``.  An InnerProduct is the KH=KW=H=W=1 case.
+
+    pad: an int, or (pad_h, pad_w).  out_mode = capi.OUT_NHWC_F32 returns pixel-major fp32 rows
+    [N][Ho][Wo][Cout_pad] (the head-tap partial sums).  dyn: a device int32 tensor of one element, the
+    number of images / rows to compute (rows at or above it are left as they were).  out: a tensor or
+    Planes of the returned kind to write into instead of a new one."""
     n, h, wd, c = x.hi.shape
     assert w.hi.shape[3] == c, (w.hi.shape, x.hi.shape)
-    ho, wo = h + 2 * pad - w.kh + 1, wd + 2 * pad - w.kw + 1
+    pad_h, pad_w = (pad, pad) if isinstance(pad, int) else pad
+    ho, wo = h + 2 * pad_h - w.kh + 1, wd + 2 * pad_w - w.kw + 1
     cout_pad = w.hi.shape[0]
+    if out_mode is None:
+        out_mode = capi.OUT_NCHW_F32 if out_f32 else capi.OUT_NHWC_BF16
     d = capi.ConvDesc()
     d.x_hi, d.x_lo = capi.ptr(x.hi), capi.ptr(x.lo)
     d.N, d.H, d.W, d.C = n, h, wd, c
     d.w_hi, d.w_lo, d.bias = capi.ptr(w.hi), capi.ptr(w.lo), capi.ptr(w.bias)
-    d.Cout, d.Cout_pad, d.KH, d.KW, d.pad_h, d.pad_w = w.cout, cout_pad, w.kh, w.kw, pad, pad
+    d.Cout, d.Cout_pad, d.KH, d.KW, d.pad_h, d.pad_w = w.cout, cout_pad, w.kh, w.kw, pad_h, pad_w
     d.relu = int(relu)
-    if out_f32:
-        y = torch.empty((n, w.cout, ho, wo), dtype=torch.float32, device=x.hi.device)
-        d.out_mode, d.y_f32 = capi.OUT_NCHW_F32, capi.ptr(y)
+    if dyn is not None:
+        assert dyn.is_cuda and dyn.dtype == torch.int32 and dyn.numel() == 1
+        d.dyn_n = capi.ptr(dyn)
+    if out_mode in (capi.OUT_NCHW_F32, capi.OUT_NHWC_F32):
+        shape = (n, w.cout, ho, wo) if out_mode == capi.OUT_NCHW_F32 else (n, ho, wo, cout_pad)
+        y = torch.empty(shape, dtype=torch.float32, device=x.hi.device) if out is None else out
+        assert tuple(y.shape) == shape and y.dtype == torch.float32 and y.is_contiguous()
+        d.out_mode, d.y_f32 = out_mode, capi.ptr(y)
         out = y
     else:
-        if out_split is None:
-            out_split = x.lo is not None
-        y_hi = torch.empty((n, ho, wo, cout_pad), dtype=torch.bfloat16, device=x.hi.device)
-        y_lo = torch.empty_like(y_hi) if out_split else None
+        assert out_mode == capi.OUT_NHWC_BF16
+        if out is None:
+            if out_split is None:
+                out_split = x.lo is not None
+            y_hi = torch.empty((n, ho, wo, cout_pad), dtype=torch.bfloat16, device=x.hi.device)
+            y_lo = torch.empty_like(y_hi) if out_split else None
+            out = Planes(y_hi, y_lo, w.cout)
+        else:
+            assert not pool and out.shape == (n, ho, wo, cout_pad)
+            y_hi, y_lo = out.hi, out.lo
         d.out_mode, d.y_hi, d.y_lo = capi.OUT_NHWC_BF16, capi.ptr(y_hi), capi.ptr(y_lo)
-        out = Planes(y_hi, y_lo, w.cout)
         if pool:   # "both": conv output and its fused 2x2 max pool; "only": pooled tensor alone
             p_hi = torch.empty((n, ho // 2, wo // 2, cout_pad), dtype=torch.bfloat16, device=x.hi.device)
             p_lo = torch.empty_like(p_hi) if out_split else None
@@ -148,15 +167,25 @@ def conv_forward(x: Planes, w: PackedWeights, pad: int, relu: bool, out_f32: boo
     return out
 
 
-def pool_forward(x: Planes, kernel: int, stride: int, mode: int = capi.POOL_MAX) -> Planes:
+def pool_forward(x: Planes, kernel: int, stride: int, mode: int = capi.POOL_MAX, dyn: torch.Tensor | None = None,
+                 out: Planes | None = None) -> Planes:
+    """dyn: a device int32 tensor of one element, the number of images to pool (mscnn_pool_forward_dyn);
+    out: planes to write into instead of new ones."""
     n, h, w, c = x.hi.shape
     ho = -(-(h - kernel) // stride) + 1
     wo = -(-(w - kernel) // stride) + 1
-    y_hi = torch.empty((n, ho, wo, c), dtype=torch.bfloat16, device=x.hi.device)
-    y_lo = torch.empty_like(y_hi) if x.lo is not None else None
-    capi.check(capi.lib().mscnn_pool_forward(capi.ptr(x.hi), capi.ptr(x.lo), capi.ptr(y_hi), capi.ptr(y_lo),
-                                             n, h, w, c, kernel, stride, mode, _stream()), "pool_forward")
-    return Planes(y_hi, y_lo, x.channels)
+    if out is None:
+        y_hi = torch.empty((n, ho, wo, c), dtype=torch.bfloat16, device=x.hi.device)
+        y_lo = torch.empty_like(y_hi) if x.lo is not None else None
+        out = Planes(y_hi, y_lo, x.channels)
+    assert out.shape == (n, ho, wo, c)
+    args = (capi.ptr(x.hi), capi.ptr(x.lo), capi.ptr(out.hi), capi.ptr(out.lo), n, h, w, c, kernel, stride, mode)
+    if dyn is None:
+        capi.check(capi.lib().mscnn_pool_forward(*args, _stream()), "pool_forward")
+    else:
+        assert dyn.is_cuda and dyn.dtype == torch.int32 and dyn.numel() == 1
+        capi.check(capi.lib().mscnn_pool_forward_dyn(*args, capi.ptr(dyn), _stream()), "pool_forward_dyn")
+    return out
 
 
 def deconv2x_forward(x: Planes, w: torch.Tensor) -> Planes:
@@ -231,16 +260,51 @@ def roi_pool_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled: int, 
     return out
 
 
-def roi_align_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled: int, scale: float,
-                      pad_ratio: float) -> Planes:
-    """ROIAlign grid [R, pooled+1, pooled+1, C] (roi_align_layer.cpp:49-139)."""
+def roi_pool_multi_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled: int, scale: float,
+                           pad_ratios, channel_offsets, out: Planes | None = None, out_channels: int | None = None,
+                           dyn: torch.Tensor | None = None) -> Planes:
+    """Up to four pad_ratio variants of one ROI set in one launch; variant i is written at channel offset
+    channel_offsets[i] of a [R, pooled, pooled, out_channels] output.  dyn: device int32 ROI count."""
+    import ctypes as C
     n, h, w, c = x.hi.shape
-    y_hi = torch.zeros((num_rois, pooled + 1, pooled + 1, c), dtype=torch.bfloat16, device=x.hi.device)
-    y_lo = torch.zeros_like(y_hi) if x.lo is not None else None
-    out = Planes(y_hi, y_lo, c)
-    capi.check(capi.lib().mscnn_roi_align_forward(capi.ptr(x.hi), capi.ptr(x.lo), n, h, w, c, capi.ptr(rois),
-                                                  num_rois, pooled, pooled, scale, pad_ratio, capi.ptr(out.hi),
-                                                  capi.ptr(out.lo), c, 0, _stream()), "roi_align_forward")
+    nv = len(pad_ratios)
+    assert len(channel_offsets) == nv
+    ctot = out_channels or nv * c
+    if out is None:
+        y_hi = torch.zeros((num_rois, pooled, pooled, ctot), dtype=torch.bfloat16, device=x.hi.device)
+        y_lo = torch.zeros_like(y_hi) if x.lo is not None else None
+        out = Planes(y_hi, y_lo, ctot)
+    ratios = (C.c_float * max(nv, 1))(*pad_ratios)
+    offs = (C.c_int * max(nv, 1))(*channel_offsets)
+    args = (capi.ptr(x.hi), capi.ptr(x.lo), n, h, w, c, capi.ptr(rois), num_rois, pooled, pooled, scale, nv,
+            C.cast(ratios, C.c_void_p), C.cast(offs, C.c_void_p), capi.ptr(out.hi), capi.ptr(out.lo), ctot)
+    if dyn is None:
+        capi.check(capi.lib().mscnn_roi_pool_multi_forward(*args, _stream()), "roi_pool_multi_forward")
+    else:
+        assert dyn.is_cuda and dyn.dtype == torch.int32 and dyn.numel() == 1
+        capi.check(capi.lib().mscnn_roi_pool_multi_forward_dyn(*args, capi.ptr(dyn), _stream()),
+                   "roi_pool_multi_forward_dyn")
+    return out
+
+
+def roi_align_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled: int, scale: float,
+                      pad_ratio: float, out: Planes | None = None, channel_offset: int = 0,
+                      out_channels: int | None = None, dyn: torch.Tensor | None = None) -> Planes:
+    """ROIAlign grid [R, pooled+1, pooled+1, C] (roi_align_layer.cpp:49-139), written at channel offset
+    ``channel_offset`` of an ``out_channels``-wide output.  dyn: device int32 ROI count."""
+    n, h, w, c = x.hi.shape
+    ctot = out_channels or c
+    if out is None:
+        y_hi = torch.zeros((num_rois, pooled + 1, pooled + 1, ctot), dtype=torch.bfloat16, device=x.hi.device)
+        y_lo = torch.zeros_like(y_hi) if x.lo is not None else None
+        out = Planes(y_hi, y_lo, ctot)
+    args = (capi.ptr(x.hi), capi.ptr(x.lo), n, h, w, c, capi.ptr(rois), num_rois, pooled, pooled, scale, pad_ratio,
+            capi.ptr(out.hi), capi.ptr(out.lo), ctot, channel_offset)
+    if dyn is None:
+        capi.check(capi.lib().mscnn_roi_align_forward(*args, _stream()), "roi_align_forward")
+    else:
+        assert dyn.is_cuda and dyn.dtype == torch.int32 and dyn.numel() == 1
+        capi.check(capi.lib().mscnn_roi_align_forward_dyn(*args, capi.ptr(dyn), _stream()), "roi_align_forward_dyn")
     return out
 
 

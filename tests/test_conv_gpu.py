@@ -172,6 +172,51 @@ def test_conv_head_f32_nchw(cuda, k, pad, split):
         _report("head", got, ref, 1e-4, 1e-4 * float(ref.pow(2).mean().sqrt()))  # fp32 accumulation over K=6272
 
 
+def _head_taps(x, wt, b, split):
+    """The Net's k x k head path: the horizontal taps as GEMM columns (mscnn_pack_head_weights, a k x 1 convolution
+    into pixel-major fp32 rows P[pixel][dx * Cout + co]), then mscnn_head_gather sums P over dx and adds the bias."""
+    from mscnn_b200 import capi, ops
+    cout, cin, k, _ = wt.shape
+    n, _, h, w = x.shape
+    n_pad = (k * cout + 63) // 64 * 64
+    cin_pad = ops.pad64(cin)
+    hi = torch.empty((n_pad, k, 1, cin_pad), dtype=torch.bfloat16, device=x.device)
+    lo = torch.empty_like(hi) if split else None
+    L = capi.lib()
+    stream = torch.cuda.current_stream().cuda_stream
+    capi.check(L.mscnn_pack_head_weights(capi.ptr(wt), capi.ptr(hi), capi.ptr(lo), cout, cin, k, n_pad, cin_pad,
+                                         stream), "pack_head_weights")
+    wp = ops.PackedWeights(hi, lo, torch.zeros(n_pad, dtype=torch.float32, device=x.device), n_pad, k, 1)
+    p = ops.conv_forward(ops.nchw_to_planes(x, split), wp, (k // 2, 0), relu=False, out_mode=capi.OUT_NHWC_F32)
+    assert tuple(p.shape) == (n, h, w, n_pad)
+    y = torch.empty((n, cout, h, w), dtype=torch.float32, device=x.device)
+    capi.check(L.mscnn_head_gather(capi.ptr(p), n_pad, capi.ptr(b), capi.ptr(y), n, h, w, cout, k, k // 2, stream),
+               "head_gather")
+    return y
+
+
+@pytest.mark.parametrize("split", [True, False], ids=["split", "bf16"])
+@pytest.mark.parametrize("cin", [64, 512])
+@pytest.mark.parametrize("cout", [6, 9])
+@pytest.mark.parametrize("k", [3, 5, 7])
+def test_conv_head_taps(cuda, k, cout, cin, split):
+    """The LFCN heads as the Net runs them (the only non-square convolution and the only OUT_NHWC_F32 user), vs fp64,
+    at test_conv_head_f32_nchw's bars.  Widths and heights below the reach of the taps, a single pixel, and a width
+    past one 128-pixel tile."""
+    g = torch.Generator(device="cpu").manual_seed(100 * k + cout + cin)
+    for n, h, w in [(1, 1, 1), (2, 3, k - 1), (3, 12, 40), (1, 5, 129)]:
+        x = torch.randn((n, cin, h, w), generator=g).to(cuda)
+        wt = (torch.randn((cout, cin, k, k), generator=g) * 0.02).to(cuda)
+        b = (torch.randn((cout,), generator=g) * 0.1).to(cuda)
+        got = _head_taps(x, wt, b, split)
+        torch.cuda.synchronize()
+        if split:
+            ref = _ref_conv(x, wt, b, k // 2, False)
+        else:
+            ref = _ref_conv(x.bfloat16().float(), wt.bfloat16().float(), b, k // 2, False)
+        _report(f"head taps k={k} shape={(n, h, w)}", got, ref, 1e-4, 1e-4 * float(ref.pow(2).mean().sqrt()))
+
+
 @pytest.mark.parametrize("split", [True, False], ids=["split", "bf16"])
 def test_inner_product(cuda, split):
     """InnerProduct (inner_product_layer.cpp:84-97): Y = X W^T + b with X the NCHW flattening of

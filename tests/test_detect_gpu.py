@@ -135,12 +135,17 @@ def _bf16_exact(a):
     return torch.from_numpy(a).bfloat16().float().numpy()
 
 
+ROI_POOL_CASES = [(pr, s, p, c) for c in (128, 512) for pr, s, p in [(0.0, 0.125, 7), (0.25, 0.125, 7), (0.25, 0.25, 5)]]
+
+
 @pytest.mark.parametrize("split", [True, False], ids=["split", "bf16"])
-@pytest.mark.parametrize("pad_ratio,scale,pooled", [(0.0, 0.125, 7), (0.25, 0.125, 7), (0.25, 0.25, 5)])
-def test_roi_pool_parity(cuda, split, pad_ratio, scale, pooled):
+# C = 512 (conv4_3): every lane pools two channel groups.  The C = 128 cases keep their original ids.
+@pytest.mark.parametrize("pad_ratio,scale,pooled,c", ROI_POOL_CASES,
+                         ids=[f"{pr}-{s}-{p}" + ("" if c == 128 else f"-c{c}") for pr, s, p, c in ROI_POOL_CASES])
+def test_roi_pool_parity(cuda, split, pad_ratio, scale, pooled, c):
     from mscnn_b200 import ops
     rng = np.random.default_rng(5)
-    n, c, h, w = 2, 128, 24, 80
+    n, h, w = 2, 24, 80
     x = _bf16_exact(rng.standard_normal((n, c, h, w)).astype(np.float32))
     img_w, img_h = w / scale, h / scale
     r = 200
@@ -174,17 +179,23 @@ def test_roi_pool_fused_concat(cuda):
     assert np.array_equal(got, ref)
 
 
+POOL_CASES = [("MAX", 24, 80, 2, 2), ("MAX", 9, 15, 2, 2), ("AVE", 12, 16, 2, 2), ("AVE", 7, 5, 2, 2),
+              # stride 1 (the cascade nets' AVE 2/1 on the ROIAlign grid) and 3/2 windows that overlap, odd sizes
+              ("MAX", 7, 9, 2, 1), ("AVE", 6, 11, 2, 1), ("MAX", 9, 15, 3, 2), ("AVE", 8, 13, 3, 2)]
+
+
 @pytest.mark.parametrize("split", [True, False], ids=["split", "bf16"])
-@pytest.mark.parametrize("mode,h,w", [("MAX", 24, 80), ("MAX", 9, 15), ("AVE", 12, 16), ("AVE", 7, 5)])
-def test_pool_parity(cuda, split, mode, h, w):
-    """2x2 stride 2, including odd sizes where ceil mode adds a clipped last window
+@pytest.mark.parametrize("mode,h,w,k,s", POOL_CASES,
+                         ids=[f"{m}-{h}-{w}" + ("" if (k, s) == (2, 2) else f"-k{k}s{s}") for m, h, w, k, s in POOL_CASES])
+def test_pool_parity(cuda, split, mode, h, w, k, s):
+    """2x2 stride 2, 2x2 stride 1 and 3x3 stride 2, including odd sizes where ceil mode adds a clipped last window
     (pooling_layer.cpp:90-93)."""
     from mscnn_b200 import capi, ops
     rng = np.random.default_rng(13)
     x = _bf16_exact(rng.standard_normal((2, 64, h, w)).astype(np.float32))
-    ref = port.pool(x, 2, 2, 0, mode)
+    ref = port.pool(x, k, s, 0, mode)
     xp = ops.nchw_to_planes(torch.from_numpy(x).to(cuda), split)
-    out = ops.pool_forward(xp, 2, 2, capi.POOL_MAX if mode == "MAX" else capi.POOL_AVE)
+    out = ops.pool_forward(xp, k, s, capi.POOL_MAX if mode == "MAX" else capi.POOL_AVE)
     got = ops.planes_to_nchw(out).cpu().numpy()
     assert got.shape == ref.shape
     if mode == "MAX":
