@@ -17,15 +17,27 @@ namespace caffe {
 // constant, gaussian, bilinear (the only ones the MS-CNN prototxts name); anything else aborts.
 CAFFE_API void FillBlob(const FillerParameter& filler, Blob<float>* blob);
 
-// Device copies of packed weights (planes) owned by Convolution / InnerProduct layers.
+// Device copies of the packed weights (planes) and zero-padded biases owned by Convolution / InnerProduct layers,
+// brought up to date in the first forward after a change: a forward with unchanged parameters, precision and shapes
+// allocates and copies nothing, so it can be captured into a CUDA graph.
+struct PackedBias {
+  float* data = nullptr;
+  int len = 0;  // padded length
+  const Blob<float>* src = nullptr;
+  unsigned long version = ~0ul;
+  ~PackedBias();
+  void update(Blob<float>* b, int n, int n_pad);  // b[0:n], then zeros up to n_pad (b == NULL: all zeros)
+};
 struct PackedParam {
-  PlaneStore w;          // [Cout_pad][KH][KW][Cin_pad] bf16 hi (+lo)
-  float* bias = nullptr; // [Cout_pad]
-  int cout_pad = 0, cin_pad = 0;
-  unsigned long w_version = ~0ul, b_version = ~0ul;
-  bool split = false;
-  long key = -1;         // layout key (fc: bottom C*H*W arrangement)
-  ~PackedParam();
+  enum Route { CONV, HEAD, CONV1_1, FC };
+  // what `w` holds: the route that packed it, its padding and (fc) the bottom's C, H, W
+  struct Layout { int route, split, out_pad, in_pad, c, h, w; };
+  PlaneStore w;  // bf16 hi (+ lo when layout.split)
+  Layout layout = {-1};
+  unsigned long w_version = ~0ul;
+  PackedBias bias, gather_bias;  // [layout.out_pad] for the kernel; k x k heads: [Cout] for the tap gather
+  // re-packs with pack(w_f32, hi, lo) when wb's version or the layout changed; lo = NULL unless l.split
+  template <typename Pack> void update_weights(Blob<float>* wb, const Layout& l, size_t bytes, Pack pack);
 };
 
 /// InputLayer: /root/reference/src/caffe/layers/input_layer.cpp:8-22
@@ -73,10 +85,6 @@ class CAFFE_API ConvolutionLayer : public Layer<Dtype> {
   int num_output_, channels_, kernel_h_, kernel_w_, pad_h_, pad_w_;
   bool bias_term_, fuse_relu_;
   PackedParam packed_;
-  float* head_bias_ = nullptr;        // narrow k x k heads: bias applied by the tap gather
-  unsigned long head_bias_version_ = ~0ul;
- public:
-  virtual ~ConvolutionLayer();
 };
 
 /// DeconvolutionLayer: deconv_layer.cpp:8-40, restricted to the depthwise 4/2/1 bilinear-upsampling
@@ -253,7 +261,7 @@ template <typename Dtype>
 class CAFFE_API ROIPoolingLayer : public Layer<Dtype> {
  public:
   explicit ROIPoolingLayer(const LayerParameter& param)
-      : Layer<Dtype>(param), concat_top_(nullptr), concat_offset_(0), concat_channels_(0), rows_source_(nullptr) {}
+      : Layer<Dtype>(param), concat_top_(nullptr), concat_offset_(0), concat_channels_(0) {}
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "ROIPooling"; }
@@ -261,9 +269,6 @@ class CAFFE_API ROIPoolingLayer : public Layer<Dtype> {
   virtual inline int MaxBottomBlobs() const { return 2; }
   virtual inline int MinTopBlobs() const { return 1; }
   virtual inline int MaxTopBlobs() const { return 1; }
-  // mscnn_b200 extension (set by Net): the BoxOutput layer this layer's ROI list descends from (per-image row counts
-  // for the gather schedule; NULL = unknown origin, plain schedule).
-  void set_rows_source(const BoxOutputLayer<Dtype>* box) { rows_source_ = box; }
   // mscnn_b200 extension (set by Net): write into `target` (the Concat top) at a channel offset.
   void set_concat_target(Blob<Dtype>* target, int channel_offset, int total_channels) {
     concat_top_ = target; concat_offset_ = channel_offset; concat_channels_ = total_channels;
@@ -290,7 +295,6 @@ class CAFFE_API ROIPoolingLayer : public Layer<Dtype> {
   float spatial_scale_, pad_ratio_;
   Blob<Dtype>* concat_top_;
   int concat_offset_, concat_channels_;
-  const BoxOutputLayer<Dtype>* rows_source_;
   vector<Sibling> siblings_;
   bool done_by_leader_ = false;
 };

@@ -12,8 +12,45 @@ namespace caffe {
 static inline int pad64(int c) { return (c + 63) / 64 * 64; }
 static inline int out_pad(int c) { return c > 32 ? pad64(c) : 32; }
 
-PackedParam::~PackedParam() {
-  if (bias) cudaFree(bias);
+PackedBias::~PackedBias() {
+  if (data) cudaFree(data);
+}
+void PackedBias::update(Blob<float>* b, int n, int n_pad) {
+  const unsigned long ver = b ? b->version() : 0;
+  if (data && len == n_pad && src == b && version == ver) return;
+  if (data && len != n_pad) { CUDA_CHECK(cudaFree(data)); data = nullptr; }
+  if (!data) CUDA_CHECK(cudaMalloc(&data, sizeof(float) * n_pad));
+  CUDA_CHECK(cudaMemsetAsync(data, 0, sizeof(float) * n_pad, Caffe::stream()));
+  if (b)
+    CUDA_CHECK(cudaMemcpyAsync(data, b->gpu_data(), sizeof(float) * n, cudaMemcpyDeviceToDevice, Caffe::stream()));
+  len = n_pad;
+  src = b;
+  version = ver;
+}
+template <typename Pack>
+void PackedParam::update_weights(Blob<float>* wb, const Layout& l, size_t bytes, Pack pack) {
+  if (w_version == wb->version() && memcmp(&layout, &l, sizeof(l)) == 0) return;
+  w.reserve(bytes, l.split);
+  pack(wb->gpu_data(), w.hi, l.split ? w.lo : nullptr);
+  w_version = wb->version();
+  layout = l;
+}
+
+// The mscnn_conv_desc fields every route through mscnn_conv_forward shares; the caller sets out_mode, the outputs,
+// pooling and relu.
+static mscnn_conv_desc conv_desc(const Blob<float>::Planes& x, const PackedParam& pk, int N, int H, int W, int C,
+                                 int cout, int kh, int kw, int pad_h, int pad_w, const int* dyn_n) {
+  mscnn_conv_desc d;
+  memset(&d, 0, sizeof(d));
+  d.x_hi = x.hi; d.x_lo = x.lo;
+  d.N = N; d.H = H; d.W = W; d.C = C;
+  d.w_hi = pk.w.hi; d.w_lo = pk.layout.split ? pk.w.lo : nullptr;
+  d.bias = pk.bias.data;
+  d.Cout = cout; d.Cout_pad = pk.layout.out_pad;
+  d.KH = kh; d.KW = kw;
+  d.pad_h = pad_h; d.pad_w = pad_w;
+  d.dyn_n = dyn_n;
+  return d;
 }
 
 void FillBlob(const FillerParameter& filler, Blob<float>* blob) {
@@ -118,47 +155,12 @@ void ConvolutionLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const 
   top[0]->Reshape(bottom[0]->num(), num_output_, ho, wo);
 }
 
-// (re)pack weights when the fp32 blobs or the precision changed
-static void ensure_packed_conv(PackedParam* pk, Blob<float>* w, Blob<float>* b, bool split, int cout, int cin,
-                               int kh, int kw) {
-  const int cout_pad = out_pad(cout);
-  const int cin_pad = pad64(cin);
-  const bool stale_w = pk->w_version != w->version() || pk->split != split || pk->cout_pad != cout_pad ||
-                       pk->cin_pad != cin_pad;
-  if (stale_w) {
-    const size_t bytes = (size_t)cout_pad * kh * kw * cin_pad * 2;
-    pk->w.reserve(bytes, split);
-    MSCNN_CHECK(mscnn_pack_conv_weights(w->gpu_data(), pk->w.hi, split ? pk->w.lo : nullptr, cout, cin, kh, kw,
-                                        cout_pad, cin_pad, Caffe::stream()));
-    pk->w_version = w->version();
-    pk->split = split;
-  }
-  const unsigned long bver = b ? b->version() : 0;
-  if (!pk->bias || pk->cout_pad != cout_pad || pk->b_version != bver) {
-    if (pk->bias && pk->cout_pad != cout_pad) { CUDA_CHECK(cudaFree(pk->bias)); pk->bias = nullptr; }
-    if (!pk->bias) CUDA_CHECK(cudaMalloc(&pk->bias, sizeof(float) * cout_pad));
-    CUDA_CHECK(cudaMemsetAsync(pk->bias, 0, sizeof(float) * cout_pad, Caffe::stream()));
-    if (b)
-      CUDA_CHECK(cudaMemcpyAsync(pk->bias, b->gpu_data(), sizeof(float) * cout, cudaMemcpyDeviceToDevice,
-                                 Caffe::stream()));
-    pk->b_version = bver;
-  }
-  pk->cout_pad = cout_pad;
-  pk->cin_pad = cin_pad;
-}
-
-template <typename Dtype>
-ConvolutionLayer<Dtype>::~ConvolutionLayer() {
-  if (head_bias_) cudaFree(head_bias_);
-}
-
 template <typename Dtype>
 void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   const bool split = Caffe::split();
   const int N = bottom[0]->num(), H = bottom[0]->height(), W = bottom[0]->width();
+  Blob<Dtype>* wb = this->blobs_[0].get();
   Blob<Dtype>* bias = bias_term_ ? this->blobs_[1].get() : nullptr;
-  mscnn_conv_desc d;
-  memset(&d, 0, sizeof(d));
   // Narrow k x k proposal heads (LFCN_*: 9 or 6 outputs, 5x5 / 7x7, "same" padding): the horizontal
   // taps move into the GEMM's N dimension and a 1-D gather sums them (mscnn_head_gather in the C ABI).
   const bool head_path = (num_output_ == 9 || num_output_ == 6) && kernel_h_ == kernel_w_ && kernel_h_ > 1 &&
@@ -167,86 +169,51 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
   if (head_path) {
     const int k = kernel_h_;
     const int n_pad = (k * num_output_ + 63) / 64 * 64;
-    Blob<Dtype>* wb = this->blobs_[0].get();
-    if (packed_.w_version != wb->version() || packed_.split != split || packed_.cout_pad != n_pad) {
-      packed_.w.reserve((size_t)n_pad * k * channels_ * 2, split);
-      MSCNN_CHECK(mscnn_pack_head_weights(wb->gpu_data(), packed_.w.hi, split ? packed_.w.lo : nullptr, num_output_,
-                                          channels_, k, n_pad, channels_, Caffe::stream()));
-      if (packed_.bias) CUDA_CHECK(cudaFree(packed_.bias));
-      CUDA_CHECK(cudaMalloc(&packed_.bias, sizeof(float) * n_pad));
-      CUDA_CHECK(cudaMemsetAsync(packed_.bias, 0, sizeof(float) * n_pad, Caffe::stream()));  // bias is added later
-      packed_.w_version = wb->version();
-      packed_.split = split;
-      packed_.cout_pad = n_pad;
-    }
-    const unsigned long bver = bias ? bias->version() : 0;
-    if (!head_bias_ || head_bias_version_ != bver) {
-      if (!head_bias_) CUDA_CHECK(cudaMalloc(&head_bias_, sizeof(float) * num_output_));
-      CUDA_CHECK(cudaMemsetAsync(head_bias_, 0, sizeof(float) * num_output_, Caffe::stream()));
-      if (bias)
-        CUDA_CHECK(cudaMemcpyAsync(head_bias_, bias->gpu_data(), sizeof(float) * num_output_,
-                                   cudaMemcpyDeviceToDevice, Caffe::stream()));
-      head_bias_version_ = bver;
-    }
+    packed_.update_weights(wb, {PackedParam::HEAD, split, n_pad, channels_, 0, 0, 0},
+                           (size_t)n_pad * k * channels_ * 2, [&](const float* w, void* hi, void* lo) {
+      MSCNN_CHECK(mscnn_pack_head_weights(w, hi, lo, num_output_, channels_, k, n_pad, channels_, Caffe::stream()));
+    });
+    packed_.bias.update(nullptr, 0, n_pad);  // the bias is added by the gather
+    packed_.gather_bias.update(bias, num_output_, num_output_);
     typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
     float* P = static_cast<float*>(Caffe::scratch((size_t)N * H * W * n_pad * sizeof(float)));
-    d.x_hi = x.hi; d.x_lo = x.lo;
-    d.N = N; d.H = H; d.W = W; d.C = x.cpad;
-    d.w_hi = packed_.w.hi; d.w_lo = split ? packed_.w.lo : nullptr;
-    d.bias = packed_.bias;
-    d.Cout = n_pad; d.Cout_pad = n_pad;
-    d.KH = k; d.KW = 1;        // vertical taps stay in K ...
-    d.pad_h = pad_h_; d.pad_w = 0;
-    d.out_mode = MSCNN_OUT_NHWC_F32;  // ... horizontal taps are columns of P
+    // vertical taps stay in K, horizontal taps are columns of P
+    mscnn_conv_desc d = conv_desc(x, packed_, N, H, W, x.cpad, n_pad, k, 1, pad_h_, 0, this->dyn_rows_device());
+    d.out_mode = MSCNN_OUT_NHWC_F32;
     d.y_f32 = P;
-    d.dyn_n = this->dyn_rows_device();
-  MSCNN_CHECK(mscnn_conv_forward(&d, Caffe::stream()));
-    MSCNN_CHECK(mscnn_head_gather(P, n_pad, head_bias_, top[0]->mutable_gpu_data(), N, H, W, num_output_, k, pad_h_,
-                                  Caffe::stream()));
+    MSCNN_CHECK(mscnn_conv_forward(&d, Caffe::stream()));
+    MSCNN_CHECK(mscnn_head_gather(P, n_pad, packed_.gather_bias.data, top[0]->mutable_gpu_data(), N, H, W, num_output_,
+                                  k, pad_h_, Caffe::stream()));
     return;
   }
   // conv1_1 (3 -> 64 channels, 3x3, pad 1): K = 27 is far below one 64-channel tensor-core k-block.
   // One kernel from the fp32 NCHW blob to planes: pixel rows staged once, the horizontal taps are
-  // descriptor-shifted views of them (mscnn_conv1_tc_forward, conv_c3_tc.cu).
+  // descriptor-shifted views of them (mscnn_conv1_tc_forward, conv_c3_tc.cu).  Its packed image serves
+  // both precisions, so a precision switch does not re-pack it.
   if (channels_ == 3 && kernel_h_ == 3 && kernel_w_ == 3 && pad_h_ == 1 && pad_w_ == 1 && num_output_ == 64) {
-    Blob<Dtype>* wb = this->blobs_[0].get();
-    if (packed_.w_version != wb->version()) {
-      packed_.w.reserve((size_t)mscnn_conv1_tc_packed_bytes(), false);
-      MSCNN_CHECK(mscnn_pack_conv1_tc_weights(wb->gpu_data(), packed_.w.hi, 1, Caffe::stream()));
-      packed_.w_version = wb->version();
-    }
-    const unsigned long bver = bias ? bias->version() : 0;
-    if (!packed_.bias || packed_.b_version != bver) {
-      if (!packed_.bias) CUDA_CHECK(cudaMalloc(&packed_.bias, sizeof(float) * 64));
-      CUDA_CHECK(cudaMemsetAsync(packed_.bias, 0, sizeof(float) * 64, Caffe::stream()));
-      if (bias)
-        CUDA_CHECK(cudaMemcpyAsync(packed_.bias, bias->gpu_data(), sizeof(float) * 64, cudaMemcpyDeviceToDevice,
-                                   Caffe::stream()));
-      packed_.b_version = bver;
-    }
-    packed_.cout_pad = 64;
+    packed_.update_weights(wb, {PackedParam::CONV1_1, 0, 64, 0, 0, 0, 0}, (size_t)mscnn_conv1_tc_packed_bytes(),
+                           [](const float* w, void* hi, void*) {
+      MSCNN_CHECK(mscnn_pack_conv1_tc_weights(w, hi, 1, Caffe::stream()));
+    });
+    packed_.bias.update(bias, 64, 64);
     typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
-    MSCNN_CHECK(mscnn_conv1_tc_forward(bottom[0]->gpu_data(), packed_.w.hi, packed_.bias, y.hi, split ? y.lo : nullptr,
-                                       N, H, W, fuse_relu_ ? 1 : 0, Caffe::stream()));
+    MSCNN_CHECK(mscnn_conv1_tc_forward(bottom[0]->gpu_data(), packed_.w.hi, packed_.bias.data, y.hi,
+                                       split ? y.lo : nullptr, N, H, W, fuse_relu_ ? 1 : 0, Caffe::stream()));
     return;
   }
-  ensure_packed_conv(&packed_, this->blobs_[0].get(), bias, split, num_output_, channels_, kernel_h_, kernel_w_);
+  const int cout_pad = out_pad(num_output_), cin_pad = pad64(channels_);
+  const size_t bytes = (size_t)cout_pad * kernel_h_ * kernel_w_ * cin_pad * 2;
+  packed_.update_weights(wb, {PackedParam::CONV, split, cout_pad, cin_pad, 0, 0, 0}, bytes,
+                         [&](const float* w, void* hi, void* lo) {
+    MSCNN_CHECK(mscnn_pack_conv_weights(w, hi, lo, num_output_, channels_, kernel_h_, kernel_w_, cout_pad, cin_pad,
+                                        Caffe::stream()));
+  });
+  packed_.bias.update(bias, num_output_, cout_pad);
   typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
-  d.x_hi = x.hi;
-  d.x_lo = x.lo;
-  d.C = x.cpad;
-  d.KH = kernel_h_;
-  d.KW = kernel_w_;
-  d.pad_h = pad_h_;
-  d.pad_w = pad_w_;
-  d.N = N; d.H = H; d.W = W;
-  d.w_hi = packed_.w.hi;
-  d.w_lo = split ? packed_.w.lo : nullptr;
-  d.bias = packed_.bias;
-  d.Cout = num_output_;
-  d.Cout_pad = packed_.cout_pad;
+  mscnn_conv_desc d = conv_desc(x, packed_, N, H, W, x.cpad, num_output_, kernel_h_, kernel_w_, pad_h_, pad_w_,
+                                this->dyn_rows_device());
   d.relu = fuse_relu_ ? 1 : 0;
-  if (packed_.cout_pad % 64 == 0) {
+  if (cout_pad % 64 == 0) {
     d.out_mode = MSCNN_OUT_NHWC_BF16;
     const int ho = top[0]->height(), wo = top[0]->width();
     const bool pool_here = fused_pool_ && (ho % 2 == 0) && (wo % 2 == 0);
@@ -266,7 +233,6 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
     d.out_mode = MSCNN_OUT_NCHW_F32;  // narrow heads (LFCN_*): straight into the Caffe layout
     d.y_f32 = top[0]->mutable_gpu_data();
   }
-  d.dyn_n = this->dyn_rows_device();
   MSCNN_CHECK(mscnn_conv_forward(&d, Caffe::stream()));
 }
 
@@ -464,43 +430,13 @@ void InnerProductLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, c
   const int C = bottom[0]->LegacyShape(1), H = bottom[0]->LegacyShape(2), W = bottom[0]->LegacyShape(3);
   typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
   const int nout_pad = out_pad(N_);
-  const long key = ((long)C << 32) | ((long)H << 16) | W;
-  Blob<Dtype>* wb = this->blobs_[0].get();
-  if (packed_.w_version != wb->version() || packed_.split != split || packed_.key != key ||
-      packed_.cout_pad != nout_pad) {
-    const size_t bytes = (size_t)nout_pad * H * W * x.cpad * 2;
-    packed_.w.reserve(bytes, split);
-    MSCNN_CHECK(mscnn_pack_fc_weights(wb->gpu_data(), packed_.w.hi, split ? packed_.w.lo : nullptr, N_, C, H, W,
-                                      nout_pad, x.cpad, Caffe::stream()));
-    packed_.w_version = wb->version();
-    packed_.split = split;
-    packed_.key = key;
-  }
-  Blob<Dtype>* bb = bias_term_ ? this->blobs_[1].get() : nullptr;
-  const unsigned long bver = bb ? bb->version() : 0;
-  if (!packed_.bias || packed_.cout_pad != nout_pad || packed_.b_version != bver) {
-    if (packed_.bias && packed_.cout_pad != nout_pad) { CUDA_CHECK(cudaFree(packed_.bias)); packed_.bias = nullptr; }
-    if (!packed_.bias) CUDA_CHECK(cudaMalloc(&packed_.bias, sizeof(float) * nout_pad));
-    CUDA_CHECK(cudaMemsetAsync(packed_.bias, 0, sizeof(float) * nout_pad, Caffe::stream()));
-    if (bb)
-      CUDA_CHECK(cudaMemcpyAsync(packed_.bias, bb->gpu_data(), sizeof(float) * N_, cudaMemcpyDeviceToDevice,
-                                 Caffe::stream()));
-    packed_.b_version = bver;
-  }
-  packed_.cout_pad = nout_pad;
-
-  mscnn_conv_desc d;
-  memset(&d, 0, sizeof(d));
-  d.x_hi = x.hi;
-  d.x_lo = x.lo;
-  d.N = M_; d.H = 1; d.W = 1;
-  d.C = H * W * x.cpad;  // NHWC flattening of the bottom
-  d.w_hi = packed_.w.hi;
-  d.w_lo = split ? packed_.w.lo : nullptr;
-  d.bias = packed_.bias;
-  d.Cout = N_;
-  d.Cout_pad = nout_pad;
-  d.KH = d.KW = 1;
+  packed_.update_weights(this->blobs_[0].get(), {PackedParam::FC, split, nout_pad, x.cpad, C, H, W},
+                         (size_t)nout_pad * H * W * x.cpad * 2, [&](const float* w, void* hi, void* lo) {
+    MSCNN_CHECK(mscnn_pack_fc_weights(w, hi, lo, N_, C, H, W, nout_pad, x.cpad, Caffe::stream()));
+  });
+  packed_.bias.update(bias_term_ ? this->blobs_[1].get() : nullptr, N_, nout_pad);
+  // the NHWC flattening of the bottom is the channel vector of a 1 x 1 "image"
+  mscnn_conv_desc d = conv_desc(x, packed_, M_, 1, 1, H * W * x.cpad, N_, 1, 1, 0, 0, this->dyn_rows_device());
   d.relu = fuse_relu_ ? 1 : 0;
   if (nout_pad % 64 == 0) {
     typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
@@ -511,7 +447,6 @@ void InnerProductLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, c
     d.out_mode = MSCNN_OUT_NCHW_F32;  // cls_pred / bbox_pred: [R][N_] fp32, the Caffe layout
     d.y_f32 = top[0]->mutable_gpu_data();
   }
-  d.dyn_n = this->dyn_rows_device();
   MSCNN_CHECK(mscnn_conv_forward(&d, Caffe::stream()));
 }
 

@@ -322,28 +322,6 @@ void Net<Dtype>::FuseLayers() {
     }
     cat->set_fused(true);
   }
-  // (b') ROIPooling whose ROI list descends from a BoxOutput layer (through Split / DecodeBBox, which keep the row
-  // order and the per-image counts): the layer may ask that BoxOutput for the per-image row counts on the device, a
-  // scheduling hint for the gather kernel (mscnn_roi_pool_multi_forward's image_rows).
-  for (int i = 0; i < L; ++i) {
-    ROIPoolingLayer<Dtype>* rp = dynamic_cast<ROIPoolingLayer<Dtype>*>(layers_[i].get());
-    if (!rp || bottom_id_vecs_[i].size() < 2) continue;
-    int blob_id = bottom_id_vecs_[i][1];
-    for (int hops = 0; hops < 16 && blob_id >= 0; ++hops) {
-      int writer = -1;
-      for (int k = 0; k < i && writer < 0; ++k)
-        for (size_t t = 0; t < top_id_vecs_[k].size(); ++t)
-          if (top_id_vecs_[k][t] == blob_id) writer = k;
-      if (writer < 0) break;
-      if (BoxOutputLayer<Dtype>* box = dynamic_cast<BoxOutputLayer<Dtype>*>(layers_[writer].get())) {
-        rp->set_rows_source(box);
-        break;
-      }
-      if (dynamic_cast<SplitLayer<Dtype>*>(layers_[writer].get())) blob_id = bottom_id_vecs_[writer][0];
-      else if (dynamic_cast<DecodeBBoxLayer<Dtype>*>(layers_[writer].get())) blob_id = bottom_id_vecs_[writer][1];
-      else break;
-    }
-  }
 }
 
 // (c) a 2x2 / stride-2 MAX Pooling whose bottom was written by a Convolution (possibly through its
