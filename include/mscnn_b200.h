@@ -336,6 +336,43 @@ MSCNN_API int mscnn_cascade_detect_postprocess_sized(const mscnn_detect_cfg* cfg
                                                      const int* num_rois, void* workspace, size_t workspace_bytes,
                                                      float* dets, int* det_counts, const float* geom, void* stream);
 
+/* Final detections for several classes in one post-process, as the KITTI pedestrian / cyclist driver loops over
+ * cls_ids = [2 3] (examples/kitti_ped_cyc/run_mscnn_detection.m:48,93-121), with the WIDER drivers' detection
+ * threshold (examples/widerface/run_mscnn_detection.m:139-143: keep prob >= det_thr before bbNms when det_thr > 0).
+ * The pipeline runs over N x num_ids slots, slot n * num_ids + c = image n with class cls_ids[c]; each slot's result
+ * equals bit for bit the single-class entry's with cls_id = cls_ids[c] (and, with det_thr > 0, that result without its
+ * rows of prob < det_thr: greedy NMS only lets a box suppress lower-ranked ones).
+ *   dets fp32 [N][num_ids][max_rois_per_image][5], det_counts int[N][num_ids]; geom NULL (the cfg's ratio_* / org_*)
+ *   or HOST [N][4] as in the *_sized entries.  cfg->cls_id is ignored.
+ *   _packed: the payload layout above over N * num_ids slots, mscnn_detect_payload_floats(N * num_ids, cap) floats.
+ *   Workspace: mscnn_detect_classes_workspace_bytes (= the single-class plan of N * num_ids images).
+ * Every argument is checked on the host before any CUDA call: num_ids outside 1..MSCNN_MAX_DETECT_CLASSES, an id
+ * outside 1..cfg->num_cls, repeated ids, a non-finite det_thr or N outside 1..1024 return MSCNN_ERR_INVALID. */
+#define MSCNN_MAX_DETECT_CLASSES 8
+typedef struct mscnn_detect_classes {
+  int num_ids;                           /* 1..MSCNN_MAX_DETECT_CLASSES */
+  int cls_ids[MSCNN_MAX_DETECT_CLASSES]; /* 1-based, distinct, each <= cfg->num_cls; output order = this order */
+  float det_thr;                         /* > 0: keep prob >= det_thr before NMS; <= 0: off (the drivers' -1) */
+} mscnn_detect_classes;
+MSCNN_API int mscnn_detect_classes_workspace_bytes(const mscnn_detect_cfg* cfg, int N,
+                                                   const mscnn_detect_classes* classes, size_t* bytes);
+MSCNN_API int mscnn_detect_postprocess_classes(const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes, int N,
+                                               const float* proposals_score, const float* cls_pred,
+                                               const float* bbox_pred, const int* num_rois, void* workspace,
+                                               size_t workspace_bytes, float* dets, int* det_counts,
+                                               const float* geom, void* stream);
+MSCNN_API int mscnn_cascade_detect_postprocess_classes(const mscnn_detect_cfg* cfg,
+                                                       const mscnn_detect_classes* classes, int N,
+                                                       const float* proposals, const float* cls_prob,
+                                                       const float* output_bbox, const int* num_rois, void* workspace,
+                                                       size_t workspace_bytes, float* dets, int* det_counts,
+                                                       const float* geom, void* stream);
+MSCNN_API int mscnn_detect_postprocess_classes_packed(const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes,
+                                                      int N, const float* proposals_score, const float* cls_pred,
+                                                      const float* bbox_pred, const int* num_rois, void* workspace,
+                                                      size_t workspace_bytes, float* payload, const float* geom,
+                                                      void* stream);
+
 /* ------------------------------------------------------------------------------------
  * Image pre-processing (the step in front of the path, SURVEY.md 8(f)-3).  Replaces the MATLAB code
  * before net.forward in examples/kitti_car/run_mscnn_detection.m:64-69 and
@@ -487,6 +524,18 @@ MSCNN_API int mscnn_net_detect(void* net, const mscnn_detect_cfg* cfg, float* de
 MSCNN_API int mscnn_net_detect_cascade(void* net, const mscnn_detect_cfg* cfg, const char* proposals_blob,
                              const char* cls_prob_blob, const char* output_bbox_blob, float* dets_dev,
                              int* det_counts_dev);
+/* Several classes of the last forward in one post-process (mscnn_detect_postprocess_classes): dets_dev
+ * [N][num_ids][max_rois_per_image][5], det_counts_dev [N][num_ids], the last forward's per-image geometry applied per
+ * slot.  _push: packed over N * num_ids slots into an exchange created with mscnn_detect_payload_floats(N * num_ids,
+ * cap) floats per rank (any other size is refused). */
+MSCNN_API int mscnn_net_detect_classes(void* net, const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes,
+                                       float* dets_dev, int* det_counts_dev);
+MSCNN_API int mscnn_net_detect_cascade_classes(void* net, const mscnn_detect_cfg* cfg,
+                                               const mscnn_detect_classes* classes, const char* proposals_blob,
+                                               const char* cls_prob_blob, const char* output_bbox_blob,
+                                               float* dets_dev, int* det_counts_dev);
+MSCNN_API int mscnn_net_detect_push_classes(void* net, const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes,
+                                            void* xchg);
 
 
 /* ------------------------------------------------------------------------------------

@@ -71,6 +71,27 @@ class DetectCfg(C.Structure):
     ]
 
 
+MAX_DETECT_CLASSES = 8
+
+
+class DetectClasses(C.Structure):
+    """mscnn_detect_classes: the classes of one post-process call (1-based ids, output order) and the detection
+    threshold (> 0: keep prob >= det_thr before NMS; <= 0: off)."""
+    _fields_ = [("num_ids", c_int), ("cls_ids", c_int * MAX_DETECT_CLASSES), ("det_thr", c_float)]
+
+    @classmethod
+    def of(cls, cls_ids, det_thr: float = -1.0) -> "DetectClasses":
+        k = cls()
+        ids = list(cls_ids)
+        if len(ids) > MAX_DETECT_CLASSES:
+            raise MscnnError(f"at most {MAX_DETECT_CLASSES} classes per post-process, got {len(ids)}")
+        k.num_ids = len(ids)
+        for i, v in enumerate(ids):
+            k.cls_ids[i] = int(v)
+        k.det_thr = float(det_thr)
+        return k
+
+
 class PreprocessDesc(C.Structure):
     _fields_ = [("in_h", c_int), ("in_w", c_int), ("out_h", c_int), ("out_w", c_int), ("mean", c_float * 3),
                 ("swap_rb", c_int)]
@@ -173,6 +194,18 @@ def _declare(L: C.CDLL) -> None:
         [C.c_size_t] + [c_void_p] * 3
     L.mscnn_detect_image_geometry.restype = c_int
     L.mscnn_detect_image_geometry.argtypes = [c_int, c_int, c_int, c_void_p, c_void_p]
+    L.mscnn_detect_payload_floats.restype = C.c_size_t
+    L.mscnn_detect_payload_floats.argtypes = [c_int, c_int]
+    L.mscnn_detect_classes_workspace_bytes.restype = c_int
+    L.mscnn_detect_classes_workspace_bytes.argtypes = [C.POINTER(DetectCfg), c_int, C.POINTER(DetectClasses),
+                                                       C.POINTER(C.c_size_t)]
+    for f in ("mscnn_detect_postprocess_classes", "mscnn_cascade_detect_postprocess_classes"):
+        getattr(L, f).restype = c_int
+        getattr(L, f).argtypes = [C.POINTER(DetectCfg), C.POINTER(DetectClasses), c_int] + [c_void_p] * 5 + \
+            [C.c_size_t] + [c_void_p] * 4
+    L.mscnn_detect_postprocess_classes_packed.restype = c_int
+    L.mscnn_detect_postprocess_classes_packed.argtypes = [C.POINTER(DetectCfg), C.POINTER(DetectClasses), c_int] + \
+        [c_void_p] * 5 + [C.c_size_t] + [c_void_p] * 3
 
 
     L.mscnn_preprocess_create.restype = c_int

@@ -20,6 +20,7 @@
 #include <math.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 
 #include "mscnn_b200.h"
 #include "launch_count.h"
@@ -409,23 +410,32 @@ __global__ void box_finalize_kernel(const float4* __restrict__ boxes, const floa
 // (examples/kitti_car/run_mscnn_detection.m:75-120 + utils/bbNms.m:112-126 nmsMax 'maxg').
 // MATLAB evaluates the decode in single precision (matcaffe returns single, and single op double
 // yields single) and the NMS in double on the converted singles; so do these kernels.
+// The post-process runs over class SLOTS: slot s = n * num_ids + c is image n with class cls_ids[c] (image-major, so
+// the per-slot outputs of N images x C classes read as [N][C] and the packed payload keeps its layout over N * C
+// slots).  The single-class entries pass one id and det_thr <= 0.
 struct DetectParams {
-  int num_cls, cls_id;  // cls_id is 1-based like the MATLAB script
+  int num_cls;
+  int num_ids;
+  int cls_ids[MSCNN_MAX_DETECT_CLASSES];  // 1-based like the MATLAB scripts
+  float det_thr;                          // rows with prob < det_thr are dropped before the sort; -inf when off
   float mean[4], stdv[4];
   float proposal_thr;
 };
 
-// Per-image geometry [ratio_h, ratio_w, org_h, org_w] of the images n0, n0 + 1, ... of one launch (one CTA each), by
+// Per-image geometry [ratio_h, ratio_w, org_h, org_w] of the slots s0, s0 + 1, ... of one launch (one CTA each), by
 // value in the kernel parameter block (1 KB).  The MATLAB drivers read each frame's size inside their loop
 // (run_mscnn_detection.m:64-65, run_cascademscnn.m:77-80); a batch without per-image sizes repeats the cfg's four.
 constexpr int kGeomPerLaunch = 64;
 struct DetectGeom {
-  int n0;
+  int s0;
   float4 g[kGeomPerLaunch];
 };
 
-// One CTA per image: decode every ROI of the image, rank by probability (MATLAB sort 'descend'
-// is stable: ties keep the lower row first), leave boxes sorted in `sboxes` / `sscores`.
+// One CTA per slot: decode every ROI of the slot's image for the slot's class, rank by probability (MATLAB sort
+// 'descend' is stable: ties keep the lower row first), leave boxes sorted in `sboxes` / `sscores`.  With det_thr > 0
+// rows below it are dropped first, as the WIDER drivers do before bbNms (examples/widerface/run_mscnn_detection.m:
+// 139-143): 'maxg' NMS only lets a box suppress boxes ranked after it, and every row below the threshold ranks after
+// every row at or above it, so dropping them before NMS equals dropping them from the unthresholded result.
 // CASCADE = false: MS-CNN driver (run_mscnn_detection.m:75-116): prop = proposals_score [R][6],
 //   cls = cls_pred logits [R][num_cls], bbox = bbox_pred deltas [R][4 num_cls].
 // CASCADE = true: cascade driver (examples/kitti_car/run_cascademscnn.m:99-126): prop = the stage's
@@ -442,7 +452,12 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
                           int* __restrict__ counts) {
   extern __shared__ unsigned long long sk[];
   __shared__ int s_valid;
-  const int n = geom.n0 + blockIdx.x, tid = threadIdx.x;
+  const int s = geom.s0 + blockIdx.x, tid = threadIdx.x;
+  const int n = s / p.num_ids, c = s - n * p.num_ids;
+  int id = p.cls_ids[0] - 1;
+#pragma unroll
+  for (int k = 1; k < MSCNN_MAX_DETECT_CLASSES; ++k)  // static indices: the ids stay in the parameter bank
+    if (c == k) id = p.cls_ids[k] - 1;
   const float4 gn = geom.g[blockIdx.x];
   const float ratio_h = gn.x, ratio_w = gn.y, org_h = gn.z, org_w = gn.w;
   int start = 0;
@@ -452,7 +467,6 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
   if (tid == 0) s_valid = 0;
   for (int i = tid; i < Kpad; i += kTopkThreads) sk[i] = 0ull;
   __syncthreads();
-  const int id = p.cls_id - 1;
   for (int i = tid; i < cnt; i += kTopkThreads) {
     if (CASCADE) {
       const float* q = prop + (size_t)(start + i) * 5;
@@ -465,7 +479,8 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
       const float w = x2 - x1 + 1.f, h = y2 - y1 + 1.f;                                                    // :106
       const float prob = cls[(size_t)(start + i) * p.num_cls + id];
       if (prob != prob) continue;  // bbNms: kp = bbs(:,5) > -inf drops NaN
-      dboxes[(size_t)n * Kpad + i] = make_float4(x1, y1, w, h);
+      if (prob < p.det_thr) continue;  // widerface/run_cascademscnn.m:130-131
+      dboxes[(size_t)s * Kpad + i] = make_float4(x1, y1, w, h);
       sk[i] = ((unsigned long long)float_orderable(prob) << 32) | (unsigned int)(0xFFFFFFFFu - (unsigned)i);
       atomicAdd(&s_valid, 1);
       continue;
@@ -493,7 +508,8 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
     tx = fmaxf(0.f, tx); ty = fmaxf(0.f, ty);
     tw = fminf(tw, org_w - tx); th = fminf(th, org_h - ty);
     if (prob != prob) continue;  // bbNms: kp = bbs(:,5) > -inf drops NaN
-    dboxes[(size_t)n * Kpad + i] = make_float4(tx, ty, tw, th);
+    if (prob < p.det_thr) continue;  // widerface/run_mscnn_detection.m:139-143
+    dboxes[(size_t)s * Kpad + i] = make_float4(tx, ty, tw, th);
     sk[i] = ((unsigned long long)float_orderable(prob) << 32) | (unsigned int)(0xFFFFFFFFu - (unsigned)i);
     atomicAdd(&s_valid, 1);
   }
@@ -503,10 +519,10 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
   for (int i = tid; i < M; i += kTopkThreads) {
     const unsigned long long k = sk[i];
     const unsigned int src = 0xFFFFFFFFu - (unsigned int)(k & 0xFFFFFFFFull);
-    sboxes[(size_t)n * Kpad + i] = dboxes[(size_t)n * Kpad + src];
-    sscores[(size_t)n * Kpad + i] = orderable_float((uint32_t)(k >> 32));
+    sboxes[(size_t)s * Kpad + i] = dboxes[(size_t)s * Kpad + src];
+    sscores[(size_t)s * Kpad + i] = orderable_float((uint32_t)(k >> 32));
   }
-  if (tid == 0) counts[n] = M;
+  if (tid == 0) counts[s] = M;
 }
 
 // dets[n][r] = [x y w h prob], r < det_counts[n], in kept (score-descending) order.
@@ -770,30 +786,56 @@ static DetWs plan_det_ws(int N, int Kpad) {
 }
 }  // namespace mscnn
 
-static int det_cfg_check(const mscnn_detect_cfg* c, int N, int* Kpad) {
-  if (!c || N <= 0 || N > 1024 || c->num_cls < 2 || c->cls_id < 1 || c->cls_id > c->num_cls)
-    return MSCNN_ERR_INVALID;
+// The class set of the single-class entries: cfg->cls_id, no detection threshold.
+static mscnn_detect_classes single_class(const mscnn_detect_cfg* c) {
+  mscnn_detect_classes k;
+  memset(&k, 0, sizeof(k));
+  k.num_ids = 1;
+  k.cls_ids[0] = c ? c->cls_id : 0;
+  k.det_thr = -1.f;
+  return k;
+}
+
+// cfg, N and the class set (cfg->cls_id is not read: the single-class entries pass it as the set's one id).
+static int det_cfg_check(const mscnn_detect_cfg* c, const mscnn_detect_classes* k, int N, int* Kpad) {
+  if (!c || !k || N <= 0 || N > 1024 || c->num_cls < 2) return MSCNN_ERR_INVALID;
   if (c->max_rois_per_image <= 0 || c->max_rois_per_image > 8192) return MSCNN_ERR_INVALID;
+  if (k->num_ids < 1 || k->num_ids > MSCNN_MAX_DETECT_CLASSES || !isfinite(k->det_thr)) return MSCNN_ERR_INVALID;
+  for (int i = 0; i < k->num_ids; ++i) {
+    if (k->cls_ids[i] < 1 || k->cls_ids[i] > c->num_cls) return MSCNN_ERR_INVALID;
+    for (int j = 0; j < i; ++j)
+      if (k->cls_ids[j] == k->cls_ids[i]) return MSCNN_ERR_INVALID;
+  }
   *Kpad = next_pow2(c->max_rois_per_image);
   return MSCNN_OK;
 }
 
 extern "C" int mscnn_detect_workspace_bytes(const mscnn_detect_cfg* cfg, int N, size_t* bytes) {
+  const mscnn_detect_classes one = single_class(cfg);
+  return mscnn_detect_classes_workspace_bytes(cfg, N, &one, bytes);
+}
+
+extern "C" int mscnn_detect_classes_workspace_bytes(const mscnn_detect_cfg* cfg, int N,
+                                                    const mscnn_detect_classes* classes, size_t* bytes) {
   int Kpad;
-  const int rc = det_cfg_check(cfg, N, &Kpad);
+  const int rc = det_cfg_check(cfg, classes, N, &Kpad);
   if (rc) return rc;
   if (!bytes) return MSCNN_ERR_INVALID;
-  *bytes = plan_det_ws(N, Kpad).total;
+  *bytes = plan_det_ws(N * classes->num_ids, Kpad).total;
   return MSCNN_OK;
 }
 
-int mscnn::detect_postprocess(bool cascade, const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
-                              const float* cls_pred, const float* bbox_pred, const int* num_rois, void* workspace,
-                              size_t workspace_bytes, const float* geom, const DetectOut& out, void* stream_v) {
+int mscnn::detect_postprocess(bool cascade, const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes, int N,
+                              const float* proposals_score, const float* cls_pred, const float* bbox_pred,
+                              const int* num_rois, void* workspace, size_t workspace_bytes, const float* geom,
+                              const DetectOut& out, void* stream_v) {
   cudaStream_t stream = (cudaStream_t)stream_v;
+  const mscnn_detect_classes one = single_class(cfg);
+  if (!classes) classes = &one;
   int Kpad;
-  const int rc = det_cfg_check(cfg, N, &Kpad);
+  const int rc = det_cfg_check(cfg, classes, N, &Kpad);
   if (rc) return rc;
+  const int C = classes->num_ids, S = N * C;  // class slots, image-major
   if (!proposals_score || !cls_pred || !bbox_pred || !num_rois || !workspace) return MSCNN_ERR_INVALID;
   if (out.push) {
     if (out.push->count < 1 || out.push->count > kMaxPushRanks || !out.done_counter) return MSCNN_ERR_INVALID;
@@ -803,12 +845,15 @@ int mscnn::detect_postprocess(bool cascade, const mscnn_detect_cfg* cfg, int N, 
   if (geom)
     for (int k = 0; k < 4 * N; ++k)
       if (!(geom[k] > 0.f) || geom[k] == INFINITY) return MSCNN_ERR_INVALID;
-  const DetWs w = plan_det_ws(N, Kpad);
+  const DetWs w = plan_det_ws(S, Kpad);
   if (workspace_bytes < w.total) return MSCNN_ERR_NOMEM;
   char* ws = (char*)workspace;
   DetectParams p;
+  memset(&p, 0, sizeof(p));
   p.num_cls = cfg->num_cls;
-  p.cls_id = cfg->cls_id;
+  p.num_ids = C;
+  for (int c = 0; c < C; ++c) p.cls_ids[c] = classes->cls_ids[c];
+  p.det_thr = classes->det_thr > 0.f ? classes->det_thr : -INFINITY;  // <= 0: off, as the drivers' -1
   for (int k = 0; k < 4; ++k) { p.mean[k] = cfg->bbox_mean[k]; p.stdv[k] = cfg->bbox_std[k]; }
   p.proposal_thr = cfg->proposal_thr;
   float4* dboxes = (float4*)(ws + w.dboxes);
@@ -825,14 +870,15 @@ int mscnn::detect_postprocess(bool cascade, const mscnn_detect_cfg* cfg, int N, 
     e = cudaFuncSetAttribute(detect_decode_sort_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)smem);
   if (e != cudaSuccess) return MSCNN_ERR_CUDA;
-  for (int n0 = 0; n0 < N; n0 += kGeomPerLaunch) {
-    const int blocks = N - n0 < kGeomPerLaunch ? N - n0 : kGeomPerLaunch;
+  for (int s0 = 0; s0 < S; s0 += kGeomPerLaunch) {
+    const int blocks = S - s0 < kGeomPerLaunch ? S - s0 : kGeomPerLaunch;
     DetectGeom g;
-    g.n0 = n0;
-    for (int i = 0; i < blocks; ++i)
-      g.g[i] = geom ? make_float4(geom[4 * (n0 + i)], geom[4 * (n0 + i) + 1], geom[4 * (n0 + i) + 2],
-                                  geom[4 * (n0 + i) + 3])
+    g.s0 = s0;
+    for (int i = 0; i < blocks; ++i) {
+      const int n = (s0 + i) / C;
+      g.g[i] = geom ? make_float4(geom[4 * n], geom[4 * n + 1], geom[4 * n + 2], geom[4 * n + 3])
                     : make_float4(cfg->ratio_h, cfg->ratio_w, cfg->org_h, cfg->org_w);
+    }
     mscnn::note_launch();
     if (cascade)
       detect_decode_sort_kernel<true><<<blocks, kTopkThreads, smem, stream>>>(p, g, proposals_score, cls_pred, bbox_pred,
@@ -845,22 +891,22 @@ int mscnn::detect_postprocess(bool cascade, const mscnn_detect_cfg* cfg, int N, 
   }
   const int words = Kpad / 64;
   mscnn::note_launch();
-  nms_mask_kernel<<<dim3(words, words, N), 64, 0, stream>>>(sboxes, counts, Kpad, words,
+  nms_mask_kernel<<<dim3(words, words, S), 64, 0, stream>>>(sboxes, counts, Kpad, words,
                                                            BbNmsTest{(double)cfg->nms_overlap}, mask);
   const size_t scan_smem = (size_t)2 * 64 * words * 8;
   e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_smem);
   if (e != cudaSuccess) return MSCNN_ERR_CUDA;
   mscnn::note_launch();
-  nms_scan_kernel<<<N, kScanThreads, scan_smem, stream>>>(mask, counts, Kpad, words, 0, keep_idx, keep_count);
+  nms_scan_kernel<<<S, kScanThreads, scan_smem, stream>>>(mask, counts, Kpad, words, 0, keep_idx, keep_count);
   mscnn::note_launch();
   if (out.push)
-    detect_push_packed_kernel<<<N, 256, 0, stream>>>(sboxes, sscores, keep_idx, keep_count, Kpad,
-                                                    cfg->max_rois_per_image, N, *out.push, out.seq, out.done_counter);
+    detect_push_packed_kernel<<<S, 256, 0, stream>>>(sboxes, sscores, keep_idx, keep_count, Kpad,
+                                                    cfg->max_rois_per_image, S, *out.push, out.seq, out.done_counter);
   else if (out.payload)
-    detect_write_packed_kernel<<<N, 256, 0, stream>>>(sboxes, sscores, keep_idx, keep_count, Kpad,
-                                                     cfg->max_rois_per_image, N, out.payload);
+    detect_write_packed_kernel<<<S, 256, 0, stream>>>(sboxes, sscores, keep_idx, keep_count, Kpad,
+                                                     cfg->max_rois_per_image, S, out.payload);
   else
-    detect_write_kernel<<<N, 256, 0, stream>>>(sboxes, sscores, keep_idx, keep_count, Kpad,
+    detect_write_kernel<<<S, 256, 0, stream>>>(sboxes, sscores, keep_idx, keep_count, Kpad,
                                               cfg->max_rois_per_image, out.dets, out.det_counts);
   e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -874,7 +920,7 @@ extern "C" int mscnn_detect_postprocess(const mscnn_detect_cfg* cfg, int N, cons
                                         const float* cls_pred, const float* bbox_pred, const int* num_rois,
                                         void* workspace, size_t workspace_bytes, float* dets,
                                         int* det_counts, void* stream) {
-  return detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+  return detect_postprocess(false, cfg, nullptr, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
                             nullptr, DetectOut::padded(dets, det_counts), stream);
 }
 
@@ -883,7 +929,7 @@ extern "C" int mscnn_detect_postprocess_sized(const mscnn_detect_cfg* cfg, int N
                                               void* workspace, size_t workspace_bytes, float* dets, int* det_counts,
                                               const float* geom, void* stream) {
   if (!geom) return MSCNN_ERR_INVALID;
-  return detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+  return detect_postprocess(false, cfg, nullptr, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
                             geom, DetectOut::padded(dets, det_counts), stream);
 }
 
@@ -912,7 +958,7 @@ extern "C" int mscnn_detect_postprocess_packed(const mscnn_detect_cfg* cfg, int 
                                                const float* cls_pred, const float* bbox_pred, const int* num_rois,
                                                void* workspace, size_t workspace_bytes, float* payload, void* stream) {
   if (!payload) return MSCNN_ERR_INVALID;
-  return detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+  return detect_postprocess(false, cfg, nullptr, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
                             nullptr, DetectOut::packed(payload), stream);
 }
 
@@ -921,7 +967,7 @@ extern "C" int mscnn_detect_postprocess_packed_sized(const mscnn_detect_cfg* cfg
                                                      const int* num_rois, void* workspace, size_t workspace_bytes,
                                                      float* payload, const float* geom, void* stream) {
   if (!payload || !geom) return MSCNN_ERR_INVALID;
-  return detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
+  return detect_postprocess(false, cfg, nullptr, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes,
                             geom, DetectOut::packed(payload), stream);
 }
 
@@ -929,7 +975,7 @@ extern "C" int mscnn_cascade_detect_postprocess(const mscnn_detect_cfg* cfg, int
                                                 const float* cls_prob, const float* output_bbox,
                                                 const int* num_rois, void* workspace, size_t workspace_bytes,
                                                 float* dets, int* det_counts, void* stream) {
-  return detect_postprocess(true, cfg, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes,
+  return detect_postprocess(true, cfg, nullptr, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes,
                             nullptr, DetectOut::padded(dets, det_counts), stream);
 }
 
@@ -938,6 +984,37 @@ extern "C" int mscnn_cascade_detect_postprocess_sized(const mscnn_detect_cfg* cf
                                                       const int* num_rois, void* workspace, size_t workspace_bytes,
                                                       float* dets, int* det_counts, const float* geom, void* stream) {
   if (!geom) return MSCNN_ERR_INVALID;
-  return detect_postprocess(true, cfg, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes,
+  return detect_postprocess(true, cfg, nullptr, N, proposals, cls_prob, output_bbox, num_rois, workspace, workspace_bytes,
                             geom, DetectOut::padded(dets, det_counts), stream);
+}
+
+// Several classes in one post-process: N x num_ids slots, slot n * num_ids + c = image n, class cls_ids[c].
+extern "C" int mscnn_detect_postprocess_classes(const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes, int N,
+                                                const float* proposals_score, const float* cls_pred,
+                                                const float* bbox_pred, const int* num_rois, void* workspace,
+                                                size_t workspace_bytes, float* dets, int* det_counts,
+                                                const float* geom, void* stream) {
+  if (!classes) return MSCNN_ERR_INVALID;
+  return detect_postprocess(false, cfg, classes, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace,
+                            workspace_bytes, geom, DetectOut::padded(dets, det_counts), stream);
+}
+
+extern "C" int mscnn_cascade_detect_postprocess_classes(const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes,
+                                                        int N, const float* proposals, const float* cls_prob,
+                                                        const float* output_bbox, const int* num_rois, void* workspace,
+                                                        size_t workspace_bytes, float* dets, int* det_counts,
+                                                        const float* geom, void* stream) {
+  if (!classes) return MSCNN_ERR_INVALID;
+  return detect_postprocess(true, cfg, classes, N, proposals, cls_prob, output_bbox, num_rois, workspace,
+                            workspace_bytes, geom, DetectOut::padded(dets, det_counts), stream);
+}
+
+extern "C" int mscnn_detect_postprocess_classes_packed(const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes,
+                                                       int N, const float* proposals_score, const float* cls_pred,
+                                                       const float* bbox_pred, const int* num_rois, void* workspace,
+                                                       size_t workspace_bytes, float* payload, const float* geom,
+                                                       void* stream) {
+  if (!classes || !payload) return MSCNN_ERR_INVALID;
+  return detect_postprocess(false, cfg, classes, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace,
+                            workspace_bytes, geom, DetectOut::packed(payload), stream);
 }

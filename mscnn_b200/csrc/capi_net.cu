@@ -65,11 +65,11 @@ struct DetectInputs {
   const float *prop, *cls, *bbox;
   const float* geom;  // per-image geometry of the last forward, NULL when it had none (= the cfg's scalars)
 };
-// Checks that the box layer and the three input blobs exist and that cfg keeps every proposal, grows the workspace and
-// looks up the last forward's geometry.
-int detect_inputs(NetHandle* h, const mscnn_detect_cfg* cfg, const char* prop, const char* cls, const char* bbox,
-                  DetectInputs* in) {
-  if (!h->box || !cfg || !prop || !cls || !bbox || !h->net->has_blob(prop) || !h->net->has_blob(cls) ||
+// Checks that the box layer and the three input blobs exist and that cfg keeps every proposal, grows the workspace (for
+// N x classes->num_ids slots; classes NULL = cfg->cls_id alone) and looks up the last forward's geometry.
+int detect_inputs(NetHandle* h, const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes, const char* prop,
+                  const char* cls, const char* bbox, DetectInputs* in) {
+  if (!h || !h->box || !cfg || !prop || !cls || !bbox || !h->net->has_blob(prop) || !h->net->has_blob(cls) ||
       !h->net->has_blob(bbox))
     return MSCNN_ERR_INVALID;
   const int N = h->net->input_blobs()[0]->num();
@@ -81,7 +81,8 @@ int detect_inputs(NetHandle* h, const mscnn_detect_cfg* cfg, const char* prop, c
     return MSCNN_ERR_INVALID;
   }
   size_t need = 0;
-  const int rc = mscnn_detect_workspace_bytes(cfg, N, &need);
+  const int rc = classes ? mscnn_detect_classes_workspace_bytes(cfg, N, classes, &need)
+                         : mscnn_detect_workspace_bytes(cfg, N, &need);
   if (rc) return rc;
   if (need > h->det_ws_bytes) {
     if (h->det_ws) cudaFree(h->det_ws);
@@ -450,9 +451,9 @@ int mscnn_net_num_proposals(void* h, int image) {
 int mscnn_net_detect(void* hv, const mscnn_detect_cfg* cfg, float* dets_dev, int* det_counts_dev) {
   NetHandle* h = H(hv);
   DetectInputs in;
-  const int rc = detect_inputs(h, cfg, "proposals_score", "cls_pred", "bbox_pred", &in);
+  const int rc = detect_inputs(h, cfg, nullptr, "proposals_score", "cls_pred", "bbox_pred", &in);
   if (rc) return rc;
-  return mscnn::detect_postprocess(false, cfg, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
+  return mscnn::detect_postprocess(false, cfg, nullptr, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
                                    h->det_ws_bytes, in.geom, mscnn::DetectOut::padded(dets_dev, det_counts_dev),
                                    Caffe::stream());
 }
@@ -462,7 +463,7 @@ int mscnn_net_detect_gather(void* hv, const mscnn_detect_cfg* cfg, void* comm, f
   NetHandle* h = H(hv);
   if (!comm || !payload_all) return MSCNN_ERR_INVALID;
   DetectInputs in;
-  int rc = detect_inputs(h, cfg, "proposals_score", "cls_pred", "bbox_pred", &in);
+  int rc = detect_inputs(h, cfg, nullptr, "proposals_score", "cls_pred", "bbox_pred", &in);
   if (rc) return rc;
   int nranks = 0, rank = 0;
   rc = mscnn_comm_info(comm, &nranks, &rank, nullptr);
@@ -470,7 +471,7 @@ int mscnn_net_detect_gather(void* hv, const mscnn_detect_cfg* cfg, void* comm, f
   const size_t per = mscnn_detect_payload_floats(in.N, cfg->max_rois_per_image);
   rc = mscnn_comm_stream_wait(comm, Caffe::stream());
   if (rc) return rc;
-  rc = mscnn::detect_postprocess(false, cfg, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
+  rc = mscnn::detect_postprocess(false, cfg, nullptr, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
                                  h->det_ws_bytes, in.geom, mscnn::DetectOut::packed(payload_all + (size_t)rank * per),
                                  Caffe::stream());
   if (rc) return rc;
@@ -482,9 +483,9 @@ int mscnn_net_detect_push(void* hv, const mscnn_detect_cfg* cfg, void* xchg) {
   NetHandle* h = H(hv);
   if (!xchg) return MSCNN_ERR_INVALID;
   DetectInputs in;
-  const int rc = detect_inputs(h, cfg, "proposals_score", "cls_pred", "bbox_pred", &in);
+  const int rc = detect_inputs(h, cfg, nullptr, "proposals_score", "cls_pred", "bbox_pred", &in);
   if (rc) return rc;
-  return mscnn::xchg_detect_push(cfg, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
+  return mscnn::xchg_detect_push(cfg, nullptr, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
                                  h->det_ws_bytes, xchg, in.geom, Caffe::stream());
 }
 int mscnn_net_detect_cascade(void* hv, const mscnn_detect_cfg* cfg, const char* proposals_blob,
@@ -492,11 +493,51 @@ int mscnn_net_detect_cascade(void* hv, const mscnn_detect_cfg* cfg, const char* 
                              int* det_counts_dev) {
   NetHandle* h = H(hv);
   DetectInputs in;
-  const int rc = detect_inputs(h, cfg, proposals_blob, cls_prob_blob, output_bbox_blob, &in);
+  const int rc = detect_inputs(h, cfg, nullptr, proposals_blob, cls_prob_blob, output_bbox_blob, &in);
   if (rc) return rc;
   if (h->net->blob_by_name(cls_prob_blob)->channels() != cfg->num_cls) return MSCNN_ERR_INVALID;
-  return mscnn::detect_postprocess(true, cfg, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
+  return mscnn::detect_postprocess(true, cfg, nullptr, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
                                    h->det_ws_bytes, in.geom, mscnn::DetectOut::padded(dets_dev, det_counts_dev),
                                    Caffe::stream());
+}
+// Several classes of the last forward in one post-process: N x num_ids slots, image-major.  The class set is checked
+// before the net is touched.
+int mscnn_net_detect_classes(void* hv, const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes,
+                             float* dets_dev, int* det_counts_dev) {
+  size_t unused = 0;
+  if (!classes || mscnn_detect_classes_workspace_bytes(cfg, 1, classes, &unused) != MSCNN_OK) return MSCNN_ERR_INVALID;
+  NetHandle* h = H(hv);
+  DetectInputs in;
+  const int rc = detect_inputs(h, cfg, classes, "proposals_score", "cls_pred", "bbox_pred", &in);
+  if (rc) return rc;
+  return mscnn::detect_postprocess(false, cfg, classes, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(),
+                                   h->det_ws, h->det_ws_bytes, in.geom,
+                                   mscnn::DetectOut::padded(dets_dev, det_counts_dev), Caffe::stream());
+}
+int mscnn_net_detect_cascade_classes(void* hv, const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes,
+                                     const char* proposals_blob, const char* cls_prob_blob,
+                                     const char* output_bbox_blob, float* dets_dev, int* det_counts_dev) {
+  size_t unused = 0;
+  if (!classes || mscnn_detect_classes_workspace_bytes(cfg, 1, classes, &unused) != MSCNN_OK) return MSCNN_ERR_INVALID;
+  NetHandle* h = H(hv);
+  DetectInputs in;
+  const int rc = detect_inputs(h, cfg, classes, proposals_blob, cls_prob_blob, output_bbox_blob, &in);
+  if (rc) return rc;
+  if (h->net->blob_by_name(cls_prob_blob)->channels() != cfg->num_cls) return MSCNN_ERR_INVALID;
+  return mscnn::detect_postprocess(true, cfg, classes, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(),
+                                   h->det_ws, h->det_ws_bytes, in.geom,
+                                   mscnn::DetectOut::padded(dets_dev, det_counts_dev), Caffe::stream());
+}
+int mscnn_net_detect_push_classes(void* hv, const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes,
+                                  void* xchg) {
+  size_t unused = 0;
+  if (!classes || !xchg || mscnn_detect_classes_workspace_bytes(cfg, 1, classes, &unused) != MSCNN_OK)
+    return MSCNN_ERR_INVALID;
+  NetHandle* h = H(hv);
+  DetectInputs in;
+  const int rc = detect_inputs(h, cfg, classes, "proposals_score", "cls_pred", "bbox_pred", &in);
+  if (rc) return rc;
+  return mscnn::xchg_detect_push(cfg, classes, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
+                                 h->det_ws_bytes, xchg, in.geom, Caffe::stream());
 }
 }

@@ -200,18 +200,25 @@ int mscnn_xchg_wait(void* xv, void* stream) {
 int mscnn_detect_postprocess_push(const mscnn_detect_cfg* cfg, int N, const float* proposals_score, const float* cls_pred,
                                   const float* bbox_pred, const int* num_rois, void* workspace, size_t workspace_bytes,
                                   void* xv, void* stream) {
-  return mscnn::xchg_detect_push(cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace, workspace_bytes, xv,
-                                 nullptr, stream);
+  return mscnn::xchg_detect_push(cfg, nullptr, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace,
+                                 workspace_bytes, xv, nullptr, stream);
 }
 
 }  // extern "C"
 
-int mscnn::xchg_detect_push(const mscnn_detect_cfg* cfg, int N, const float* proposals_score, const float* cls_pred,
-                            const float* bbox_pred, const int* num_rois, void* workspace, size_t workspace_bytes,
-                            void* xv, const float* geom, void* stream) {
+int mscnn::xchg_detect_push(const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes, int N,
+                            const float* proposals_score, const float* cls_pred, const float* bbox_pred,
+                            const int* num_rois, void* workspace, size_t workspace_bytes, void* xv, const float* geom,
+                            void* stream) {
   Xchg* x = static_cast<Xchg*>(xv);
-  if (!x || !cfg) return MSCNN_ERR_INVALID;
-  if (mscnn_detect_payload_floats(N, cfg->max_rois_per_image) != x->per) return MSCNN_ERR_INVALID;
+  if (!x) return MSCNN_ERR_INVALID;
+  // every argument is checked (host only) before the flow-control wait below is queued
+  size_t ws_need = 0;
+  const int crc = classes ? mscnn_detect_classes_workspace_bytes(cfg, N, classes, &ws_need)
+                          : mscnn_detect_workspace_bytes(cfg, N, &ws_need);
+  if (crc != MSCNN_OK) return crc;
+  const int slots = N * (classes ? classes->num_ids : 1);
+  if (mscnn_detect_payload_floats(slots, cfg->max_rois_per_image) != x->per) return MSCNN_ERR_INVALID;
   for (int p = 0; p < x->nranks; ++p)
     if (!x->peer[p]) return MSCNN_ERR_INVALID;  // not connected yet
   const unsigned int seq = x->seq + 1, gen = seq % x->gens;
@@ -228,8 +235,9 @@ int mscnn::xchg_detect_push(const mscnn_detect_cfg* cfg, int N, const float* pro
     t.flag[p] = gen_flags(x->peer[p], x, gen) + x->rank;
   }
   unsigned int* counter = reinterpret_cast<unsigned int*>(x->local + (size_t)x->gens * x->gen_bytes);
-  const int rc = mscnn::detect_postprocess(false, cfg, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace,
-                                           workspace_bytes, geom, mscnn::DetectOut::pushed(&t, seq, counter), stream);
+  const int rc = mscnn::detect_postprocess(false, cfg, classes, N, proposals_score, cls_pred, bbox_pred, num_rois,
+                                           workspace, workspace_bytes, geom, mscnn::DetectOut::pushed(&t, seq, counter),
+                                           stream);
   if (rc == MSCNN_OK) x->seq = seq;
   return rc;
 }

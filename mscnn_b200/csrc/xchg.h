@@ -36,15 +36,17 @@ struct DetectOut {
 };
 
 // The MS-CNN (cascade = false) or cascade (cascade = true) post-process of N images.  geom: HOST [N][4] = ratio_h,
-// ratio_w, org_h, org_w per image, or NULL for the cfg's four scalars.
-int detect_postprocess(bool cascade, const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
-                       const float* cls_pred, const float* bbox_pred, const int* num_rois, void* workspace,
-                       size_t workspace_bytes, const float* geom, const DetectOut& out, void* stream);
+// ratio_w, org_h, org_w per image, or NULL for the cfg's four scalars.  classes: NULL = cfg->cls_id alone without a
+// detection threshold; otherwise the outputs hold N x classes->num_ids slots in image-major order.
+int detect_postprocess(bool cascade, const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes, int N,
+                       const float* proposals_score, const float* cls_pred, const float* bbox_pred, const int* num_rois,
+                       void* workspace, size_t workspace_bytes, const float* geom, const DetectOut& out, void* stream);
 
-// mscnn_detect_postprocess_push with optional per-image geometry (HOST [N][4], NULL = the cfg's scalars): the Net
-// facade's entry.
-int xchg_detect_push(const mscnn_detect_cfg* cfg, int N, const float* proposals_score, const float* cls_pred,
-                     const float* bbox_pred, const int* num_rois, void* workspace, size_t workspace_bytes, void* xchg,
-                     const float* geom, void* stream);
+// mscnn_detect_postprocess_push with optional per-image geometry (HOST [N][4], NULL = the cfg's scalars) and class set
+// (NULL = cfg->cls_id; the exchange must then carry mscnn_detect_payload_floats(N * num_ids, cap) floats per rank):
+// the Net facade's entry.
+int xchg_detect_push(const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes, int N,
+                     const float* proposals_score, const float* cls_pred, const float* bbox_pred, const int* num_rois,
+                     void* workspace, size_t workspace_bytes, void* xchg, const float* geom, void* stream);
 
 }  // namespace mscnn

@@ -64,6 +64,16 @@ def _declare(L):
     L.mscnn_net_detect_cascade.restype = C.c_int
     L.mscnn_net_detect_cascade.argtypes = [C.c_void_p, C.POINTER(capi.DetectCfg), C.c_char_p, C.c_char_p, C.c_char_p,
                                            C.c_void_p, C.c_void_p]
+    L.mscnn_net_detect_classes.restype = C.c_int
+    L.mscnn_net_detect_classes.argtypes = [C.c_void_p, C.POINTER(capi.DetectCfg), C.POINTER(capi.DetectClasses),
+                                           C.c_void_p, C.c_void_p]
+    L.mscnn_net_detect_cascade_classes.restype = C.c_int
+    L.mscnn_net_detect_cascade_classes.argtypes = [C.c_void_p, C.POINTER(capi.DetectCfg),
+                                                   C.POINTER(capi.DetectClasses), C.c_char_p, C.c_char_p, C.c_char_p,
+                                                   C.c_void_p, C.c_void_p]
+    L.mscnn_net_detect_push_classes.restype = C.c_int
+    L.mscnn_net_detect_push_classes.argtypes = [C.c_void_p, C.POINTER(capi.DetectCfg), C.POINTER(capi.DetectClasses),
+                                                C.c_void_p]
     L.mscnn_set_precision.argtypes = [C.c_int]
     L.mscnn_set_stream.argtypes = [C.c_void_p]
     L.mscnn_set_device.argtypes = [C.c_int]
@@ -270,6 +280,29 @@ class Net:
     def detect(self, cfg: capi.DetectCfg, dets_dev_ptr: int, counts_dev_ptr: int) -> None:
         capi.check(self._L.mscnn_net_detect(self._h, cfg, dets_dev_ptr, counts_dev_ptr), "net_detect")
 
+    def detect_classes(self, cfg: capi.DetectCfg, classes: capi.DetectClasses, dets_dev_ptr: int,
+                       counts_dev_ptr: int) -> None:
+        """Final detections of several classes in one post-process (mscnn_net_detect_classes): dets
+        [N][C][max_rois_per_image][5], counts [N][C], slot [n][c] = image n, class classes.cls_ids[c]."""
+        capi.check(self._L.mscnn_net_detect_classes(self._h, cfg, classes, dets_dev_ptr, counts_dev_ptr),
+                   "net_detect_classes")
+
+    def detect_cascade_classes(self, cfg: capi.DetectCfg, classes: capi.DetectClasses, dets_dev_ptr: int,
+                               counts_dev_ptr: int, stage: str = "3rd", cls_prob: str | None = None) -> None:
+        """detect_cascade for several classes: dets [N][C][max_rois_per_image][5], counts [N][C]."""
+        prop = "proposals" if stage == "1st" else f"proposals_{stage}"
+        capi.check(self._L.mscnn_net_detect_cascade_classes(self._h, cfg, classes, prop.encode(),
+                                                            (cls_prob or f"cls_prob_{stage}").encode(),
+                                                            f"output_bbox_{stage}".encode(), dets_dev_ptr,
+                                                            counts_dev_ptr), "net_detect_cascade_classes")
+
+    def detect_push_classes(self, cfg: capi.DetectCfg, classes: capi.DetectClasses, xchg) -> None:
+        """detect_push for several classes: the payload covers N x C slots, so `xchg` must be a
+        parallel.PeerExchange made for batch * C slots (PeerExchange(batch * C, cap, ...))."""
+        from . import parallel
+        parallel._declare_xchg(self._L)
+        capi.check(self._L.mscnn_net_detect_push_classes(self._h, cfg, classes, xchg.handle), "net_detect_push_classes")
+
     def fused_producer(self, layer: str) -> str:
         """The layer that does `layer`'s work (itself unless the fusion pass folded it into another layer)."""
         i = self._L.mscnn_net_fused_producer(self._h, self.layer_names.index(layer))
@@ -320,6 +353,15 @@ def kitti_detect_cfg(net_h: int, net_w: int, max_rois: int = 2000, num_cls: int 
     cfg.org_h, cfg.org_w = float(oh), float(ow)
     cfg.max_rois_per_image = max_rois
     return cfg
+
+
+def kitti_ped_cyc_detect_cfg(net_h: int, net_w: int, max_rois: int = 2000,
+                             org_hw: tuple[int, int] | None = None) -> tuple[capi.DetectCfg, capi.DetectClasses]:
+    """Post-process settings of examples/kitti_ped_cyc/run_mscnn_detection.m:42-51 for the pedestrian / cyclist nets
+    (cls_pred of 3 classes: bg, ped, cyc): the cfg and the class set cls_ids = [2 3] without a detection threshold,
+    for Net.detect_classes.  Slot [n][0] holds the pedestrians, [n][1] the cyclists."""
+    cfg = kitti_detect_cfg(net_h, net_w, max_rois=max_rois, num_cls=3, cls_id=2, org_hw=org_hw)
+    return cfg, capi.DetectClasses.of([2, 3])
 
 
 def image_geometry(net_hw: tuple[int, int], org_hw_list) -> np.ndarray:

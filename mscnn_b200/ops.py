@@ -369,6 +369,55 @@ def detect_postprocess(cfg: capi.DetectCfg, n: int, proposals_score, cls_pred, b
     return _detect("detect_postprocess", cfg, n, (proposals_score, cls_pred, bbox_pred), num_out, geometry)
 
 
+def _detect_classes(entry: str, cfg: capi.DetectCfg, classes: capi.DetectClasses, n: int, inputs, num_out, geometry,
+                    packed: bool = False):
+    """Post-process of several classes through mscnn_<entry>: padded dets [n, C, cap, 5] + counts [n, C], or (packed)
+    the payload over n * C slots."""
+    import ctypes as C
+    dev = inputs[0].device
+    nbytes = C.c_size_t(0)
+    capi.check(capi.lib().mscnn_detect_classes_workspace_bytes(cfg, n, classes, C.byref(nbytes)),
+               "detect_classes_workspace")
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    g = None
+    if geometry is not None:
+        g = np.ascontiguousarray(geometry, dtype=np.float32)
+        assert g.shape == (n, 4), (g.shape, n)
+    head = (cfg, classes, n, *map(capi.ptr, inputs), capi.ptr(num_out), capi.ptr(ws), nbytes.value)
+    if packed:
+        payload = torch.zeros(capi.lib().mscnn_detect_payload_floats(n * classes.num_ids, cfg.max_rois_per_image),
+                              dtype=torch.float32, device=dev)
+        capi.check(getattr(capi.lib(), "mscnn_" + entry)(*head, capi.ptr(payload), capi.ptr(g), _stream()), entry)
+        return payload
+    dets = torch.zeros((n, classes.num_ids, cfg.max_rois_per_image, 5), dtype=torch.float32, device=dev)
+    counts = torch.zeros((n, classes.num_ids), dtype=torch.int32, device=dev)
+    capi.check(getattr(capi.lib(), "mscnn_" + entry)(*head, capi.ptr(dets), capi.ptr(counts), capi.ptr(g), _stream()),
+               entry)
+    return dets, counts
+
+
+def detect_postprocess_classes(cfg: capi.DetectCfg, classes: capi.DetectClasses, n: int, proposals_score, cls_pred,
+                               bbox_pred, num_out, geometry=None):
+    """Final detections of the classes `classes.cls_ids` in one post-process: dets [n][C][cap][5], counts [n][C]
+    (slot [i][c] = image i, class cls_ids[c]); geometry as in detect_postprocess."""
+    return _detect_classes("detect_postprocess_classes", cfg, classes, n, (proposals_score, cls_pred, bbox_pred),
+                           num_out, geometry)
+
+
+def cascade_detect_postprocess_classes(cfg: capi.DetectCfg, classes: capi.DetectClasses, n: int, proposals, cls_prob,
+                                       output_bbox, num_out, geometry=None):
+    """The cascade post-process of several classes: dets [n][C][cap][5], counts [n][C]."""
+    return _detect_classes("cascade_detect_postprocess_classes", cfg, classes, n, (proposals, cls_prob, output_bbox),
+                           num_out, geometry)
+
+
+def detect_postprocess_classes_packed(cfg: capi.DetectCfg, classes: capi.DetectClasses, n: int, proposals_score,
+                                      cls_pred, bbox_pred, num_out, geometry=None) -> torch.Tensor:
+    """detect_postprocess_classes in the exchange's packed layout over n * C slots (mscnn_detect_payload_floats)."""
+    return _detect_classes("detect_postprocess_classes_packed", cfg, classes, n,
+                           (proposals_score, cls_pred, bbox_pred), num_out, geometry, packed=True)
+
+
 def conv1_tc_forward(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None, relu: bool, split: bool) -> Planes:
     """conv1_1 (3 -> 64, 3x3, pad 1) as the single tensor-core kernel: x [N,3,H,W] fp32 NCHW -> planes."""
     n, c, h, wd = x.shape
