@@ -109,6 +109,10 @@ MSCNN_API int mscnn_conv_forward(const mscnn_conv_desc* d, void* stream);
 /* Host-only: the launch plan mscnn_conv_forward would use for `d` as one line of text (kernel instantiation, pixel box,
  * operand staging, pipeline depth); no CUDA call, the pointers only have to be non-NULL. */
 MSCNN_API int mscnn_conv_plan_describe(const mscnn_conv_desc* d, char* buf, int cap);
+/* Host-only: the number of launch plans mscnn_conv_forward holds in its cache (one per distinct descriptor, including
+ * the tensor addresses).  A net that changes input size adds its convolutions' plans once per new shape; the cache is
+ * emptied when it reaches 4096 entries. */
+MSCNN_API int mscnn_conv_plan_count(void);
 
 /* Weight packing (done once at load time; replaces nothing in the reference -- Caffe keeps
  * [Cout][Cin][KH][KW] fp32, blob layout base_conv_layer.cpp:135-142).
@@ -443,6 +447,15 @@ MSCNN_API int mscnn_kitti_write_det_file(const char* path, int N, const float* h
 MSCNN_API int mscnn_kitti_write_labels(const char* car_det_file, const char* ped_det_file, const char* cyc_det_file,
                                        const char* list_path, const char* save_dir, double score_scale);
 MSCNN_API int mscnn_kitti_evaluate(const char* gt_dir, const char* result_dir, const char* list_path, double* ap);
+
+/* WIDER FACE result files (examples/widerface/run_mscnn_detection.m:177-196, run_cascademscnn.m:165-184), host-only:
+ * creates event_dir (and any missing parent) and writes <event_dir>/<image_names[n]>.txt for every image n: the name,
+ * the detection count, then one "%d %d %d %d %f" row per detection = x y w h rounded half away from zero (MATLAB
+ * round), and the probability.  host_dets [N][max_rois_per_image][5] = [x y w h prob] and host_counts [N] are host
+ * copies of a post-process's outputs (one class).  An empty name, a name with '/', a count outside
+ * 0..max_rois_per_image or a non-finite value in a kept row returns MSCNN_ERR_INVALID before anything is created. */
+MSCNN_API int mscnn_widerface_write_results(const char* event_dir, int N, const char* const* image_names,
+                                            const float* host_dets, const int* host_counts, int max_rois_per_image);
 
 /* ------------------------------------------------------------------------------------
  * Net facade: caffe::Net<float> of the Caffe-API mirror (mscnn_b200/csrc/caffe_api) for hosts that

@@ -125,6 +125,8 @@ def _declare(L: C.CDLL) -> None:
     L.mscnn_conv_forward.argtypes = [C.POINTER(ConvDesc), c_void_p]
     L.mscnn_conv_plan_describe.restype = c_int
     L.mscnn_conv_plan_describe.argtypes = [C.POINTER(ConvDesc), C.c_char_p, c_int]
+    L.mscnn_conv_plan_count.restype = c_int
+    L.mscnn_conv_plan_count.argtypes = []
     L.mscnn_pack_conv_weights.restype = c_int
     L.mscnn_pack_conv_weights.argtypes = [c_void_p, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]
     L.mscnn_pack_fc_weights.restype = c_int
@@ -233,6 +235,8 @@ def _declare(L: C.CDLL) -> None:
     L.mscnn_kitti_write_labels.argtypes = [C.c_char_p] * 5 + [C.c_double]
     L.mscnn_kitti_evaluate.restype = c_int
     L.mscnn_kitti_evaluate.argtypes = [C.c_char_p] * 3 + [c_void_p]
+    L.mscnn_widerface_write_results.restype = c_int
+    L.mscnn_widerface_write_results.argtypes = [C.c_char_p, c_int, C.POINTER(C.c_char_p), c_void_p, c_void_p, c_int]
 
 
     L.mscnn_conv1_tc_packed_bytes.restype = c_int

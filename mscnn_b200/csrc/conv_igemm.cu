@@ -835,3 +835,11 @@ extern "C" int mscnn_conv_plan_describe(const mscnn_conv_desc* d, char* buf, int
                          plan.smem, p.dyn_n ? 1 : 0, p.rowshare, p.a_stages);
   return (n > 0 && n < cap) ? MSCNN_OK : MSCNN_ERR_INVALID;
 }
+
+// Entries in the launch-plan cache.  A net adds one per convolution for every new combination of input shape and blob
+// addresses it runs with; the table is emptied when it reaches 4096 entries, so it stays bounded however many input
+// sizes a process goes through.
+extern "C" int mscnn_conv_plan_count(void) {
+  std::lock_guard<std::mutex> lk(mscnn::g_plan_mu);
+  return (int)mscnn::g_plans.size();
+}

@@ -7,12 +7,15 @@
 //                                writeLabels.m record format, which is not part of the reference repository)
 //   mscnn_kitti_evaluate         examples/kitti_result/eval/evaluate_object.cpp:1-784 (the KITTI object
 //                                benchmark's 2-D detection evaluation: 41 recall points, easy/moderate/hard)
+//   mscnn_widerface_write_results  examples/widerface/run_mscnn_detection.m:177-196, run_cascademscnn.m:165-184
+//                                (one <image name>.txt per image of a WIDER FACE event)
 //
 // The evaluator is restated, not transcribed: one pass builds per-image class views (care / ignore / other
 // flags, don't-care boxes), the recall thresholds come from the score list of a no-threshold matching pass, and
 // a second matching pass per threshold accumulates tp / fp / fn.  Floating-point operations are kept in the
 // reference's order so that the written statistics files are byte-identical to the reference tool's
 // (tests/test_kitti_eval.py runs the reference tool, compiled verbatim into oracle/_ref, on the same files).
+#include <errno.h>
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -315,6 +318,41 @@ int mscnn_kitti_write_det_file(const char* path, int N, const float* host_dets, 
               (double)d[3], (double)d[4]);
     }
   fclose(fp);
+  return MSCNN_OK;
+}
+
+int mscnn_widerface_write_results(const char* event_dir, int N, const char* const* image_names, const float* host_dets,
+                                  const int* host_counts, int max_rois_per_image) {
+  // every argument is checked before the file system is touched
+  if (!event_dir || !*event_dir || N < 0 || max_rois_per_image < 1 ||
+      (N > 0 && (!image_names || !host_dets || !host_counts)))
+    return MSCNN_ERR_INVALID;
+  for (int n = 0; n < N; ++n) {
+    if (!image_names[n] || !*image_names[n] || strchr(image_names[n], '/')) return MSCNN_ERR_INVALID;
+    if (host_counts[n] < 0 || host_counts[n] > max_rois_per_image) return MSCNN_ERR_INVALID;
+    for (int k = 0; k < 5 * host_counts[n]; ++k)  // finite and small enough for the integer conversion below
+      if (!(fabs(host_dets[(size_t)n * max_rois_per_image * 5 + k]) < 1e15)) return MSCNN_ERR_INVALID;
+  }
+  // mkdir(comp_id_dir), mkdir(event_dir): every missing directory of the path
+  std::string dir(event_dir);
+  for (size_t i = 1; i <= dir.size(); ++i) {
+    if (i < dir.size() && dir[i] != '/') continue;
+    const std::string part = dir.substr(0, i);
+    if (mkdir(part.c_str(), 0777) != 0 && errno != EEXIST) return MSCNN_ERR_INVALID;
+  }
+  for (int n = 0; n < N; ++n) {
+    const std::string path = dir + "/" + image_names[n] + ".txt";
+    FILE* fp = fopen(path.c_str(), "w");
+    if (!fp) return MSCNN_ERR_INVALID;
+    fprintf(fp, "%s\n%d\n", image_names[n], host_counts[n]);
+    for (int k = 0; k < host_counts[n]; ++k) {
+      const float* d = host_dets + ((size_t)n * max_rois_per_image + k) * 5;
+      // MATLAB round() is half away from zero, as C round(); the integer conversion prints round(-0.4) as 0
+      fprintf(fp, "%lld %lld %lld %lld %f\n", (long long)round((double)d[0]), (long long)round((double)d[1]),
+              (long long)round((double)d[2]), (long long)round((double)d[3]), (double)d[4]);
+    }
+    if (fclose(fp) != 0) return MSCNN_ERR_INVALID;
+  }
   return MSCNN_OK;
 }
 

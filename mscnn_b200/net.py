@@ -364,6 +364,16 @@ def kitti_ped_cyc_detect_cfg(net_h: int, net_w: int, max_rois: int = 2000,
     return cfg, capi.DetectClasses.of([2, 3])
 
 
+def widerface_detect_cfg(net_h: int, net_w: int, max_rois: int = 3000, org_hw: tuple[int, int] | None = None,
+                         det_thr: float = 0.05) -> tuple[capi.DetectCfg, capi.DetectClasses]:
+    """Post-process settings of examples/widerface/run_mscnn_detection.m:36-57 (run_cascademscnn.m:54-67): 2 classes
+    (bg, face), face = class 2 with det_thr 0.05, bbox_stds [.1 .1 .2 .2], NMS overlap 0.3, proposal_thr -5.  The
+    cfg and class set for Net.detect_classes / detect_cascade_classes; max_rois covers BoxOutput's max_nms_num (3000)."""
+    cfg = kitti_detect_cfg(net_h, net_w, max_rois=max_rois, num_cls=2, cls_id=2, org_hw=org_hw)
+    cfg.proposal_thr, cfg.nms_overlap = -5.0, 0.3
+    return cfg, capi.DetectClasses.of([2], det_thr)
+
+
 def image_geometry(net_hw: tuple[int, int], org_hw_list) -> np.ndarray:
     """float32 [N][4] = ratio_h, ratio_w, org_h, org_w per image (mscnn_detect_image_geometry, host only): the
     `geometry=` of ops.detect_postprocess, with the same values kitti_detect_cfg(*net_hw, org_hw=...) stores."""

@@ -81,7 +81,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     args = ap.parse_args()
     import torch
-    from mscnn_b200 import capi, models, net as mnet
+    from mscnn_b200 import models, net as mnet
     torch.cuda.set_device(0)
     mnet.set_device(0)
     side = torch.cuda.Stream()          # a CUDA graph cannot be captured on the legacy default stream
@@ -91,14 +91,7 @@ def main():
     cfg = mnet.kitti_detect_cfg(576, 1920)
     res["config1"] = run("mscnn-7s-576-2x full detection forward, 1x3x576x1920 (BASELINE.json configs[1])",
                          models.kitti(576, 1920, 7, True, batch=1), 576, 1920, 1, cfg, args.steps, args.warmup)
-    wcfg = capi.DetectCfg()
-    wcfg.num_cls, wcfg.cls_id = 2, 2                       # examples/widerface/run_mscnn_detection.m:36-52
-    for k, v in enumerate([0.1, 0.1, 0.2, 0.2]):
-        wcfg.bbox_std[k], wcfg.bbox_mean[k] = v, 0.0
-    wcfg.proposal_thr, wcfg.nms_overlap = -5.0, 0.3
-    wcfg.ratio_h = wcfg.ratio_w = 1.0
-    wcfg.org_h, wcfg.org_w = 768.0, 1024.0
-    wcfg.max_rois_per_image = 3000
+    wcfg, _ = mnet.widerface_detect_cfg(768, 1024)         # net.detect: class 2 alone, without det_thr
     res["config4"] = run("WIDER FACE mscnn-12s-2x forward, 8x3x768x1024 (BASELINE.json configs[4])",
                          models.widerface(768, 1024, batch=8), 768, 1024, 8, wcfg, args.steps, args.warmup)
     print(json.dumps(res))
