@@ -51,6 +51,14 @@ constexpr int kProducerWarps = 4;            // warpgroup 0
 constexpr int kThreads = 32 * kProducerWarps + 256;  // + two MMA / epilogue warpgroups
 constexpr int kEpiThreads = 256;
 constexpr int kEpiBarId = 1;
+// Shared memory, offsets from its 1024-aligned base: the output staging buffers (1024-aligned for the swizzled TMA
+// stores), the resident weights, the pixel-row stages, the bias and the stage barriers; kSmemBytes adds the slack for
+// aligning the base.
+constexpr int kWOff = kEpiBufs * 2 * kEpiPlane;
+constexpr int kAOff = kWOff + 2 * kWPlaneBytes;
+constexpr int kBiasOff = kAOff + kStages * kStageBytes;
+constexpr int kBarOff = kBiasOff + kCout * 4;
+constexpr int kSmemBytes = kBarOff + 16 * kStages + 1024;
 
 struct Params {
   const float* x;     // [N][3][H][W] fp32
@@ -67,17 +75,12 @@ conv_c3_tc_kernel(const __grid_constant__ CUtensorMap tmO_hi, const __grid_const
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
-  const uint32_t sEpi = smem_base;                                   // 1024-aligned staging buffers
+  const uint32_t sEpi = smem_base, sW = smem_base + kWOff, sA = smem_base + kAOff;
   const int epi_buf_bytes = kEpiPlane * (p.split ? 2 : 1);
-  const uint32_t sW = sEpi + kEpiBufs * 2 * kEpiPlane;
-  const uint32_t sA = sW + 2 * kWPlaneBytes;
-  const uint32_t sMisc = sA + kStages * kStageBytes;
-  uint8_t* gW = gen + (sW - smem_base);
-  uint8_t* gA = gen + (sA - smem_base);
-  float* bias_s = reinterpret_cast<float*>(gen + (sMisc - smem_base));
-  const uint32_t sBar = sMisc + kCout * 4;
-  auto full_bar = [&](int s) { return sBar + 8u * s; };
-  auto empty_bar = [&](int s) { return sBar + 8u * (kStages + s); };
+  uint8_t* gW = gen + kWOff;
+  uint8_t* gA = gen + kAOff;
+  float* bias_s = reinterpret_cast<float*>(gen + kBiasOff);
+  ptx::Ring ring(smem_base + kBarOff, kStages);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -92,10 +95,7 @@ conv_c3_tc_kernel(const __grid_constant__ CUtensorMap tmO_hi, const __grid_const
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmO_hi);
     if (p.split) ptx::prefetch_tmap(&tmO_lo);
-    for (int s = 0; s < kStages; ++s) {
-      ptx::mbar_init(full_bar(s), 32);
-      ptx::mbar_init(empty_bar(s), 2);  // one arrival per MMA warpgroup
-    }
+    ring.init(32, 2);  // every lane of the filling producer warp, one arrival per MMA warpgroup
     ptx::fence_mbar_init();
   }
   ptx::fence_proxy_async_smem();
@@ -111,8 +111,7 @@ conv_c3_tc_kernel(const __grid_constant__ CUtensorMap tmO_hi, const __grid_const
     static_assert(kProducerWarps == kStages, "one stage per producer warp");
     constexpr int kItems = 3 * 131;                 // (dy, px) pixels a tile needs
     constexpr int kIters = (kItems + 31) / 32;      // 13
-    const int stage = warp;
-    uint32_t phase = 0;
+    ptx::Ring own(ring.bars + 16u * warp, 1);  // this warp's stage
     for (int tile = blockIdx.x + warp * gridDim.x; tile < total_tiles; tile += kStages * gridDim.x) {
       const int tw = tile % p.tiles_w;
       const int y = (tile / p.tiles_w) % p.H;
@@ -132,8 +131,8 @@ conv_c3_tc_kernel(const __grid_constant__ CUtensorMap tmO_hi, const __grid_const
         for (int c = 0; c < 3; ++c) v[it][c] = ok ? __ldg(q + c * plane) : 0.f;
       }
       // ... then wait for the slot and fill it
-      ptx::mbar_wait(empty_bar(stage), phase ^ 1u);
-      uint8_t* a_hi = gA + stage * kStageBytes;
+      own.wait_empty();
+      uint8_t* a_hi = gA + warp * kStageBytes;
 #pragma unroll
       for (int it = 0; it < kIters; ++it) {
         const int item = it * 32 + lane;
@@ -153,8 +152,8 @@ conv_c3_tc_kernel(const __grid_constant__ CUtensorMap tmO_hi, const __grid_const
         }
       }
       ptx::fence_proxy_async_smem();  // generic-proxy stores -> visible to wgmma operand reads
-      ptx::mbar_arrive(full_bar(stage));
-      phase ^= 1u;
+      ptx::mbar_arrive(own.full_bar());
+      own.advance();
     }
     return;
   }
@@ -172,17 +171,16 @@ conv_c3_tc_kernel(const __grid_constant__ CUtensorMap tmO_hi, const __grid_const
     bias_r[2 * j] = bias_s[8 * j + cq];
     bias_r[2 * j + 1] = bias_s[8 * j + cq + 1];
   }
-  int stage = 0, ebuf = 0;
-  uint32_t phase = 0;
+  int ebuf = 0;
   float acc[kCout / 2];
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int tw = tile % p.tiles_w;
     const int y = (tile / p.tiles_w) % p.H;
     const int n = tile / (p.tiles_w * p.H);
-    ptx::mbar_wait(full_bar(stage), phase);
+    ring.wait_full();
     ptx::wgmma_fence();
     {
-      const uint32_t a_hi = sA + stage * kStageBytes + static_cast<uint32_t>(wg) * 64u * 16u, a_lo = a_hi + kPlaneBytes;
+      const uint32_t a_hi = sA + ring.slot * kStageBytes + static_cast<uint32_t>(wg) * 64u * 16u, a_lo = a_hi + kPlaneBytes;
       const uint32_t w_hi = sW, w_lo = sW + kWPlaneBytes;
       uint32_t accum = 0;
 #pragma unroll
@@ -207,41 +205,21 @@ conv_c3_tc_kernel(const __grid_constant__ CUtensorMap tmO_hi, const __grid_const
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_regs(acc);
-    if (wl == 0) ptx::mbar_arrive(empty_bar(stage));  // the stage's operands have been read
-    if (++stage == kStages) {
-      stage = 0;
-      phase ^= 1u;
-    }
+    if (wl == 0) ptx::mbar_arrive(ring.empty_bar(ring.slot));  // the stage's operands have been read
+    ring.advance();
     if (issuer) ptx::tma_store_wait_read<kEpiBufs - 1>();  // the buffer we are about to overwrite has been read
     ptx::named_bar_sync(kEpiBarId, kEpiThreads);
     const uint32_t buf = sEpi + ebuf * epi_buf_bytes;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {  // 8-channel groups
+    for (int j = 0; j < 8; ++j)  // 8-channel groups
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r0 + 8 * h;
-        float f0 = acc[4 * j + 2 * h] + bias_r[2 * j];
-        float f1 = acc[4 * j + 2 * h + 1] + bias_r[2 * j + 1];
-        if (p.relu) {
-          f0 = fmaxf(f0, 0.f);
-          f1 = fmaxf(f1, 0.f);
-        }
-        // packed conversions (cvt.rn.bf16x2.f32): same rounding as two scalar ones, half the F2F issue slots
-        const __nv_bfloat162 h2 = __floats2bfloat162_rn(f0, f1);
-        const uint32_t hi = *reinterpret_cast<const uint32_t*>(&h2);
-        const __nv_bfloat162 l2 = __floats2bfloat162_rn(f0 - __uint_as_float(hi << 16),
-                                                        f1 - __uint_as_float(hi & 0xFFFF0000u));
-        const uint32_t lo = *reinterpret_cast<const uint32_t*>(&l2);
-        const uint32_t a = buf + row * 128 + static_cast<uint32_t>((j ^ (row & 7)) << 4) + 2u * cq;  // 128B swizzle
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(hi) : "memory");
-        if (p.split) asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + kEpiPlane), "r"(lo) : "memory");
-      }
-    }
+      for (int h = 0; h < 2; ++h)
+        ptx::stage_pair(buf, r0 + 8 * h, j, cq, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], bias_r[2 * j],
+                        bias_r[2 * j + 1], p.relu, p.split, kEpiPlane);
     ptx::fence_proxy_async_smem();
     ptx::named_bar_sync(kEpiBarId, kEpiThreads);
     if (issuer) {
-      ptx::tma_store_4d(&tmO_hi, buf, 0, tw * kTileW, y, n);
-      if (p.split) ptx::tma_store_4d(&tmO_lo, buf + kEpiPlane, 0, tw * kTileW, y, n);
+      ptx::tma_store_hi_lo(&tmO_hi, &tmO_lo, buf, p.split, kEpiPlane, 0, tw * kTileW, y, n);
       ptx::tma_store_commit();
     }
     if (++ebuf == kEpiBufs) ebuf = 0;
@@ -304,8 +282,7 @@ extern "C" int mscnn_conv1_tc_forward(const float* x, const void* packed_w, cons
   } else {
     maps[1] = maps[0];
   }
-  const size_t smem = (size_t)c3::kEpiBufs * 2 * c3::kEpiPlane + 2 * c3::kWPlaneBytes + c3::kStages * c3::kStageBytes +
-                      c3::kCout * 4 + 8 * (2 * c3::kStages) + 1024;
+  const size_t smem = c3::kSmemBytes;
   auto kern = p.split ? c3::conv_c3_tc_kernel<true> : c3::conv_c3_tc_kernel<false>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return MSCNN_ERR_CUDA;

@@ -79,13 +79,27 @@ struct IgemmParams {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;                       // bf16 elements = 128 B = one swizzle row
 constexpr int kABytes = kBlockM * kBlockK * 2;    // 16 KB
+constexpr int kPoolBytes = kABytes / 4;           // pooled tile: 32 rows x 128 B
 constexpr int kThreads = 384;                     // producer warpgroup + two MMA warpgroups
 constexpr int kEpiThreads = 256;
 constexpr int kEpiBarId = 1;
+constexpr int kMaxStages = 8, kMaxAStages = 4;    // deepest B ring and row-share A ring a plan builds
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
-  const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&h2);
+// Shared memory of conv_igemm_kernel<block_n, p.fat>, offsets from its 1024-aligned base: the A slots (their own ring
+// with row-share, else one per stage), the B stages, the epilogue staging buffers and a barrier block sized for the
+// deepest rings.  `total` is what a launch reserves, the slack for aligning the base included.  a_slot and the B tiles
+// are multiples of 1024 B, so every region starts 1024-aligned (128B-swizzled tiles need it).
+struct IgemmLayout {
+  int b, epi, epi_buf, bar, total;
+};
+__host__ __device__ inline IgemmLayout igemm_layout(const IgemmParams& p, int block_n) {
+  IgemmLayout l;
+  l.b = (p.rowshare ? p.a_stages : p.stages) * p.a_slot;
+  l.epi = l.b + p.stages * (p.fat ? 2 : 1) * block_n * kBlockK * 2;
+  l.epi_buf = (kABytes + (p.pool ? kPoolBytes : 0)) * (p.has_lo_out ? 2 : 1);
+  l.bar = l.epi + p.epi_bufs * l.epi_buf;
+  l.total = l.bar + 16 * (kMaxStages + (p.rowshare ? kMaxAStages : 0)) + 1024;
+  return l;
 }
 
 // FAT is a template parameter, not a runtime branch: with both MMA sequences in one body the accumulator registers
@@ -102,25 +116,17 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
                   const __grid_constant__ CUtensorMap tmP_lo, const IgemmParams p) {
   constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   constexpr int kAcc = BLOCK_N / 2;  // fp32 accumulators per thread of an MMA warpgroup
+  constexpr uint32_t kPlanes = FAT ? 2u : 1u;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-
-  const int S = p.stages;
-  const int SA = p.rowshare ? p.a_stages : S;  // A slots: their own ring (row-share) or one per stage
-  const uint32_t a_stride = p.a_slot;                      // [A_hi] or [A_hi][A_lo]
-  const uint32_t b_stride = FAT ? 2u * kBBytes : kBBytes;  // [B_hi] or [B_hi][B_lo]
-  const uint32_t sA = smem_base;
-  const uint32_t sB = sA + SA * a_stride;
-  const uint32_t sEpi = sB + S * b_stride;  // 1024-aligned: a_slot and kBBytes are multiples of 1024
-  constexpr int kPoolBytes = kABytes / 4;  // pooled tile: 32 rows x 128 B
-  const int epi_buf_bytes = (kABytes + (p.pool ? kPoolBytes : 0)) * (p.has_lo_out ? 2 : 1);
-  const uint32_t sBar = sEpi + p.epi_bufs * epi_buf_bytes;
-  // barrier layout: full[S], empty[S], then for row-share a_full[SA], a_empty[SA]
-  auto full_bar = [&](int s) { return sBar + 8u * s; };
-  auto empty_bar = [&](int s) { return sBar + 8u * (S + s); };
-  auto a_full_bar = [&](int s) { return sBar + 8u * (2 * S + s); };
-  auto a_empty_bar = [&](int s) { return sBar + 8u * (2 * S + SA + s); };
+  const IgemmLayout lay = igemm_layout(p, BLOCK_N);
+  const uint32_t a_stride = p.a_slot;                // [A_hi] or [A_hi][A_lo]
+  const uint32_t b_stride = kPlanes * kBBytes;       // [B_hi] or [B_hi][B_lo]
+  const uint32_t sA = smem_base, sB = smem_base + lay.b, sEpi = smem_base + lay.epi;
+  // the B ring (stages; without row-share its slots carry the A tiles too), then the row-share A ring
+  ptx::Ring ring(smem_base + lay.bar, p.stages);
+  ptx::Ring a_ring(smem_base + lay.bar + 16u * p.stages, p.a_stages);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -140,14 +146,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
         if (p.has_lo_out) ptx::prefetch_tmap(&tmP_lo);
       }
     }
-    for (int s = 0; s < S; ++s) {
-      ptx::mbar_init(full_bar(s), 1);
-      ptx::mbar_init(empty_bar(s), 2);  // one arrival per MMA warpgroup
-    }
-    for (int s = 0; p.rowshare && s < SA; ++s) {
-      ptx::mbar_init(a_full_bar(s), 1);
-      ptx::mbar_init(a_empty_bar(s), 2);
-    }
+    ring.init(1, 2);  // one producer arrival (+ TMA bytes), one arrival per MMA warpgroup
+    if (p.rowshare) a_ring.init(1, 2);
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -163,8 +163,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
   const int total_tiles = m_tiles * p.n_tiles;
   const int terms = FAT ? 1 : p.num_terms;
   const int num_kb = terms * p.taps_h * p.taps_w * p.cin_chunks;
-  const uint32_t a_box_bytes = static_cast<uint32_t>(p.box_w * p.box_h * p.box_n) * kBlockK * 2;
-  const uint32_t stage_tx = (FAT ? 2u : 1u) * (a_box_bytes + kBBytes);
 
   // M tile -> pixel-box origin
   auto m_coords = [&](int m, int& tw, int& th, int& tn) {
@@ -178,61 +176,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
     // ------------------------------------------------------------ TMA producer
     ptx::setmaxnreg_dec<40>();
     if (warp != 0) return;
-    // The whole warp walks the loops (warp-uniform control flow); one elected lane issues.
-    int stage = 0;
-    uint32_t phase = 0;
-    if (p.rowshare) {
-      // Row-share: the activation rows of one (term, dy, channel chunk) are fetched ONCE with a one-pixel halo on each
-      // side ({64, box_w + 2, box_h, 1} from column w0 - pad: TMA zero fill is still the padding) and serve the taps
-      // dx = 0, 1, 2; only the weight tiles are fetched per tap.
-      int sa = 0;
-      uint32_t pa = 0;
-      const uint32_t a_tx = (FAT ? 2u : 1u) * static_cast<uint32_t>((p.box_w + 2) * p.box_h) * kBlockK * 2;
-      const uint32_t b_tx = (FAT ? 2u : 1u) * kBBytes;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int n_tile = tile % p.n_tiles;
-        int tw, th, tn;
-        m_coords(tile / p.n_tiles, tw, th, tn);
-        const int w0 = tw * p.box_w - p.pad_w, h0 = th * p.box_h - p.pad_h, n0 = tn * p.box_n;
-        for (int term = 0; term < terms; ++term) {
-          const CUtensorMap* mapA = (term == 2) ? &tmA_lo : &tmA_hi;
-          const CUtensorMap* mapB = (term == 1) ? &tmB_lo : &tmB_hi;
-          for (int dy = 0; dy < p.taps_h; ++dy) {
-            for (int cc = 0; cc < p.cin_chunks; ++cc) {
-              ptx::mbar_wait(a_empty_bar(sa), pa ^ 1u);
-              if (ptx::elect_one()) {
-                ptx::mbar_expect_tx(a_full_bar(sa), a_tx);
-                const uint32_t a0 = sA + sa * a_stride;
-                ptx::tma_load_4d(a0, mapA, a_full_bar(sa), cc * kBlockK, w0, h0 + dy, n0);
-                if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, a_full_bar(sa), cc * kBlockK, w0, h0 + dy, n0);
-              }
-              __syncwarp();
-              if (++sa == SA) {
-                sa = 0;
-                pa ^= 1u;
-              }
-              for (int dx = 0; dx < p.taps_w; ++dx) {
-                const int tap = dy * p.taps_w + dx;
-                ptx::mbar_wait(empty_bar(stage), phase ^ 1u);
-                if (ptx::elect_one()) {
-                  ptx::mbar_expect_tx(full_bar(stage), b_tx);
-                  const uint32_t b0 = sB + stage * b_stride;
-                  const int kcol = (tap * p.cin_chunks + cc) * kBlockK;
-                  ptx::tma_load_2d(b0, mapB, full_bar(stage), kcol, n_tile * BLOCK_N);
-                  if (FAT) ptx::tma_load_2d(b0 + kBBytes, &tmB_lo, full_bar(stage), kcol, n_tile * BLOCK_N);
-                }
-                __syncwarp();
-                if (++stage == S) {
-                  stage = 0;
-                  phase ^= 1u;
-                }
-              }
-            }
-          }
-        }
-      }
-      return;
-    }
+    // The whole warp walks the loops (warp-uniform control flow); one elected lane issues.  Row-share fetches the
+    // activation rows of one (term, dy, channel chunk) ONCE, with a one-pixel halo on each side ({64, box_w + 2, box_h,
+    // 1} from column w0 - pad: TMA zero fill is still the padding), for the taps dx = 0, 1, 2; each stage then carries
+    // only the weight tiles.  Without row-share each stage carries the tap's shifted activation tile as well.
+    const uint32_t a_tx = kPlanes * static_cast<uint32_t>((p.box_w + (p.rowshare ? 2 : 0)) * p.box_h * p.box_n) * kBlockK * 2;
+    const uint32_t stage_tx = kPlanes * kBBytes + (p.rowshare ? 0u : a_tx);
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int n_tile = tile % p.n_tiles;
       int tw, th, tn;
@@ -243,23 +192,32 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
         const CUtensorMap* mapB = (term == 1) ? &tmB_lo : &tmB_hi;
         for (int dy = 0; dy < p.taps_h; ++dy) {
           for (int cc = 0; cc < p.cin_chunks; ++cc) {
-            for (int dx = 0; dx < p.taps_w; ++dx) {
-              const int tap = dy * p.taps_w + dx;
-              ptx::mbar_wait(empty_bar(stage), phase ^ 1u);
+            if (p.rowshare) {
+              a_ring.wait_empty();
               if (ptx::elect_one()) {
-                ptx::mbar_expect_tx(full_bar(stage), stage_tx);
-                const uint32_t a0 = sA + stage * a_stride, b0 = sB + stage * b_stride;
-                const int kcol = (tap * p.cin_chunks + cc) * kBlockK;
-                ptx::tma_load_2d(b0, mapB, full_bar(stage), kcol, n_tile * BLOCK_N);
-                if (FAT) ptx::tma_load_2d(b0 + kBBytes, &tmB_lo, full_bar(stage), kcol, n_tile * BLOCK_N);
-                ptx::tma_load_4d(a0, mapA, full_bar(stage), cc * kBlockK, w0 + dx, h0 + dy, n0);
-                if (FAT) ptx::tma_load_4d(a0 + kABytes, &tmA_lo, full_bar(stage), cc * kBlockK, w0 + dx, h0 + dy, n0);
+                const uint32_t a0 = sA + a_ring.slot * a_stride;
+                ptx::mbar_expect_tx(a_ring.full_bar(), a_tx);
+                ptx::tma_load_4d(a0, mapA, a_ring.full_bar(), cc * kBlockK, w0, h0 + dy, n0);
+                if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, a_ring.full_bar(), cc * kBlockK, w0, h0 + dy, n0);
               }
               __syncwarp();
-              if (++stage == S) {
-                stage = 0;
-                phase ^= 1u;
+              a_ring.advance();
+            }
+            for (int dx = 0; dx < p.taps_w; ++dx) {
+              const int kcol = ((dy * p.taps_w + dx) * p.cin_chunks + cc) * kBlockK;
+              ring.wait_empty();
+              if (ptx::elect_one()) {
+                const uint32_t a0 = sA + ring.slot * a_stride, b0 = sB + ring.slot * b_stride;
+                ptx::mbar_expect_tx(ring.full_bar(), stage_tx);
+                ptx::tma_load_2d(b0, mapB, ring.full_bar(), kcol, n_tile * BLOCK_N);
+                if (FAT) ptx::tma_load_2d(b0 + kBBytes, &tmB_lo, ring.full_bar(), kcol, n_tile * BLOCK_N);
+                if (!p.rowshare) {
+                  ptx::tma_load_4d(a0, mapA, ring.full_bar(), cc * kBlockK, w0 + dx, h0 + dy, n0);
+                  if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, ring.full_bar(), cc * kBlockK, w0 + dx, h0 + dy, n0);
+                }
               }
+              __syncwarp();
+              ring.advance();
             }
           }
         }
@@ -282,27 +240,27 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
   const uint32_t a_dx_step = p.rowshare ? 128u : 0u;
   const int hw_box = p.box_w * p.box_h;
   const int box_rows = hw_box * p.box_n;
-  int stage = 0;
-  uint32_t phase = 0;
-  int sa = 0;  // A ring (row-share only)
-  uint32_t pa = 0;
   int ebuf = 0;
   float acc[kAcc];
+  // the MMAs of a k-block may still read its stage (and A slot) until the next k-block's wgmma_wait<1>
+  auto release_held = [&] {
+    ring.release_held(wg_leader);
+    a_ring.release_held(wg_leader);
+  };
 
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int n_tile = tile % p.n_tiles;
     const int n_base = n_tile * BLOCK_N;
-    int prev = -1, prev_a = -1;
     int dx = 0;
     for (int kb = 0; kb < num_kb; ++kb) {
       // operands first, then the fence: between wgmma.fence and the MMAs nothing but the MMAs is issued
-      const uint32_t a0 = sA + (p.rowshare ? sa : stage) * a_stride + a_row_off + dx * a_dx_step;
-      const uint32_t b0 = sB + stage * b_stride;
+      const uint32_t a0 = sA + (p.rowshare ? a_ring.slot : ring.slot) * a_stride + a_row_off + dx * a_dx_step;
+      const uint32_t b0 = sB + ring.slot * b_stride;
       const uint64_t ah = ptx::gmma_desc_sw128(a0), bh = ptx::gmma_desc_sw128(b0);
       const uint64_t al = ptx::gmma_desc_sw128(a0 + p.a_plane), bl = ptx::gmma_desc_sw128(b0 + kBBytes);
       const uint32_t accumulate = kb != 0 ? 1u : 0u;  // the tile's first K step overwrites the accumulators
-      if (p.rowshare && dx == 0) ptx::mbar_wait(a_full_bar(sa), pa);
-      ptx::mbar_wait(full_bar(stage), phase);
+      if (p.rowshare && dx == 0) a_ring.wait_full();
+      ring.wait_full();
       ptx::fence_regs(acc);  // keep the accumulators in place across the asynchronous MMAs
       ptx::wgmma_fence();
       if constexpr (FAT) {
@@ -322,35 +280,23 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
       ptx::fence_regs(acc);
       // the previous k-block's MMAs have finished reading their stage: hand it back to the producer
       ptx::wgmma_wait<1>();
-      if (prev >= 0 && wg_leader) ptx::mbar_arrive(empty_bar(prev));
-      if (prev_a >= 0 && wg_leader) ptx::mbar_arrive(a_empty_bar(prev_a));
-      prev = stage;
-      prev_a = -1;
-      if (++stage == S) {
-        stage = 0;
-        phase ^= 1u;
-      }
+      release_held();
+      ring.hold_and_advance();
       // k-blocks run (term, dy, chunk, dx) with dx innermost: after the last dx the A slot is done with
       if (++dx == p.taps_w) {
         dx = 0;
-        if (p.rowshare) {
-          prev_a = sa;
-          if (++sa == SA) {
-            sa = 0;
-            pa ^= 1u;
-          }
-        }
+        if (p.rowshare) a_ring.hold_and_advance();
       }
     }
     ptx::wgmma_wait<0>();
     ptx::fence_regs(acc);
-    if (prev >= 0 && wg_leader) ptx::mbar_arrive(empty_bar(prev));
-    if (prev_a >= 0 && wg_leader) ptx::mbar_arrive(a_empty_bar(prev_a));
+    release_held();
 
     int tw, th, tn;
     m_coords(tile / p.n_tiles, tw, th, tn);
     if (p.out_mode == MSCNN_OUT_NHWC_BF16) {
       if constexpr (BLOCK_N >= 64) {
+        const uint32_t lo_plane = kABytes;
 #pragma unroll
         for (int chunk = 0; chunk < BLOCK_N / 64; ++chunk) {
           // the staging buffer we are about to overwrite must have been read by its TMA store
@@ -359,27 +305,15 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
             else ptx::tma_store_wait_read<1>();
           }
           ptx::named_bar_sync(kEpiBarId, kEpiThreads);
-          const uint32_t buf = sEpi + ebuf * epi_buf_bytes;
+          const uint32_t buf = sEpi + ebuf * lay.epi_buf;
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj) {  // 8-column groups of this 64-channel chunk
             const int j = chunk * 8 + jj;
             const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + n_base + 8 * j + cq));
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int r = r0 + 8 * h;
-              float f0 = acc[4 * j + 2 * h] + bb.x;
-              float f1 = acc[4 * j + 2 * h + 1] + bb.y;
-              if (p.relu) {
-                f0 = fmaxf(f0, 0.f);
-                f1 = fmaxf(f1, 0.f);
-              }
-              // packed conversions (cvt.rn.bf16x2.f32): same rounding as scalar ones, half the issue slots
-              const uint32_t hi = pack_bf16x2(f0, f1);
-              const uint32_t lo = pack_bf16x2(f0 - __uint_as_float(hi << 16), f1 - __uint_as_float(hi & 0xFFFF0000u));
-              const uint32_t a = buf + r * 128 + static_cast<uint32_t>((jj ^ (r & 7)) << 4) + 2u * cq;  // 128B swizzle
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(hi) : "memory");
-              if (p.has_lo_out) asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + kABytes), "r"(lo) : "memory");
-            }
+            for (int h = 0; h < 2; ++h)
+              ptx::stage_pair(buf, r0 + 8 * h, jj, cq, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], bb.x, bb.y, p.relu,
+                              p.has_lo_out, lo_plane);
           }
           const uint32_t pbuf = buf + kABytes * (p.has_lo_out ? 2 : 1);  // pooled staging [hi][lo]
           if (p.pool) {
@@ -405,7 +339,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
                              : "=r"(xh[0]), "=r"(xh[1]), "=r"(xh[2]), "=r"(xh[3]) : "r"(a));
                 if (p.has_lo_out)
                   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                               : "=r"(xl[0]), "=r"(xl[1]), "=r"(xl[2]), "=r"(xl[3]) : "r"(a + kABytes));
+                               : "=r"(xl[0]), "=r"(xl[1]), "=r"(xl[2]), "=r"(xl[3]) : "r"(a + lo_plane));
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
                   const float v0 = __uint_as_float(xh[q] << 16) + __uint_as_float(xl[q] << 16);
@@ -417,9 +351,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
               uint32_t oh[4], ol[4];
 #pragma unroll
               for (int q = 0; q < 4; ++q) {
-                oh[q] = pack_bf16x2(best[2 * q], best[2 * q + 1]);
-                ol[q] = pack_bf16x2(best[2 * q] - __uint_as_float(oh[q] << 16),
-                                    best[2 * q + 1] - __uint_as_float(oh[q] & 0xFFFF0000u));
+                oh[q] = ptx::pack_bf16x2(best[2 * q], best[2 * q + 1]);
+                ol[q] = ptx::pack_bf16x2(best[2 * q] - __uint_as_float(oh[q] << 16),
+                                         best[2 * q + 1] - __uint_as_float(oh[q] & 0xFFFF0000u));
               }
               const uint32_t pa = pbuf + pr * 128 + static_cast<uint32_t>((j ^ (pr & 7)) << 4);
               asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(pa), "r"(oh[0]), "r"(oh[1]),
@@ -432,18 +366,14 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
           ptx::fence_proxy_async_smem();
           ptx::named_bar_sync(kEpiBarId, kEpiThreads);
           if (issuer) {
+            // one bulk group per staging buffer, pooled tile included
             const int c0 = n_base + chunk * 64;
-            if (!p.pool || p.store_full) {
-              ptx::tma_store_4d(&tmO_hi, buf, c0, tw * p.box_w, th * p.box_h, tn * p.box_n);
-              if (p.has_lo_out)
-                ptx::tma_store_4d(&tmO_lo, buf + kABytes, c0, tw * p.box_w, th * p.box_h, tn * p.box_n);
-            }
-            if (p.pool) {
-              ptx::tma_store_4d(&tmP_hi, pbuf, c0, tw * (p.box_w >> 1), th * (p.box_h >> 1), tn * p.box_n);
-              if (p.has_lo_out)
-                ptx::tma_store_4d(&tmP_lo, pbuf + kPoolBytes, c0, tw * (p.box_w >> 1), th * (p.box_h >> 1),
-                                  tn * p.box_n);
-            }
+            if (!p.pool || p.store_full)
+              ptx::tma_store_hi_lo(&tmO_hi, &tmO_lo, buf, p.has_lo_out, lo_plane, c0, tw * p.box_w, th * p.box_h,
+                                   tn * p.box_n);
+            if (p.pool)
+              ptx::tma_store_hi_lo(&tmP_hi, &tmP_lo, pbuf, p.has_lo_out, kPoolBytes, c0, tw * (p.box_w >> 1),
+                                   th * (p.box_h >> 1), tn * p.box_n);
             ptx::tma_store_commit();
           }
           if (++ebuf == p.epi_bufs) ebuf = 0;
@@ -468,18 +398,13 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
         for (int j = 0; j < BLOCK_N / 8; ++j) {
           const int c = 8 * j + cq;
           const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + n_base + c));
-          float f0 = acc[4 * j + 2 * h] + bb.x;
-          float f1 = acc[4 * j + 2 * h + 1] + bb.y;
-          if (p.relu) {
-            f0 = fmaxf(f0, 0.f);
-            f1 = fmaxf(f1, 0.f);
-          }
+          const float2 f = ptx::bias_relu(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], bb.x, bb.y, p.relu);
           if (p.out_mode == MSCNN_OUT_NHWC_F32) {
-            *reinterpret_cast<float2*>(rbase + c) = make_float2(f0, f1);
+            *reinterpret_cast<float2*>(rbase + c) = f;
           } else {
             const int ch = n_base + c;
-            if (ch < p.out_c) obase[static_cast<size_t>(ch) * plane] = f0;
-            if (ch + 1 < p.out_c) obase[static_cast<size_t>(ch + 1) * plane] = f1;
+            if (ch < p.out_c) obase[static_cast<size_t>(ch) * plane] = f.x;
+            if (ch + 1 < p.out_c) obase[static_cast<size_t>(ch + 1) * plane] = f.y;
           }
         }
       }
@@ -616,18 +541,12 @@ extern "C" int mscnn_conv_forward(const mscnn_conv_desc* d, void* stream_v) {
     if (g_plans.size() >= 4096) g_plans.clear();  // blobs that keep moving (re-allocation): bound the table
     g_plans.emplace(key, plan);
   }
-  cudaError_t e;
-  const IgemmParams& p = plan.p;
-  switch (plan.BN) {
-    // fat stages only below BLOCK_N = 256 (build_plan): no <256, true> instantiation
-    case 256: e = launch_igemm<256, false>(plan.maps, p, plan.grid, plan.smem, device, stream); break;
-    case 128: e = p.fat ? launch_igemm<128, true>(plan.maps, p, plan.grid, plan.smem, device, stream)
-                        : launch_igemm<128, false>(plan.maps, p, plan.grid, plan.smem, device, stream); break;
-    case 64: e = p.fat ? launch_igemm<64, true>(plan.maps, p, plan.grid, plan.smem, device, stream)
-                       : launch_igemm<64, false>(plan.maps, p, plan.grid, plan.smem, device, stream); break;
-    default: e = p.fat ? launch_igemm<32, true>(plan.maps, p, plan.grid, plan.smem, device, stream)
-                       : launch_igemm<32, false>(plan.maps, p, plan.grid, plan.smem, device, stream); break;
-  }
+  // [BLOCK_N = 32 << i][fat]; fat stages only below BLOCK_N = 256 (build_plan): no <256, true> instantiation
+  static const decltype(&launch_igemm<32, false>) launch[4][2] = {
+      {launch_igemm<32, false>, launch_igemm<32, true>}, {launch_igemm<64, false>, launch_igemm<64, true>},
+      {launch_igemm<128, false>, launch_igemm<128, true>}, {launch_igemm<256, false>, nullptr}};
+  const cudaError_t e =
+      launch[__builtin_ctz(plan.BN) - 5][plan.p.fat](plan.maps, plan.p, plan.grid, plan.smem, device, stream);
   if (e != cudaSuccess) {
     fprintf(stderr, "mscnn_conv_forward: launch failed: %s\n", cudaGetErrorString(e));
     return MSCNN_ERR_CUDA;
@@ -636,6 +555,32 @@ extern "C" int mscnn_conv_forward(const mscnn_conv_desc* d, void* stream_v) {
 }
 
 namespace mscnn {
+
+// The deepest B ring, up to kMaxStages, whose layout fits the shared-memory budget (0 if none does).
+static int deepest_ring(IgemmParams p, int block_n) {
+  for (p.stages = kMaxStages; p.stages > 0 && igemm_layout(p, block_n).total > kSmemBudget; --p.stages) {
+  }
+  return p.stages;
+}
+
+// Ring depths of a candidate plan (per-tap or row-share, staging buffers preset): the B ring as deep as fits, one
+// staging buffer instead of two where two would leave it shallower than 4 stages; with row-share, room left once the B
+// ring is at its cap deepens the A ring from 2 up to kMaxAStages slots: with short k-blocks (plain bf16) two slots leave
+// only one group of three taps to cover the L2 latency of the next activation tile.
+static void fit_rings(IgemmParams& p, int block_n) {
+  p.stages = deepest_ring(p, block_n);
+  if (p.stages < 4 && p.epi_bufs == 2) {
+    p.epi_bufs = 1;
+    p.stages = deepest_ring(p, block_n);
+  }
+  while (p.rowshare && p.a_stages < kMaxAStages) {
+    IgemmParams deeper = p;
+    ++deeper.a_stages;
+    if (deepest_ring(deeper, block_n) < kMaxStages) break;
+    p.a_stages = deeper.a_stages;
+  }
+  p.stages = deepest_ring(p, block_n);
+}
 
 static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps) {
   const Config& cfg = config();
@@ -682,29 +627,19 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
   p.out_w = Wo;
   p.out_ld = d->Cout_pad;
 
-  // shared memory plan.  Fat stages (A_hi, A_lo, B_hi, B_lo of a k-block in one stage, three MMAs per K step) for
-  // the narrow-N layers of the fp32-faithful path: A_hi / B_hi are fetched once instead of twice and a barrier round
-  // trip covers 3x the MMAs.  BLOCK_N = 256 keeps single tiles: a fat stage would be 96 KB.  The choice depends on
-  // the layer alone (not on pooling), so that fused and unfused launches of a layer sum in the same order.
-  const int b_bytes = BN * kBlockK * 2;
-  p.fat = (split && BN <= 128 && !cfg.no_fat) ? 1 : 0;
-  const int epi_unit = (d->out_mode == MSCNN_OUT_NHWC_BF16) ? (kABytes + (pool ? kABytes / 4 : 0)) * (p.has_lo_out ? 2 : 1) : 0;
-  const int misc = 8 * 2 * 8 + 1024 /*alignment slack*/;
-  const int stage_bytes = (kABytes + b_bytes) * (p.fat ? 2 : 1);
-  int epi_bufs = (epi_unit == 0) ? 0 : 2;
-  int stages = (kSmemBudget - misc - epi_bufs * epi_unit) / stage_bytes;
-  if (stages < 4 && epi_bufs == 2) {
-    epi_bufs = 1;
-    stages = (kSmemBudget - misc - epi_bufs * epi_unit) / stage_bytes;
-  }
-  if (stages > 8) stages = 8;
-  if (stages < 2) return MSCNN_ERR_INVALID;
-  p.stages = stages;
-  p.epi_bufs = epi_bufs;  // 0 in fp32-output mode: no staging region is carved
-  p.a_slot = kABytes * (p.fat ? 2 : 1);
+  // Fat stages (A_hi, A_lo, B_hi, B_lo of a k-block in one stage, three MMAs per K step) for the narrow-N layers of
+  // the fp32-faithful path: A_hi / B_hi are fetched once instead of twice and a barrier round trip covers 3x the MMAs.
+  // BLOCK_N = 256 keeps single tiles: a fat stage would be 96 KB.  The choice depends on the layer alone (not on
+  // pooling), so that fused and unfused launches of a layer sum in the same order.
+  const int planes = (split && BN <= 128 && !cfg.no_fat) ? 2 : 1;
+  const bool staged = d->out_mode == MSCNN_OUT_NHWC_BF16;  // fp32 outputs carve no staging region
+  p.fat = planes == 2;
+  p.a_slot = kABytes * planes;
   p.a_plane = kABytes;
   p.a_wg_row = 64;
-  size_t smem = (size_t)stages * stage_bytes + (size_t)epi_bufs * epi_unit + misc;
+  p.epi_bufs = staged ? 2 : 0;
+  fit_rings(p, BN);
+  if (p.stages < 2) return MSCNN_ERR_INVALID;
 
   // Row-share (3 horizontal taps, one image row per MMA warpgroup: 64x2 and 128x1 boxes, BLOCK_N <= 128).  The three
   // taps dx of a (term, dy, chunk) are the same activation rows shifted by one pixel: fetch them once with a one-pixel
@@ -713,36 +648,18 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
   // has to be at least as deep (in taps) as the per-tap ring it replaces, else the per-tap plan stays.
   const bool rs_box = p.box_n == 1 && ((p.box_w == 64 && p.box_h == 2) || (p.box_w == 128 && p.box_h == 1));
   if (!cfg.no_rowshare && d->KW == 3 && BN <= 128 && rs_box) {
-    const int planes = p.fat ? 2 : 1;
-    const int a_plane = ((p.box_w + 2) * p.box_h * 128 + 1023) / 1024 * 1024;  // each plane 1024-aligned (swizzle)
-    const int a_slot = a_plane * planes;
-    const int b_stage = b_bytes * planes;
-    const int rs_misc = 8 * 2 * (8 + 4) + 1024 /*alignment slack*/;
+    IgemmParams rs = p;
+    rs.rowshare = 1;
+    rs.a_stages = 2;
+    rs.a_plane = ((p.box_w + 2) * p.box_h * 128 + 1023) / 1024 * 1024;  // each plane 1024-aligned (swizzle)
+    rs.a_slot = rs.a_plane * planes;
+    rs.a_wg_row = 64 / p.box_w * (p.box_w + 2) + 64 % p.box_w;  // halo-tile row of output pixel 64
     // a second epilogue buffer only overlaps the two 64-channel chunks of a BLOCK_N = 128 tile
-    int rs_epi = (epi_unit == 0) ? 0 : (BN > 64 ? 2 : 1);
-    int a_stages = 2;
-    auto fit = [&](int eb, int sa) { return (kSmemBudget - rs_misc - sa * a_slot - eb * epi_unit) / b_stage; };
-    int rs_stages = fit(rs_epi, a_stages);
-    if (rs_stages < 4 && rs_epi == 2) {
-      rs_epi = 1;
-      rs_stages = fit(rs_epi, a_stages);
-    }
-    // Room left with the B ring at its cap deepens the A ring (up to 4): with short k-blocks (plain bf16) two slots
-    // leave only one group of three taps to cover the L2 latency of the next activation tile.
-    while (a_stages < 4 && fit(rs_epi, a_stages + 1) >= 8) ++a_stages;
-    rs_stages = fit(rs_epi, a_stages);
-    if (rs_stages > 8) rs_stages = 8;
-    if (rs_stages >= stages) {
-      p.rowshare = 1;
-      p.a_stages = a_stages;
-      p.a_slot = a_slot;
-      p.a_plane = a_plane;
-      p.a_wg_row = 64 / p.box_w * (p.box_w + 2) + 64 % p.box_w;  // halo-tile row of output pixel 64
-      p.stages = rs_stages;
-      p.epi_bufs = rs_epi;
-      smem = (size_t)a_stages * a_slot + (size_t)rs_stages * b_stage + (size_t)rs_epi * epi_unit + rs_misc;
-    }
+    rs.epi_bufs = staged ? (BN > 64 ? 2 : 1) : 0;
+    fit_rings(rs, BN);
+    if (rs.stages >= p.stages) p = rs;
   }
+  const size_t smem = igemm_layout(p, BN).total;
   const int total_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_tiles;
   if (cfg.verbose_conv)
     fprintf(stderr, "conv plan: N=%d H=%d W=%d C=%d Cout_pad=%d k=%dx%d BN=%d box=%dx%dx%d fat=%d terms=%d rowshare=%d a_stages=%d stages=%d epi_bufs=%d smem=%zu tiles=%d\n",
@@ -757,57 +674,29 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
     plan->grid = 0;
     return MSCNN_OK;
   }
-  const uint32_t obox[4] = {64u, (uint32_t)p.box_w, (uint32_t)p.box_h, (uint32_t)p.box_n};
-  const uint32_t abox[4] = {64u, (uint32_t)(p.box_w + (p.rowshare ? 2 : 0)), (uint32_t)p.box_h, (uint32_t)p.box_n};
-  const uint64_t adim[4] = {(uint64_t)d->C, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->N};
-  int rc = tmap_nhwc_bf16(&maps[0], d->x_hi, adim, abox);
-  if (rc) return rc;
-  if (split) {
-    rc = tmap_nhwc_bf16(&maps[1], d->x_lo, adim, abox);
-    if (rc) return rc;
-  } else {
-    maps[1] = maps[0];
-  }
-  const uint64_t ktot = (uint64_t)d->KH * d->KW * d->C;
-  rc = tmap_2d_bf16(&maps[2], d->w_hi, ktot, (uint64_t)d->Cout_pad, 64u, (uint32_t)BN);
-  if (rc) return rc;
-  if (split) {
-    rc = tmap_2d_bf16(&maps[3], d->w_lo, ktot, (uint64_t)d->Cout_pad, 64u, (uint32_t)BN);
-    if (rc) return rc;
-  } else {
-    maps[3] = maps[2];
-  }
-  if (d->out_mode == MSCNN_OUT_NHWC_BF16) {
-    const uint64_t odim[4] = {(uint64_t)d->Cout_pad, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)d->N};
-    if (d->y_hi) {
-      rc = tmap_nhwc_bf16(&maps[4], d->y_hi, odim, obox);
-      if (rc) return rc;
-    } else {
-      maps[4] = maps[0];
+  // The kernel's maps A_hi, A_lo, B_hi, B_lo, O_hi, O_lo, P_hi, P_lo (P: fused pooling output).  One the launch does
+  // not use is a copy of its primary (a lo plane of its hi plane, a hi plane of A_hi), so every argument is valid.
+  const bool lo_out = staged && p.has_lo_out;
+  const void* src[8] = {d->x_hi, split ? d->x_lo : nullptr, d->w_hi, split ? d->w_lo : nullptr,
+                        staged ? d->y_hi : nullptr, lo_out ? d->y_lo : nullptr,
+                        p.pool ? d->pool_hi : nullptr, p.pool && lo_out ? d->pool_lo : nullptr};
+  const uint64_t dims[4][4] = {{(uint64_t)d->C, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->N},
+                               {},
+                               {(uint64_t)d->Cout_pad, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)d->N},
+                               {(uint64_t)d->Cout_pad, (uint64_t)(Wo / 2), (uint64_t)(Ho / 2), (uint64_t)d->N}};
+  const uint32_t boxes[4][4] = {{64u, (uint32_t)(p.box_w + (p.rowshare ? 2 : 0)), (uint32_t)p.box_h, (uint32_t)p.box_n},
+                                {},
+                                {64u, (uint32_t)p.box_w, (uint32_t)p.box_h, (uint32_t)p.box_n},
+                                {64u, (uint32_t)(p.box_w / 2), (uint32_t)(p.box_h / 2), (uint32_t)p.box_n}};
+  for (int i = 0; i < 8; ++i) {
+    if (!src[i]) {
+      maps[i] = maps[(i & 1) ? i - 1 : 0];
+      continue;
     }
-    if (p.has_lo_out && d->y_lo) {
-      rc = tmap_nhwc_bf16(&maps[5], d->y_lo, odim, obox);
-      if (rc) return rc;
-    } else {
-      maps[5] = maps[4];
-    }
-  } else {
-    maps[4] = maps[0];
-    maps[5] = maps[0];
-  }
-  maps[6] = maps[4];
-  maps[7] = maps[5];
-  if (p.pool) {
-    const uint64_t pdim[4] = {(uint64_t)d->Cout_pad, (uint64_t)(Wo / 2), (uint64_t)(Ho / 2), (uint64_t)d->N};
-    const uint32_t pbox[4] = {64u, (uint32_t)(p.box_w / 2), (uint32_t)(p.box_h / 2), (uint32_t)p.box_n};
-    rc = tmap_nhwc_bf16(&maps[6], d->pool_hi, pdim, pbox);
+    const int rc = (i >> 1) == 1
+                       ? tmap_2d_bf16(&maps[i], src[i], (uint64_t)d->KH * d->KW * d->C, (uint64_t)d->Cout_pad, 64u, (uint32_t)BN)
+                       : tmap_nhwc_bf16(&maps[i], src[i], dims[i >> 1], boxes[i >> 1]);
     if (rc) return rc;
-    if (p.has_lo_out) {
-      rc = tmap_nhwc_bf16(&maps[7], d->pool_lo, pdim, pbox);
-      if (rc) return rc;
-    } else {
-      maps[7] = maps[6];
-    }
   }
 
   int grid = mscnn_sm_count();

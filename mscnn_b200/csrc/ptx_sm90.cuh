@@ -1,9 +1,10 @@
 // Thin inline-PTX wrappers for the sm_90a features the MS-CNN kernels use:
 // mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors)
-// and the proxy fences between them.  Nothing here is generic: it is the minimal set
-// needed by conv_igemm.cu and conv_c3_tc.cu.
+// and the proxy fences between them, plus the mbarrier ring and the (hi, lo) epilogue staging both kernels share.
+// Nothing here is generic: it is the minimal set needed by conv_igemm.cu and conv_c3_tc.cu.
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -43,6 +44,40 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
+
+// A ring of `depth` shared-memory slots, each guarded by a "full" and an "empty" mbarrier (16 B per slot from `bars`).
+// Producer and consumer walk the slots in order; the parity they wait for flips each time the ring wraps.  A consumer
+// whose asynchronous reads of a slot outlive its wait holds the slot and releases it later (release_held).
+struct Ring {
+  uint32_t bars;
+  int depth, slot = 0, held = -1;
+  uint32_t phase = 0;
+  __device__ Ring(uint32_t bars_, int depth_) : bars(bars_), depth(depth_) {}
+  __device__ uint32_t full_bar() const { return bars + 16u * slot; }
+  __device__ uint32_t empty_bar(int s) const { return bars + 16u * s + 8u; }
+  __device__ void init(uint32_t fill_arrivals, uint32_t drain_arrivals) const {
+    for (int s = 0; s < depth; ++s) {
+      mbar_init(bars + 16u * s, fill_arrivals);
+      mbar_init(empty_bar(s), drain_arrivals);
+    }
+  }
+  __device__ void wait_full() const { mbar_wait(full_bar(), phase); }
+  __device__ void wait_empty() const { mbar_wait(empty_bar(slot), phase ^ 1u); }
+  __device__ void advance() {
+    if (++slot == depth) {
+      slot = 0;
+      phase ^= 1u;
+    }
+  }
+  __device__ void hold_and_advance() {
+    held = slot;
+    advance();
+  }
+  __device__ void release_held(bool arrive) {
+    if (held >= 0 && arrive) mbar_arrive(empty_bar(held));
+    held = -1;
+  }
+};
 
 // ---------------------------------------------------------------------- TMA
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
@@ -86,6 +121,39 @@ __device__ __forceinline__ void tma_store_wait_all() {
 // generic-proxy smem writes -> visible to the async proxy (TMA store source, wgmma operands)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+
+// ----------------------------------------------------------------- epilogue
+// packed conversion (cvt.rn.bf16x2.f32): rounds like two scalar ones in half the issue slots
+__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
+  const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h2);
+}
+__device__ __forceinline__ float2 bias_relu(float a0, float a1, float b0, float b1, bool relu) {
+  float f0 = a0 + b0, f1 = a1 + b1;
+  if (relu) {
+    f0 = fmaxf(f0, 0.f);
+    f1 = fmaxf(f1, 0.f);
+  }
+  return make_float2(f0, f1);
+}
+// One accumulator pair (two adjacent channels of one pixel) + bias, ReLU, split into bf16 (hi, lo) and stored into an
+// output staging tile of 128 B rows laid out for a SWIZZLE_128B TMA store: row r, 16 B chunk j, bytes [2 c, 2 c + 4)
+// of it; the lo plane lies `lo_plane` bytes after the hi plane and is written only when `lo` is set.
+__device__ __forceinline__ void stage_pair(uint32_t buf, int r, int j, int c, float a0, float a1, float b0, float b1,
+                                           bool relu, bool lo, uint32_t lo_plane) {
+  const float2 f = bias_relu(a0, a1, b0, b1, relu);
+  const uint32_t h = pack_bf16x2(f.x, f.y);
+  const uint32_t l = pack_bf16x2(f.x - __uint_as_float(h << 16), f.y - __uint_as_float(h & 0xFFFF0000u));
+  const uint32_t a = buf + r * 128 + static_cast<uint32_t>((j ^ (r & 7)) << 4) + 2u * c;
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(h) : "memory");
+  if (lo) asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + lo_plane), "r"(l) : "memory");
+}
+// TMA store of a staged (hi, lo) tile pair at NHWC coordinates (c0, c1, c2, c3); the caller commits the bulk group.
+__device__ __forceinline__ void tma_store_hi_lo(const CUtensorMap* hi, const CUtensorMap* lo, uint32_t src, bool has_lo,
+                                                uint32_t lo_plane, int c0, int c1, int c2, int c3) {
+  tma_store_4d(hi, src, c0, c1, c2, c3);
+  if (has_lo) tma_store_4d(lo, src + lo_plane, c0, c1, c2, c3);
 }
 
 // One lane of a CONVERGED warp (the lowest): lets single-thread instructions (TMA) be issued from

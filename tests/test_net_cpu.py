@@ -43,21 +43,26 @@ def test_library_carries_sm90a_tensor_core_code():
 
 def test_tensor_core_kernels_use_warpgroup_mma():
     """Every convolution instantiation and the conv1_1 kernel issue wgmma (HGMMA); nothing in the library carries
-    instructions an sm_90a part lacks."""
+    instructions an sm_90a part lacks.  Each of them has exactly one WARPGROUP.ARRIVE: the MMA sequence sits in no
+    divergent region (DESIGN.md 4.1, why FAT and SPLIT are template parameters), so ptxas adds no extra warpgroup
+    synchronisation before the MMAs."""
     out = subprocess.run(["cuobjdump", "-sass", str(ROOT / "mscnn_b200" / "libmscnn_b200.so")],
                          capture_output=True, text=True).stdout
     if not out:
         pytest.skip("cuobjdump unavailable")
-    users, fn = {}, None
+    users, arrives, fn = {}, {}, None
     for line in out.splitlines():
         m = re.search(r"Function : (\S+)", line)
         if m:
             fn = m.group(1)
         elif fn and "HGMMA" in line:
             users[fn] = users.get(fn, 0) + 1
+        elif fn and "WARPGROUP.ARRIVE" in line:
+            arrives[fn] = arrives.get(fn, 0) + 1
     for bn in (32, 64, 128, 256):
         assert any(f"conv_igemm_kernelILi{bn}E" in f for f in users), sorted(users)
     assert any("conv_c3_tc_kernel" in f for f in users), sorted(users)
+    assert {f: arrives.get(f, 0) for f in users} == {f: 1 for f in users}
     assert "arch = sm_90a" in out and "sm_100" not in out
 
 
