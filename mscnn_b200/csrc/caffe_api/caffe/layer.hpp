@@ -73,10 +73,6 @@ class CAFFE_API Layer {
 
   vector<shared_ptr<Blob<Dtype> > >& blobs() { return blobs_; }
   const LayerParameter& layer_param() const { return layer_param_; }
-  // mscnn_b200 extension: a layer whose work another layer may do for it in the same forward (a Pooling computed in
-  // the producing convolution's epilogue, a sibling ROIPooling pooled by the group's leader) forgets that mark here;
-  // Net::ForwardFromTo calls it on every layer before it runs a range, so a mark never outlives the call that set it.
-  virtual void ResetFusedState() {}
   // mscnn_b200 extension (set by Net for the layers behind a BoxOutput layer): see DynRows
   void set_dyn_rows(const DynRows* d) { dyn_rows_ = d; }
   const int* dyn_rows_device() const { return (dyn_rows_ && dyn_rows_->pending) ? dyn_rows_->device_rows : nullptr; }

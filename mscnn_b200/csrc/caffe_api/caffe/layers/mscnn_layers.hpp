@@ -54,7 +54,13 @@ class CAFFE_API InputLayer : public Layer<Dtype> {
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {}
 };
 
-template <typename Dtype> class PoolingLayer;
+// A Pooling folded into its convolution (Net::FusePooling) is computed in the convolution's epilogue exactly when the
+// convolution's output has even height and width; at odd extents the convolution stores its full output and the
+// Pooling runs itself.  Both layers decide with this, from the shape of the forward they run in.
+template <typename Dtype>
+inline bool epilogue_pools(const Blob<Dtype>& conv_top) {
+  return conv_top.height() % 2 == 0 && conv_top.width() % 2 == 0;
+}
 
 /// ConvolutionLayer: conv_layer.cpp:8-40 / base_conv_layer.cpp:15-254 (stride 1, group 1, dilation 1:
 /// every Convolution in the shipped deploy nets).  blobs_[0] = [Cout, Cin, kh, kw], blobs_[1] = [Cout].
@@ -70,16 +76,17 @@ class CAFFE_API ConvolutionLayer : public Layer<Dtype> {
   // mscnn_b200 extension: fold the in-place ReLU that follows into the epilogue (set by Net).
   void set_fuse_relu(bool f) { fuse_relu_ = f; }
   bool fuse_relu() const { return fuse_relu_; }
-  // mscnn_b200 extension (set by Net): the 2x2/2 MAX PoolingLayer that follows is computed in this
-  // layer's epilogue and written to `pool_top`; with keep_full == false nothing else reads this
-  // layer's own top, which is then never written (its blob holds no data).
-  void set_fused_pool(PoolingLayer<Dtype>* pool, Blob<Dtype>* pool_top, bool keep_full) {
-    fused_pool_ = pool; fused_pool_top_ = pool_top; fused_keep_full_ = keep_full;
-  }
-  int num_output() const { return num_output_; }
+  // mscnn_b200 extension (set by Net): the folded 2x2/2 MAX Pooling that follows is computed in this layer's epilogue
+  // and written to `pool_top` whenever epilogue_pools(top); then, with keep_full == false, nothing else reads this
+  // layer's own top, which is not written (its blob holds no data).
+  void set_fused_pool(Blob<Dtype>* pool_top, bool keep_full) { fused_pool_top_ = pool_top; fused_keep_full_ = keep_full; }
+  // the route whose epilogue can pool: 64-channel-aligned output, not conv1_1's kernel
+  bool can_fuse_pool() const { return num_output_ % 64 == 0 && !is_conv1_1(); }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
-  PoolingLayer<Dtype>* fused_pool_ = nullptr;
+  bool is_conv1_1() const {
+    return channels_ == 3 && kernel_h_ == 3 && kernel_w_ == 3 && pad_h_ == 1 && pad_w_ == 1 && num_output_ == 64;
+  }
   Blob<Dtype>* fused_pool_top_ = nullptr;
   bool fused_keep_full_ = true;
   int num_output_, channels_, kernel_h_, kernel_w_, pad_h_, pad_w_;
@@ -126,7 +133,7 @@ class CAFFE_API ReLULayer : public Layer<Dtype> {
 template <typename Dtype>
 class CAFFE_API PoolingLayer : public Layer<Dtype> {
  public:
-  explicit PoolingLayer(const LayerParameter& param) : Layer<Dtype>(param) {}
+  explicit PoolingLayer(const LayerParameter& param) : Layer<Dtype>(param), fused_(false) {}
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "Pooling"; }
@@ -136,12 +143,11 @@ class CAFFE_API PoolingLayer : public Layer<Dtype> {
   int kernel() const { return kernel_; }
   int stride() const { return stride_; }
   int mode() const { return mode_; }
-  void mark_done_by_producer() { done_by_producer_ = true; }  // the convolution's epilogue pooled already
-  virtual void ResetFusedState() { done_by_producer_ = false; }
+  void set_fused(bool f) { fused_ = f; }   // folded into the producing convolution: see epilogue_pools
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   int kernel_, stride_, mode_, pooled_h_, pooled_w_;
-  bool done_by_producer_ = false;
+  bool fused_;
 };
 
 /// SplitLayer: split_layer.cpp:9-31 (forward = share data).
@@ -261,7 +267,7 @@ template <typename Dtype>
 class CAFFE_API ROIPoolingLayer : public Layer<Dtype> {
  public:
   explicit ROIPoolingLayer(const LayerParameter& param)
-      : Layer<Dtype>(param), concat_top_(nullptr), concat_offset_(0), concat_channels_(0) {}
+      : Layer<Dtype>(param), concat_top_(nullptr), concat_channels_(0), fused_(false) {}
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "ROIPooling"; }
@@ -269,34 +275,26 @@ class CAFFE_API ROIPoolingLayer : public Layer<Dtype> {
   virtual inline int MaxBottomBlobs() const { return 2; }
   virtual inline int MinTopBlobs() const { return 1; }
   virtual inline int MaxTopBlobs() const { return 1; }
-  // mscnn_b200 extension (set by Net): write into `target` (the Concat top) at a channel offset.
+  // mscnn_b200 extensions (set by Net when it folds a Concat into its ROIPooling producers): write into `target` (the
+  // Concat top) at a channel offset instead of into top[0]; and, for the group's leader, also pool `follower`'s variant
+  // (its pad ratio, at its channel offset) in this layer's launch, after which the follower does nothing.
   void set_concat_target(Blob<Dtype>* target, int channel_offset, int total_channels) {
-    concat_top_ = target; concat_offset_ = channel_offset; concat_channels_ = total_channels;
+    concat_top_ = target; channel_offsets_[0] = channel_offset; concat_channels_ = total_channels;
   }
-  // mscnn_b200 extension (set by Net): the sibling ROIPooling layers that feed the same Concat.  The
-  // first one pools all siblings that read the same feature map / ROIs in ONE launch; the others
-  // then find their work done (done_by_leader_) and return.
-  struct Sibling {
-    ROIPoolingLayer<Dtype>* layer;
-    Blob<Dtype>* feature;
-    Blob<Dtype>* rois;
-  };
-  void set_siblings(const vector<Sibling>& s) { siblings_ = s; }
-  float pad_ratio() const { return pad_ratio_; }
-  float spatial_scale() const { return spatial_scale_; }
-  int pooled_h() const { return pooled_height_; }
-  int pooled_w() const { return pooled_width_; }
-  int concat_offset() const { return concat_offset_; }
-  void mark_done_by_leader() { done_by_leader_ = true; }
-  virtual void ResetFusedState() { done_by_leader_ = false; }
+  void add_follower(ROIPoolingLayer<Dtype>* follower) {
+    pad_ratios_.push_back(follower->pad_ratios_[0]);
+    channel_offsets_.push_back(follower->channel_offsets_[0]);
+    follower->fused_ = true;
+  }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   int channels_, height_, width_, pooled_height_, pooled_width_;
-  float spatial_scale_, pad_ratio_;
+  float spatial_scale_;
+  vector<float> pad_ratios_;     // one variant per entry, pooled in one launch: this layer's own, then its followers'
+  vector<int> channel_offsets_;  // where each variant starts in the output's channels
   Blob<Dtype>* concat_top_;
-  int concat_offset_, concat_channels_;
-  vector<Sibling> siblings_;
-  bool done_by_leader_ = false;
+  int concat_channels_;
+  bool fused_;                   // the group's leader pools this layer's variant
 };
 
 /// ROIAlignLayer: roi_align_layer.cpp:22-139 (cascade WIDER-face net).  top = [R, C, pooled_h+1, pooled_w+1].

@@ -6,8 +6,10 @@
 // in-place top handling, outputs = unconsumed tops in name order (net.cpp:268-274).
 //
 // mscnn_b200 additions (all optional, default on): a fusion pass that folds in-place ReLU into
-// the producing Convolution / InnerProduct and Concat into its ROIPooling producers
-// (set MSCNN_NO_FUSION=1 to disable), and per-layer device timing for `caffe time`-style reports.
+// the producing Convolution / InnerProduct, 2x2 MAX Pooling into the convolution before it, and
+// Concat into its ROIPooling producers (set MSCNN_NO_FUSION=1 to disable).  It fixes every fused
+// group when the net is built; no layer changes another layer's state during a forward.  Also
+// per-layer device timing for `caffe time`-style reports.
 #pragma once
 #include <map>
 #include <set>
@@ -71,12 +73,15 @@ class CAFFE_API Net {
   void set_layer_timing(bool on) { time_layers_ = on; }
   const vector<float>& layer_times_ms() const { return layer_ms_; }
 
-  // mscnn_b200 extension: fused groups.  fused_producer(i) = the layer that does layer i's work when the fusion pass
-  // folded i into it (Pooling -> its convolution, sibling ROIPooling -> the group's leader), else i.  ForwardFromTo
-  // widens `start` back to that producer, so a range may start anywhere without running a consumer on a blob its
-  // producer never wrote; fused_group_end(i) = the last layer whose work layer i does.
+  // mscnn_b200 extension: fused groups, fixed by Init.  fused_producer(i) = the layer that does layer i's work when the
+  // fusion pass folded i into it (Pooling -> its convolution, ROIPooling -> the leader of its Concat group), else i.
+  // A folded Pooling still runs itself in a forward whose extents its convolution cannot pool (epilogue_pools).
+  // ForwardFromTo widens `start` back to that producer, so a range may start anywhere without running a consumer on a
+  // blob its producer never wrote; fused_group_end(i) = the last layer whose work layer i does.
   int fused_producer(int layer) const { return fused_producer_.empty() ? layer : fused_producer_[layer]; }
   int fused_group_end(int layer) const;
+  // mscnn_b200 extension: the last layer that reads blob_name's storage, directly or through a Split top (-1: none)
+  int last_reader(const string& blob_name) const;
   // mscnn_b200 extension: data-dependent rows (layer.hpp DynRows).  No layer waits for the device in the middle of a
   // forward: the blobs behind BoxOutput keep cap rows while the kernels read the true count on the device.
   // ResolveRows() waits for the count (a 12-byte copy issued right behind BoxOutput) and trims those blobs' shapes to
@@ -119,6 +124,7 @@ class CAFFE_API Net {
   vector<Blob<Dtype>*> net_output_blobs_;
   bool time_layers_;
   vector<float> layer_ms_;
+  vector<int> storage_blob_;    // per blob: the blob whose storage it shares (itself unless a Split top)
   vector<int> fused_producer_;  // per layer: who does its work (itself unless fused away)
   int dyn_box_ = -1;            // index of the BoxOutput layer whose rows are deferred (-1: none / several)
   vector<int> dyn_layers_;      // layers whose row count derives from it, in execution order

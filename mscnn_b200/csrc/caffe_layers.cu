@@ -190,7 +190,7 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
   // One kernel from the fp32 NCHW blob to planes: pixel rows staged once, the horizontal taps are
   // descriptor-shifted views of them (mscnn_conv1_tc_forward, conv_c3_tc.cu).  Its packed image serves
   // both precisions, so a precision switch does not re-pack it.
-  if (channels_ == 3 && kernel_h_ == 3 && kernel_w_ == 3 && pad_h_ == 1 && pad_w_ == 1 && num_output_ == 64) {
+  if (is_conv1_1()) {
     packed_.update_weights(wb, {PackedParam::CONV1_1, 0, 64, 0, 0, 0, 0}, (size_t)mscnn_conv1_tc_packed_bytes(),
                            [](const float* w, void* hi, void*) {
       MSCNN_CHECK(mscnn_pack_conv1_tc_weights(w, hi, 1, Caffe::stream()));
@@ -216,7 +216,7 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
   if (cout_pad % 64 == 0) {
     d.out_mode = MSCNN_OUT_NHWC_BF16;
     const int ho = top[0]->height(), wo = top[0]->width();
-    const bool pool_here = fused_pool_ && (ho % 2 == 0) && (wo % 2 == 0);
+    const bool pool_here = fused_pool_top_ && epilogue_pools(*top[0]);
     if (!pool_here || fused_keep_full_) {
       typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
       d.y_hi = y.hi;
@@ -227,7 +227,6 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
       typename Blob<Dtype>::Planes q = fused_pool_top_->mutable_planes(split);
       d.pool_hi = q.hi;
       d.pool_lo = q.lo;
-      fused_pool_->mark_done_by_producer();
     }
   } else {
     d.out_mode = MSCNN_OUT_NCHW_F32;  // narrow heads (LFCN_*): straight into the Caffe layout
@@ -314,10 +313,7 @@ void PoolingLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const vect
 }
 template <typename Dtype>
 void PoolingLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
-  if (done_by_producer_) {  // computed in the producing convolution's epilogue
-    done_by_producer_ = false;
-    return;
-  }
+  if (fused_ && epilogue_pools(*bottom[0])) return;  // computed in the producing convolution's epilogue
   const bool split = Caffe::split();
   typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
   typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
@@ -579,7 +575,8 @@ void ROIPoolingLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bottom, cons
   pooled_height_ = p.pooled_h();
   pooled_width_ = p.pooled_w();
   spatial_scale_ = p.spatial_scale();
-  pad_ratio_ = p.pad_ratio();
+  pad_ratios_.assign(1, p.pad_ratio());
+  channel_offsets_.assign(1, 0);
 }
 template <typename Dtype>
 void ROIPoolingLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
@@ -590,45 +587,21 @@ void ROIPoolingLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const v
 }
 template <typename Dtype>
 void ROIPoolingLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
-  if (done_by_leader_) {  // a sibling already pooled this variant in its launch
-    done_by_leader_ = false;
-    return;
-  }
+  if (fused_) return;  // the group's leader pools this layer's variant in its launch
   const bool split = Caffe::split();
   typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
   const int R = bottom[1]->num();
   const Dtype* rois = bottom[1]->gpu_data();
-  if (concat_top_) {
-    // fused ConcatLayer: the Net sized concat_top_ as [R, total, ph, pw]
+  Blob<Dtype>* out = top[0];
+  if (concat_top_) {  // fused ConcatLayer: its top is [R, total, ph, pw]
     concat_top_->Reshape(R, concat_channels_, pooled_height_, pooled_width_);
-    typename Blob<Dtype>::Planes y = concat_top_->mutable_planes(split);
-    float ratios[4];
-    int offs[4];
-    int nv = 0;
-    ratios[nv] = pad_ratio_;
-    offs[nv++] = concat_offset_;
-    for (size_t i = 0; i < siblings_.size() && nv < 4; ++i) {
-      ROIPoolingLayer<Dtype>* sb = siblings_[i].layer;
-      if (sb == this) continue;
-      // same feature map (shared through Split), same ROIs, same geometry -> same launch
-      typename Blob<Dtype>::Planes sx = siblings_[i].feature->planes(split);
-      if (sx.hi == x.hi && siblings_[i].rois->gpu_data() == rois && sb->pooled_h() == pooled_height_ &&
-          sb->pooled_w() == pooled_width_ && sb->spatial_scale() == spatial_scale_) {
-        ratios[nv] = sb->pad_ratio();
-        offs[nv++] = sb->concat_offset();
-        sb->mark_done_by_leader();
-      }
-    }
-    MSCNN_CHECK(mscnn_roi_pool_multi_forward_dyn(x.hi, x.lo, x.n, x.h, x.w, x.cpad, rois, R, pooled_height_,
-                                                 pooled_width_, spatial_scale_, nv, ratios, offs, y.hi, y.lo, y.cpad,
-                                                 this->dyn_rows_device(), Caffe::stream()));
-  } else {
-    typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
-    const int off0 = 0;
-    MSCNN_CHECK(mscnn_roi_pool_multi_forward_dyn(x.hi, x.lo, x.n, x.h, x.w, x.cpad, rois, R, pooled_height_,
-                                                 pooled_width_, spatial_scale_, 1, &pad_ratio_, &off0, y.hi, y.lo,
-                                                 y.cpad, this->dyn_rows_device(), Caffe::stream()));
+    out = concat_top_;
   }
+  typename Blob<Dtype>::Planes y = out->mutable_planes(split);
+  MSCNN_CHECK(mscnn_roi_pool_multi_forward_dyn(x.hi, x.lo, x.n, x.h, x.w, x.cpad, rois, R, pooled_height_, pooled_width_,
+                                               spatial_scale_, (int)pad_ratios_.size(), pad_ratios_.data(),
+                                               channel_offsets_.data(), y.hi, y.lo, y.cpad, this->dyn_rows_device(),
+                                               Caffe::stream()));
 }
 
 // ------------------------------------------------------------------------------- ROIAlign

@@ -158,6 +158,12 @@ void Net<Dtype>::Init(const NetParameter& in_param) {
   for (size_t i = 0; i < blob_names_.size(); ++i) blob_names_index_[blob_names_[i]] = (int)i;
   for (size_t i = 0; i < layer_names_.size(); ++i) layer_names_index_[layer_names_[i]] = (int)i;
   layer_ms_.assign(layers_.size(), 0.f);
+  storage_blob_.resize(blobs_.size());
+  for (size_t b = 0; b < blobs_.size(); ++b) storage_blob_[b] = (int)b;
+  for (size_t i = 0; i < layers_.size(); ++i)  // a Split's tops share its bottom's storage (SplitLayer::Forward_gpu)
+    if (dynamic_cast<SplitLayer<Dtype>*>(layers_[i].get()))
+      for (size_t t = 0; t < top_id_vecs_[i].size(); ++t)
+        storage_blob_[top_id_vecs_[i][t]] = storage_blob_[bottom_id_vecs_[i][0]];
   fused_producer_.resize(layers_.size());
   for (size_t i = 0; i < layers_.size(); ++i) fused_producer_[i] = (int)i;
   if (!std::getenv("MSCNN_NO_FUSION")) {
@@ -277,7 +283,7 @@ void Net<Dtype>::FuseLayers() {
   for (int i = 0; i < L; ++i) {
     ConcatLayer<Dtype>* cat = dynamic_cast<ConcatLayer<Dtype>*>(layers_[i].get());
     if (!cat || bottom_vecs_[i].size() < 2) continue;
-    vector<ROIPoolingLayer<Dtype>*> producers;
+    vector<int> offset(L, -1);  // per layer: the channel offset at which a producer writes the Concat top
     bool ok = true;
     int total = 0;
     for (size_t b = 0; b < bottom_id_vecs_[i].size() && ok; ++b) {
@@ -289,35 +295,35 @@ void Net<Dtype>::FuseLayers() {
         for (size_t bb = 0; bb < bottom_id_vecs_[k].size(); ++bb)
           if (bottom_id_vecs_[k][bb] == blob_id) ++readers;
       }
-      ROIPoolingLayer<Dtype>* rp = writer >= 0 ? dynamic_cast<ROIPoolingLayer<Dtype>*>(layers_[writer].get()) : NULL;
       const int c = bottom_vecs_[i][b]->channels();
-      if (!rp || readers != 1 || c % 64 != 0) ok = false;
-      producers.push_back(rp);
+      if (writer < 0 || !dynamic_cast<ROIPoolingLayer<Dtype>*>(layers_[writer].get()) || readers != 1 || c % 64 != 0)
+        ok = false;
+      else
+        offset[writer] = total;
       total += c;
     }
     if (!ok) continue;
-    int off = 0;
-    vector<typename ROIPoolingLayer<Dtype>::Sibling> sibs;
-    for (size_t b = 0; b < producers.size(); ++b) {
-      producers[b]->set_concat_target(top_vecs_[i][0], off, total);
-      off += bottom_vecs_[i][b]->channels();
-    }
-    for (int k = 0; k < L; ++k)  // execution order
-      for (size_t b = 0; b < producers.size(); ++b)
-        if (layers_[k].get() == producers[b]) {
-          typename ROIPoolingLayer<Dtype>::Sibling sb = {producers[b], bottom_vecs_[k][0], bottom_vecs_[k][1]};
-          sibs.push_back(sb);
-        }
-    // only the FIRST producer in execution order leads; it needs every sibling's inputs
-    if (!sibs.empty()) {
-      sibs[0].layer->set_siblings(sibs);
-      int leader = -1;
-      for (int k = 0; k < L; ++k) {
-        for (size_t b = 0; b < sibs.size(); ++b)
-          if (layers_[k].get() == sibs[b].layer) {
-            if (leader < 0) leader = k;
-            else fused_producer_[k] = leader;
-          }
+    // The first producer in execution order leads.  A later one that pools the same feature map with the same ROIs
+    // (Split tops share their bottom's storage) and the same geometry joins the leader's launch, up to the kernel's 4
+    // variants; any other producer launches its own.
+    int leader = -1, variants = 0;
+    for (int k = 0; k < L; ++k) {
+      if (offset[k] < 0) continue;
+      ROIPoolingLayer<Dtype>* rp = static_cast<ROIPoolingLayer<Dtype>*>(layers_[k].get());
+      rp->set_concat_target(top_vecs_[i][0], offset[k], total);
+      if (leader < 0) {
+        leader = k;
+        variants = 1;
+        continue;
+      }
+      const ROIPoolingParameter& p = rp->layer_param().roi_pooling_param();
+      const ROIPoolingParameter& q = layers_[leader]->layer_param().roi_pooling_param();
+      if (variants < 4 && storage_blob_[bottom_id_vecs_[k][0]] == storage_blob_[bottom_id_vecs_[leader][0]] &&
+          storage_blob_[bottom_id_vecs_[k][1]] == storage_blob_[bottom_id_vecs_[leader][1]] &&
+          p.pooled_h() == q.pooled_h() && p.pooled_w() == q.pooled_w() && p.spatial_scale() == q.spatial_scale()) {
+        static_cast<ROIPoolingLayer<Dtype>*>(layers_[leader].get())->add_follower(rp);
+        fused_producer_[k] = leader;
+        ++variants;
       }
     }
     cat->set_fused(true);
@@ -325,8 +331,8 @@ void Net<Dtype>::FuseLayers() {
 }
 
 // (c) a 2x2 / stride-2 MAX Pooling whose bottom was written by a Convolution (possibly through its
-// fused in-place ReLU) is computed in that convolution's epilogue.  If nothing else reads the
-// un-pooled blob it is not written at all.
+// fused in-place ReLU) is computed in that convolution's epilogue whenever the extents are even
+// (epilogue_pools).  If nothing else reads the un-pooled blob it is then not written at all.
 template <typename Dtype>
 void Net<Dtype>::FusePooling() {
   const int L = (int)layers_.size();
@@ -350,7 +356,7 @@ void Net<Dtype>::FusePooling() {
     }
     if (!ok || conv_idx < 0) continue;
     ConvolutionLayer<Dtype>* conv = static_cast<ConvolutionLayer<Dtype>*>(layers_[conv_idx].get());
-    if (conv->num_output() % 64 != 0) continue;
+    if (!conv->can_fuse_pool()) continue;
     // other readers of the un-pooled blob (in-place layers excluded)?
     int readers = 0;
     for (int k = 0; k < L; ++k) {
@@ -364,9 +370,20 @@ void Net<Dtype>::FusePooling() {
     bool is_net_output = false;
     for (size_t o = 0; o < net_output_blob_indices_.size(); ++o)
       is_net_output = is_net_output || (net_output_blob_indices_[o] == blob_id);
-    conv->set_fused_pool(pool, top_vecs_[i][0], readers > 0 || is_net_output);
+    conv->set_fused_pool(top_vecs_[i][0], readers > 0 || is_net_output);
+    pool->set_fused(true);
     fused_producer_[i] = conv_idx;
   }
+}
+
+template <typename Dtype>
+int Net<Dtype>::last_reader(const string& blob_name) const {
+  const int storage = storage_blob_[blob_names_index_.at(blob_name)];
+  int last = -1;
+  for (size_t i = 0; i < layers_.size(); ++i)
+    for (size_t b = 0; b < bottom_id_vecs_[i].size(); ++b)
+      if (storage_blob_[bottom_id_vecs_[i][b]] == storage) last = (int)i;
+  return last;
 }
 
 template <typename Dtype>
@@ -451,7 +468,6 @@ Dtype Net<Dtype>::ForwardFromTo(int start, int end) {
   CHECK_GE(start, 0);
   CHECK_LT(end, (int)layers_.size());
   start = fused_producer(start);  // a range never starts inside a fused group (net.hpp fused_producer)
-  for (size_t i = 0; i < layers_.size(); ++i) layers_[i]->ResetFusedState();
   if (GraphForward(start, end)) {
     if (!lazy_rows_) ResolveRows();
     return Dtype(0);

@@ -2,7 +2,6 @@
 // gateway matlab/+caffe/private/caffe_.cpp and pycaffe's _caffe.cpp play in the reference).
 // Lookup failures return MSCNN_ERR_INVALID; structural errors abort like Caffe (LOG(FATAL)).
 #include <cstring>
-#include <algorithm>
 #include <sstream>
 #include <string>
 
@@ -388,17 +387,6 @@ int mscnn_net_set_blob_async(void* h, const char* name, const float* host, long 
         cudaEventCreateWithFlags(&nh->inputs_consumed, cudaEventDisableTiming) != cudaSuccess)
       return MSCNN_ERR_CUDA;
   }
-  // last layer that reads the blob, looking through Split layers (their tops share the blob's storage)
-  int consumer = -1;
-  const std::vector<std::vector<Blob<float>*> >& bv = net->bottom_vecs();
-  const std::vector<std::vector<Blob<float>*> >& tv = net->top_vecs();
-  std::vector<Blob<float>*> aliases(1, b);
-  for (size_t i = 0; i < bv.size(); ++i)
-    for (Blob<float>* q : bv[i])
-      if (std::find(aliases.begin(), aliases.end(), q) != aliases.end()) {
-        consumer = (int)i;
-        if (std::string(net->layers()[i]->type()) == "Split") aliases.insert(aliases.end(), tv[i].begin(), tv[i].end());
-      }
   float* dst = b->mutable_gpu_data();
   if (nh->consumed_valid && cudaStreamWaitEvent(nh->copy_stream, nh->inputs_consumed, 0) != cudaSuccess) return MSCNN_ERR_CUDA;
   if (!nh->consumed_valid) {
@@ -411,7 +399,7 @@ int mscnn_net_set_blob_async(void* h, const char* name, const float* host, long 
       cudaEventRecord(nh->input_ready, nh->copy_stream) != cudaSuccess)
     return MSCNN_ERR_CUDA;
   nh->pending_input = true;
-  nh->pending_consumer = consumer;
+  nh->pending_consumer = net->last_reader(name);
   return MSCNN_OK;
 }
 // CUDA-graph replay of whole forwards (Net::set_graph_mode): off by default

@@ -103,8 +103,9 @@ def _layer_io(net):
 
 
 def _unstored_blobs(net):
-    """Blobs the fused net never writes: the un-pooled output of a convolution whose pooling runs in its epilogue,
-    and the tops of ROIPooling layers that write straight into their Concat's output."""
+    """Blobs the fused net never writes: the un-pooled output of a convolution whose pooling runs in its epilogue (at
+    even extents; at odd ones the convolution stores it and the Pooling runs itself), and the tops of ROIPooling layers
+    that write straight into their Concat's output."""
     io = _layer_io(net)
     skip = set()
     for name, typ in zip(net.layer_names, net.layer_types):
@@ -112,7 +113,9 @@ def _unstored_blobs(net):
         if prod == name:
             continue
         if typ == "Pooling":
-            skip.update(io[name][0][:1])
+            bottom = io[name][0][0]
+            if all(e % 2 == 0 for e in net.blob_shape(bottom)[2:]):
+                skip.add(bottom)
         elif typ == "ROIPooling":
             skip.update(io[name][1])
             skip.update(io[prod][1])
@@ -127,6 +130,8 @@ def _same(a, b):
 NETS = [
     ("kitti8s_fp32", "kitti", (192, 640, 8, False), "fp32"),
     ("kitti8s_bf16", "kitti", (192, 640, 8, False), "bf16"),
+    # conv3_3 is 25 x 81: pool3 runs itself, pool1 and pool2 stay in their convolutions' epilogues
+    ("kitti8s_odd", "kitti", (100, 324, 8, False), "fp32"),
     ("kitti7s_2x", "kitti", (96, 320, 7, True), "fp32"),
     ("kitti_cascade", "kitti_cascade", (96, 320), "fp32"),
     ("wider_cascade", "widerface_cascade", (128, 192), "fp32"),
@@ -179,6 +184,9 @@ def test_unfused_and_synced_nets_are_bit_identical(cuda, case, monkeypatch):
     base = nets["default"]
     skip = _unstored_blobs(base)
     assert not _unstored_blobs(nets["MSCNN_NO_FUSION"])
+    if (h, w) == (100, 324):
+        assert base.fused_producer("pool3") == "conv3_3" and "conv3_3" not in skip
+        assert {"conv1_2", "conv2_2"} <= skip
     assert sum(props["default"]) > 0
     for variant in ("MSCNN_NO_FUSION", "MSCNN_SYNC_ROWS"):
         net = nets[variant]
