@@ -412,6 +412,17 @@ MSCNN_API int mscnn_preprocess_forward_sized(void* plan, int N, const int* in_hw
                                              float* data, void* stream);
 MSCNN_API int mscnn_preprocess_forward_sized_host(void* plan, int N, const int* in_hw,
                                                   const unsigned char* host_images, float* data, void* stream);
+/* Grayscale frames ([h][w] or [h][w][1] uint8, as imread returns them) beside colour ones, in any mix and sizes.  The
+ * cascade drivers repmat a gray frame to three channels (examples/kitti_car/run_cascademscnn.m:76,
+ * examples/citypersons/run_cascademscnn.m:82); slot n of `data` equals bit for bit the result for that repmat'ed frame.
+ *   in_c: HOST int [N] = channels of each image, 1 (gray) or 3 (RGB); NULL = all 3, which is the _sized entry.  Image n
+ *   starts at byte sum_{m<n} h_m * w_m * c_m.  Any other channel count returns MSCNN_ERR_INVALID before any CUDA call.
+ * A plan's staging and intermediate buffers are rewritten by every call: a call on another stream than the plan's
+ * previous one first waits, on the device, for that call's launches (an event the plan records behind them). */
+MSCNN_API int mscnn_preprocess_forward_sized_c(void* plan, int N, const int* in_hw, const int* in_c,
+                                               const unsigned char* images, float* data, void* stream);
+MSCNN_API int mscnn_preprocess_forward_sized_c_host(void* plan, int N, const int* in_hw, const int* in_c,
+                                                    const unsigned char* host_images, float* data, void* stream);
 /* Host-only helpers (no CUDA call; usable on a GPU-less box):
  * imresize's tap tables for one dimension: returns the tap count P (<= cap_taps) and fills
  * host_weights / host_indices as [out_len][cap_taps] (0-based indices); mscnn_imresize_taps = P alone. */
@@ -512,6 +523,28 @@ MSCNN_API int mscnn_net_set_input_images(void* net, const char* blob, void* prep
  * batch k + 1, detect batch k" pairs each batch with its own sizes.  mscnn_net_set_input_images drops recorded sizes. */
 MSCNN_API int mscnn_net_set_input_images_sized(void* net, const char* blob, void* preprocess_plan, int N,
                                                const int* in_hw, const unsigned char* host_images);
+/* The same with gray frames among them: in_c [N] as in mscnn_preprocess_forward_sized_c (NULL = all colour). */
+MSCNN_API int mscnn_net_set_input_images_sized_c(void* net, const char* blob, void* preprocess_plan, int N,
+                                                 const int* in_hw, const int* in_c, const unsigned char* host_images);
+/* Pre-processing of the NEXT forward's frames while the current forward runs: what mscnn_net_set_input_images /
+ * _sized_c do (staging copy, both resize passes into the blob, recorded sizes), issued on the net's private copy stream
+ * (mscnn_net_copy_stream) exactly as mscnn_net_set_blob_async orders its copy.  That stream first waits, on the device,
+ * for the point where the forward in flight has stopped reading `blob` (the whole graph of a replayed forward); the next
+ * mscnn_net_forward waits for the work on the device, never on the host.  The recorded sizes are the geometry of that
+ * next forward, so "forward k, set k + 1, detect k" pairs each batch with its own sizes.  The blob must already have
+ * the batch's shape (N x 3 x out_h x out_w).
+ * Who waits for what: the plan's device staging and intermediate buffers are reused in stream order (another stream
+ * waits for the plan's previous call, see mscnn_preprocess_forward_sized_c).  host_images is read by the H2D copy on the
+ * copy stream: it must stay valid until that copy has run, which a host wait on an event recorded on
+ * mscnn_net_copy_stream after this call, or on anything queued behind the next forward, guarantees (pageable memory is
+ * copied out before the call returns). */
+MSCNN_API int mscnn_net_set_input_images_async(void* net, const char* blob, void* preprocess_plan, int N,
+                                               const unsigned char* host_images);
+MSCNN_API int mscnn_net_set_input_images_sized_async(void* net, const char* blob, void* preprocess_plan, int N,
+                                                     const int* in_hw, const int* in_c,
+                                                     const unsigned char* host_images);
+/* The copy stream of the *_async entries (a cudaStream_t, created on first use; NULL if it cannot be created). */
+MSCNN_API void* mscnn_net_copy_stream(void* net);
 MSCNN_API int mscnn_net_set_input_geometry(void* net, int N, const int* org_hw);
 MSCNN_API int mscnn_net_forward(void* net, int from_layer, int to_layer); /* inclusive; to < 0 = last */
 /* mscnn_net_forward returns with the forward QUEUED on the stream: no layer waits for the device, not even BoxOutput,

@@ -221,6 +221,9 @@ def _declare(L: C.CDLL) -> None:
     for f in ("mscnn_preprocess_forward_sized", "mscnn_preprocess_forward_sized_host"):
         getattr(L, f).restype = c_int
         getattr(L, f).argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    for f in ("mscnn_preprocess_forward_sized_c", "mscnn_preprocess_forward_sized_c_host"):
+        getattr(L, f).restype = c_int
+        getattr(L, f).argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     L.mscnn_imresize_taps.restype = c_int
     L.mscnn_imresize_taps.argtypes = [c_int, c_int]
     L.mscnn_imresize_contributions.restype = c_int

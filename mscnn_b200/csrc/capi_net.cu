@@ -46,16 +46,49 @@ int settle_pending(NetHandle* nh) {
   return cudaStreamWaitEvent(Caffe::stream(), nh->input_ready, 0) == cudaSuccess ? MSCNN_OK : MSCNN_ERR_CUDA;
 }
 // The input blob `name` as the destination of plan's pre-processing of N images: it must hold exactly N images of the
-// plan's output size.  A pending asynchronous upload is settled first.
-int preprocess_target(NetHandle* nh, const char* name, void* plan, int N, float** dst) {
+// plan's output size.
+int images_target(NetHandle* nh, const char* name, void* plan, int N, Blob<float>** dst) {
   nh->net->ResolveRowsFor(name);
   if (!nh->net->has_blob(name)) return MSCNN_ERR_INVALID;
   mscnn_preprocess_desc d;
   if (mscnn_preprocess_get_desc(plan, &d) != MSCNN_OK) return MSCNN_ERR_INVALID;
   Blob<float>* b = nh->net->blob_by_name(name).get();
   if (b->count() != (long)N * 3 * d.out_h * d.out_w) return MSCNN_ERR_INVALID;
+  *dst = b;
+  return MSCNN_OK;
+}
+// The same for a synchronous write: a pending asynchronous upload is settled first.
+int preprocess_target(NetHandle* nh, const char* name, void* plan, int N, float** dst) {
+  Blob<float>* b = nullptr;
+  const int rc = images_target(nh, name, plan, N, &b);
+  if (rc) return rc;
   if (settle_pending(nh) != MSCNN_OK) return MSCNN_ERR_CUDA;
   *dst = b->mutable_gpu_data();
+  return MSCNN_OK;
+}
+// Asynchronous input writes (mscnn_net_set_blob_async, mscnn_net_set_input_images*_async) go on the net's copy stream,
+// which first waits, on the device, for the point where the forward in flight no longer reads the input blob.
+int async_begin(NetHandle* nh) {
+  if (!nh->copy_stream) {
+    if (cudaStreamCreateWithFlags(&nh->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&nh->input_ready, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&nh->inputs_consumed, cudaEventDisableTiming) != cudaSuccess)
+      return MSCNN_ERR_CUDA;
+  }
+  if (nh->consumed_valid && cudaStreamWaitEvent(nh->copy_stream, nh->inputs_consumed, 0) != cudaSuccess) return MSCNN_ERR_CUDA;
+  if (!nh->consumed_valid) {
+    // no forward has recorded a consumption point yet: order after everything queued on the net stream
+    if (cudaEventRecord(nh->inputs_consumed, Caffe::stream()) != cudaSuccess ||
+        cudaStreamWaitEvent(nh->copy_stream, nh->inputs_consumed, 0) != cudaSuccess)
+      return MSCNN_ERR_CUDA;
+  }
+  return MSCNN_OK;
+}
+// ... and mark the write as the next forward's input: that forward waits for input_ready on the device.
+int async_end(NetHandle* nh, const char* name) {
+  if (cudaEventRecord(nh->input_ready, nh->copy_stream) != cudaSuccess) return MSCNN_ERR_CUDA;
+  nh->pending_input = true;
+  nh->pending_consumer = nh->net->last_reader(name);
   return MSCNN_OK;
 }
 // The post-process inputs of the last forward, as every mscnn_net_detect* entry needs them.
@@ -269,19 +302,61 @@ int mscnn_net_set_input_images(void* h, const char* name, void* plan, int N, con
   return mscnn_preprocess_forward_host(plan, N, host_images, dst, Caffe::stream());
 }
 // The same for images of different original sizes (run_mscnn_detection.m:64-65 reads each frame's size): records
-// them as the geometry of the next forward.
-int mscnn_net_set_input_images_sized(void* h, const char* name, void* plan, int N, const int* in_hw,
-                                     const unsigned char* host_images) {
+// them as the geometry of the next forward.  in_c: channels per image (1 = gray, 3 = colour), NULL = all colour.
+int mscnn_net_set_input_images_sized_c(void* h, const char* name, void* plan, int N, const int* in_hw, const int* in_c,
+                                       const unsigned char* host_images) {
   if (N < 1 || !in_hw || !host_images) return MSCNN_ERR_INVALID;
   for (int n = 0; n < N; ++n)
-    if (in_hw[2 * n] < 1 || in_hw[2 * n + 1] < 1) return MSCNN_ERR_INVALID;
+    if (in_hw[2 * n] < 1 || in_hw[2 * n + 1] < 1 || (in_c && in_c[n] != 1 && in_c[n] != 3)) return MSCNN_ERR_INVALID;
   float* dst = nullptr;
   int rc = preprocess_target(H(h), name, plan, N, &dst);
   if (rc) return rc;
-  rc = mscnn_preprocess_forward_sized_host(plan, N, in_hw, host_images, dst, Caffe::stream());
+  rc = mscnn_preprocess_forward_sized_c_host(plan, N, in_hw, in_c, host_images, dst, Caffe::stream());
   if (rc != MSCNN_OK) return rc;
   H(h)->next_org_hw.assign(in_hw, in_hw + 2 * N);
   return MSCNN_OK;
+}
+int mscnn_net_set_input_images_sized(void* h, const char* name, void* plan, int N, const int* in_hw,
+                                     const unsigned char* host_images) {
+  return mscnn_net_set_input_images_sized_c(h, name, plan, N, in_hw, nullptr, host_images);
+}
+// The pre-processing of the NEXT forward's images while the current one runs: the staging copy and both resize passes
+// go on the copy stream, behind the point where the forward in flight has stopped reading the blob; the next
+// mscnn_net_forward waits for them on the device.  in_hw NULL = N images of the plan's own size (no recorded sizes).
+static int set_input_images_async(void* h, const char* name, void* plan, int N, const int* in_hw, const int* in_c,
+                                  const unsigned char* host_images) {
+  NetHandle* nh = H(h);
+  if (N < 1 || !host_images) return MSCNN_ERR_INVALID;
+  if (in_hw)
+    for (int n = 0; n < N; ++n)
+      if (in_hw[2 * n] < 1 || in_hw[2 * n + 1] < 1 || (in_c && in_c[n] != 1 && in_c[n] != 3)) return MSCNN_ERR_INVALID;
+  Blob<float>* b = nullptr;
+  int rc = images_target(nh, name, plan, N, &b);
+  if (rc) return rc;
+  if ((rc = async_begin(nh)) != MSCNN_OK) return rc;
+  float* dst = b->mutable_gpu_data();
+  rc = in_hw ? mscnn_preprocess_forward_sized_c_host(plan, N, in_hw, in_c, host_images, dst, nh->copy_stream)
+             : mscnn_preprocess_forward_host(plan, N, host_images, dst, nh->copy_stream);
+  if (rc != MSCNN_OK) return rc;
+  if ((rc = async_end(nh, name)) != MSCNN_OK) return rc;
+  if (in_hw)
+    nh->next_org_hw.assign(in_hw, in_hw + 2 * N);
+  else
+    nh->next_org_hw.clear();
+  return MSCNN_OK;
+}
+int mscnn_net_set_input_images_async(void* h, const char* name, void* plan, int N, const unsigned char* host_images) {
+  return set_input_images_async(h, name, plan, N, nullptr, nullptr, host_images);
+}
+int mscnn_net_set_input_images_sized_async(void* h, const char* name, void* plan, int N, const int* in_hw,
+                                           const int* in_c, const unsigned char* host_images) {
+  if (!in_hw) return MSCNN_ERR_INVALID;
+  return set_input_images_async(h, name, plan, N, in_hw, in_c, host_images);
+}
+void* mscnn_net_copy_stream(void* h) {
+  NetHandle* nh = H(h);
+  if (!nh->copy_stream && async_begin(nh) != MSCNN_OK) return nullptr;
+  return nh->copy_stream;
 }
 int mscnn_net_set_input_geometry(void* h, int N, const int* org_hw) {
   if (N < 0) return MSCNN_ERR_INVALID;
@@ -381,26 +456,12 @@ int mscnn_net_set_blob_async(void* h, const char* name, const float* host, long 
   if (!net->has_blob(name)) return MSCNN_ERR_INVALID;
   Blob<float>* b = net->blob_by_name(name).get();
   if (b->count() != count) return MSCNN_ERR_INVALID;
-  if (!nh->copy_stream) {
-    if (cudaStreamCreateWithFlags(&nh->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&nh->input_ready, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&nh->inputs_consumed, cudaEventDisableTiming) != cudaSuccess)
-      return MSCNN_ERR_CUDA;
-  }
+  int rc = async_begin(nh);
+  if (rc) return rc;
   float* dst = b->mutable_gpu_data();
-  if (nh->consumed_valid && cudaStreamWaitEvent(nh->copy_stream, nh->inputs_consumed, 0) != cudaSuccess) return MSCNN_ERR_CUDA;
-  if (!nh->consumed_valid) {
-    // no forward has recorded a consumption point yet: order after everything queued on the net stream
-    if (cudaEventRecord(nh->inputs_consumed, Caffe::stream()) != cudaSuccess ||
-        cudaStreamWaitEvent(nh->copy_stream, nh->inputs_consumed, 0) != cudaSuccess)
-      return MSCNN_ERR_CUDA;
-  }
-  if (cudaMemcpyAsync(dst, host, sizeof(float) * count, cudaMemcpyHostToDevice, nh->copy_stream) != cudaSuccess ||
-      cudaEventRecord(nh->input_ready, nh->copy_stream) != cudaSuccess)
+  if (cudaMemcpyAsync(dst, host, sizeof(float) * count, cudaMemcpyHostToDevice, nh->copy_stream) != cudaSuccess)
     return MSCNN_ERR_CUDA;
-  nh->pending_input = true;
-  nh->pending_consumer = net->last_reader(name);
-  return MSCNN_OK;
+  return async_end(nh, name);
 }
 // CUDA-graph replay of whole forwards (Net::set_graph_mode): off by default
 int mscnn_net_set_graph(void* h, int on) {

@@ -19,6 +19,12 @@
 // Tap tables are built on the host in fp64 (mscnn_imresize_contributions, testable without a GPU); the
 // kernels multiply and add in the table's tap order without FMA contraction (-fmad=false), so the result
 // is bit-identical to the numpy restatement in oracle/port.py.
+//
+// Grayscale frames ([h][w] or [h][w][1], as imread returns them): the cascade drivers turn them into RGB first
+// (`if (size(img,3)==1), img = repmat(img,[1 1 3]); end`, examples/kitti_car/run_cascademscnn.m:76,
+// examples/citypersons/run_cascademscnn.m:82).  imresize works per channel, so the three copies would resize to the
+// same bytes: here the one channel is resized once, and the second pass writes its value into all three planes,
+// each minus its own mean.  The result is bit for bit that of the repmat'ed frame.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>
@@ -113,6 +119,11 @@ struct PreprocessPlan {
   size_t mid_cap = 0;
   unsigned char* stage = nullptr;  // device copy of host images (mscnn_preprocess_forward*_host)
   size_t stage_cap = 0;
+  // `stage` and `mid` are rewritten by every call.  A call issued on another stream than the previous one first makes
+  // its stream wait, on the device, for this event, recorded behind the previous call's last launch.
+  cudaEvent_t used = nullptr;
+  cudaStream_t used_on = nullptr;
+  bool used_valid = false;
 };
 
 // One image of a batch as both passes see it.  The descriptors of a launch travel by value in the kernel parameter
@@ -120,6 +131,7 @@ struct PreprocessPlan {
 struct ImageDesc {
   size_t src, mid;  // byte offsets of the image in the input batch and of its intermediate image
   int in_h, in_w;   // original size
+  int channels;     // 3 (interleaved RGB) or 1 (gray: the one channel stands for all three)
   int mid_h, mid_w; // size after the first pass
   int first_dim;    // the first pass resizes along this dimension (0: height), the second along the other
   DevTable t1, t2;  // tap tables of the first and the second pass
@@ -138,23 +150,23 @@ __device__ __forceinline__ double round_u8(double v) {
   return round(v);
 }
 
-// First pass: resize image d[blockIdx.y] of the launch along one dimension, uint8 [h][w][3] -> uint8 [mid_h][mid_w][3].
-// One thread per output byte (the three channels of a pixel are adjacent bytes, so a warp writes 32 consecutive bytes
+// First pass: resize image d[blockIdx.y] of the launch along one dimension, uint8 [h][w][C] -> uint8 [mid_h][mid_w][C].
+// One thread per output byte (the C channels of a pixel are adjacent bytes, so a warp writes 32 consecutive bytes
 // and reads `taps` rows or pixel neighbourhoods that its lanes share).
 //   along = 0: out[y][x][c] = sum_k w[y][k] * in[idx[y][k]][x][c]   (out_h x in_w)
 //   along = 1: out[y][x][c] = sum_k w[x][k] * in[y][idx[x][k]][c]   (in_h x out_w)
-__global__ void imresize_pass_u8_kernel(const unsigned char* __restrict__ images, unsigned char* __restrict__ mid,
-                                        const ImageBatch b) {
-  const ImageDesc& D = b.d[blockIdx.y];
+template <int C>
+__device__ __forceinline__ void imresize_pass_u8(const ImageDesc& D, const unsigned char* __restrict__ images,
+                                                 unsigned char* __restrict__ mid) {
   const int in_w = D.in_w, out_w = D.mid_w, along = D.first_dim, taps = D.t1.taps;
   const double* __restrict__ w = D.t1.w;
   const int* __restrict__ idx = D.t1.idx;
   const unsigned char* img = images + D.src;
   unsigned char* out = mid + D.mid;
-  const size_t total = (size_t)D.mid_h * out_w * 3;
+  const size_t total = (size_t)D.mid_h * out_w * C;
   for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(e % 3);
-    const size_t p = e / 3;
+    const int c = (int)(e % C);
+    const size_t p = e / C;
     const int x = (int)(p % out_w);
     const int y = (int)(p / out_w);
     const int o = along == 0 ? y : x;
@@ -163,31 +175,56 @@ __global__ void imresize_pass_u8_kernel(const unsigned char* __restrict__ images
     double acc = 0.0;
     for (int k = 0; k < taps; ++k) {
       const int s = ir[k];
-      const size_t off = along == 0 ? ((size_t)s * in_w + x) * 3 + c : ((size_t)y * in_w + s) * 3 + c;
+      const size_t off = along == 0 ? ((size_t)s * in_w + x) * C + c : ((size_t)y * in_w + s) * C + c;
       acc = __dadd_rn(acc, __dmul_rn(wr[k], (double)img[off]));
     }
     out[e] = (unsigned char)round_u8(acc);
   }
 }
 
+__global__ void imresize_pass_u8_kernel(const unsigned char* __restrict__ images, unsigned char* __restrict__ mid,
+                                        const ImageBatch b) {
+  const ImageDesc& D = b.d[blockIdx.y];
+  if (D.channels == 3)
+    imresize_pass_u8<3>(D, images, mid);
+  else
+    imresize_pass_u8<1>(D, images, mid);
+}
+
 // Second pass + channel swap + mean subtraction + HWC -> CHW, into slot b.n0 + blockIdx.y of the blob.  One thread
 // per output pixel; a warp writes 32 consecutive floats of each of the three output planes.
-__global__ void imresize_pass_to_blob_kernel(const unsigned char* __restrict__ mid, float* __restrict__ data,
-                                             int out_h, int out_w, const ImageBatch b, float mean0, float mean1,
-                                             float mean2, int swap_rb) {
-  const ImageDesc& D = b.d[blockIdx.y];
+template <int C>
+__device__ __forceinline__ void imresize_pass_to_blob(const ImageDesc& D, const unsigned char* __restrict__ mid,
+                                                      float* __restrict__ data, int out_h, int out_w, int n,
+                                                      float mean0, float mean1, float mean2, int swap_rb) {
   const int in_w = D.mid_w, along = 1 - D.first_dim, taps = D.t2.taps;
   const double* __restrict__ w = D.t2.w;
   const int* __restrict__ idx = D.t2.idx;
   const unsigned char* img = mid + D.mid;
   const size_t plane = (size_t)out_h * out_w;
-  float* out = data + (size_t)(b.n0 + blockIdx.y) * 3 * plane;
+  float* out = data + (size_t)n * 3 * plane;
   for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < plane; e += (size_t)gridDim.x * blockDim.x) {
     const int x = (int)(e % out_w);
     const int y = (int)(e / out_w);
     const int o = along == 0 ? y : x;
     const double* wr = w + (size_t)o * taps;
     const int* ir = idx + (size_t)o * taps;
+    float* dst = out + (size_t)y * out_w + x;
+    if (C == 1) {
+      // gray: the three channels of the repmat'ed frame are equal, whatever the swap
+      double a = 0.0;
+#pragma unroll 1
+      for (int k = 0; k < taps; ++k) {
+        const int s = ir[k];
+        const unsigned char* q = img + (along == 0 ? (size_t)s * in_w + x : (size_t)y * in_w + s);
+        a = __dadd_rn(a, __dmul_rn(wr[k], (double)q[0]));
+      }
+      const float v = (float)round_u8(a);
+      dst[0] = v - mean0;
+      dst[plane] = v - mean1;
+      dst[2 * plane] = v - mean2;
+      continue;
+    }
     double a0 = 0.0, a1 = 0.0, a2 = 0.0;
     for (int k = 0; k < taps; ++k) {
       const int s = ir[k];
@@ -198,12 +235,21 @@ __global__ void imresize_pass_to_blob_kernel(const unsigned char* __restrict__ m
       a2 = __dadd_rn(a2, __dmul_rn(wk, (double)q[2]));
     }
     const float v0 = (float)round_u8(a0), v1 = (float)round_u8(a1), v2 = (float)round_u8(a2);
-    float* dst = out + (size_t)y * out_w + x;
     // output channel order after test_image(:,:,[3 2 1]): plane 0 = input channel 2 when swapping
     dst[0] = (swap_rb ? v2 : v0) - mean0;
     dst[plane] = v1 - mean1;
     dst[2 * plane] = (swap_rb ? v0 : v2) - mean2;
   }
+}
+
+__global__ void imresize_pass_to_blob_kernel(const unsigned char* __restrict__ mid, float* __restrict__ data,
+                                             int out_h, int out_w, const ImageBatch b, float mean0, float mean1,
+                                             float mean2, int swap_rb) {
+  const ImageDesc& D = b.d[blockIdx.y];
+  if (D.channels == 3)
+    imresize_pass_to_blob<3>(D, mid, data, out_h, out_w, b.n0 + blockIdx.y, mean0, mean1, mean2, swap_rb);
+  else
+    imresize_pass_to_blob<1>(D, mid, data, out_h, out_w, b.n0 + blockIdx.y, mean0, mean1, mean2, swap_rb);
 }
 
 // No resize needed in a dimension (out == in): imresize still runs the pass, and the cubic kernel at
@@ -259,10 +305,11 @@ static int tables_for(PreprocessPlan* p, int in_h, int in_w, int* index) {
   return MSCNN_OK;
 }
 
-static bool sizes_valid(int N, const int* in_hw) {
+// Sizes >= 1; channel counts 1 or 3 (in_c NULL: every image is colour).
+static bool sizes_valid(int N, const int* in_hw, const int* in_c = nullptr) {
   if (N < 1 || !in_hw) return false;
   for (int n = 0; n < N; ++n)
-    if (in_hw[2 * n] < 1 || in_hw[2 * n + 1] < 1) return false;
+    if (in_hw[2 * n] < 1 || in_hw[2 * n + 1] < 1 || (in_c && in_c[n] != 1 && in_c[n] != 3)) return false;
   return true;
 }
 
@@ -280,10 +327,11 @@ static unsigned grid_x(size_t work, unsigned cap) {
   return (unsigned)(blocks > cap ? cap : blocks);
 }
 
-// Images packed back to back in batch order (image n starts at byte sum_{m<n} h_m w_m 3) -> data [N][3][out_h][out_w].
-// Both passes cover up to kImagesPerLaunch images per launch, image = blockIdx.y.
-static int forward_sized(PreprocessPlan* p, int N, const int* in_hw, const unsigned char* images, float* data,
-                         cudaStream_t st) {
+// Images packed back to back in batch order (image n starts at byte sum_{m<n} h_m w_m c_m) -> data
+// [N][3][out_h][out_w].  `host` images are first copied into the plan's staging buffer on `st`.  Both passes cover up to
+// kImagesPerLaunch images per launch, image = blockIdx.y.
+static int forward_sized(PreprocessPlan* p, int N, const int* in_hw, const int* in_c, const unsigned char* images,
+                         bool host, float* data, cudaStream_t st) {
   const mscnn_preprocess_desc& d = p->d;
   std::vector<ImageDesc> desc(N);
   size_t src = 0, mid = 0;
@@ -297,16 +345,24 @@ static int forward_sized(PreprocessPlan* p, int N, const int* in_hw, const unsig
     D.mid = mid;
     D.in_h = s.in_h;
     D.in_w = s.in_w;
+    D.channels = in_c ? in_c[n] : 3;
     D.first_dim = s.first_dim;
     D.mid_h = s.first_dim == 0 ? d.out_h : s.in_h;
     D.mid_w = s.first_dim == 0 ? s.in_w : d.out_w;
     D.t1 = s.first_dim == 0 ? s.th : s.tw;
     D.t2 = s.first_dim == 0 ? s.tw : s.th;
-    src += (size_t)s.in_h * s.in_w * 3;
-    mid += (size_t)D.mid_h * D.mid_w * 3;
+    src += (size_t)s.in_h * s.in_w * D.channels;
+    mid += (size_t)D.mid_h * D.mid_w * D.channels;
   }
-  const int rc = grow(&p->mid, &p->mid_cap, mid);
+  int rc = grow(&p->mid, &p->mid_cap, mid);
+  if (rc == MSCNN_OK && host) rc = grow(&p->stage, &p->stage_cap, src);
   if (rc != MSCNN_OK) return rc;
+  if (!p->used && cudaEventCreateWithFlags(&p->used, cudaEventDisableTiming) != cudaSuccess) return MSCNN_ERR_CUDA;
+  if (p->used_valid && p->used_on != st && cudaStreamWaitEvent(st, p->used, 0) != cudaSuccess) return MSCNN_ERR_CUDA;
+  if (host) {
+    if (cudaMemcpyAsync(p->stage, images, src, cudaMemcpyHostToDevice, st) != cudaSuccess) return MSCNN_ERR_CUDA;
+    images = p->stage;
+  }
   const size_t px = (size_t)d.out_h * d.out_w;
   for (int n0 = 0; n0 < N; n0 += kImagesPerLaunch) {
     const int count = N - n0 < kImagesPerLaunch ? N - n0 : kImagesPerLaunch;
@@ -315,7 +371,7 @@ static int forward_sized(PreprocessPlan* p, int N, const int* in_hw, const unsig
     size_t mid_max = 0;
     for (int i = 0; i < count; ++i) {
       b.d[i] = desc[n0 + i];
-      const size_t m = (size_t)b.d[i].mid_h * b.d[i].mid_w * 3;
+      const size_t m = (size_t)b.d[i].mid_h * b.d[i].mid_w * b.d[i].channels;
       if (m > mid_max) mid_max = m;
     }
     const unsigned cap = 132u * 64 / count;  // at most 132 x 64 blocks per launch, as before
@@ -326,6 +382,9 @@ static int forward_sized(PreprocessPlan* p, int N, const int* in_hw, const unsig
                                                                                d.swap_rb);
     note_launch();
   }
+  if (cudaEventRecord(p->used, st) != cudaSuccess) return MSCNN_ERR_CUDA;
+  p->used_on = st;
+  p->used_valid = true;
   return cudaPeekAtLastError() == cudaSuccess ? MSCNN_OK : MSCNN_ERR_CUDA;
 }
 
@@ -394,28 +453,33 @@ int mscnn_preprocess_destroy(void* plan) {
   for (SizeTables& s : p->sizes) free_tables(&s);
   cudaFree(p->mid);
   cudaFree(p->stage);
+  if (p->used) cudaEventDestroy(p->used);
   delete p;
   return MSCNN_OK;
 }
 
+int mscnn_preprocess_forward_sized_c(void* plan, int N, const int* in_hw, const int* in_c,
+                                     const unsigned char* images, float* data, void* stream) {
+  PreprocessPlan* p = static_cast<PreprocessPlan*>(plan);
+  if (!p || !sizes_valid(N, in_hw, in_c) || !images || !data) return MSCNN_ERR_INVALID;
+  return forward_sized(p, N, in_hw, in_c, images, false, data, (cudaStream_t)stream);
+}
+
+int mscnn_preprocess_forward_sized_c_host(void* plan, int N, const int* in_hw, const int* in_c,
+                                          const unsigned char* host_images, float* data, void* stream) {
+  PreprocessPlan* p = static_cast<PreprocessPlan*>(plan);
+  if (!p || !sizes_valid(N, in_hw, in_c) || !host_images || !data) return MSCNN_ERR_INVALID;
+  return forward_sized(p, N, in_hw, in_c, host_images, true, data, (cudaStream_t)stream);
+}
+
 int mscnn_preprocess_forward_sized(void* plan, int N, const int* in_hw, const unsigned char* images, float* data,
                                    void* stream) {
-  PreprocessPlan* p = static_cast<PreprocessPlan*>(plan);
-  if (!p || !sizes_valid(N, in_hw) || !images || !data) return MSCNN_ERR_INVALID;
-  return forward_sized(p, N, in_hw, images, data, (cudaStream_t)stream);
+  return mscnn_preprocess_forward_sized_c(plan, N, in_hw, nullptr, images, data, stream);
 }
 
 int mscnn_preprocess_forward_sized_host(void* plan, int N, const int* in_hw, const unsigned char* host_images,
                                         float* data, void* stream) {
-  PreprocessPlan* p = static_cast<PreprocessPlan*>(plan);
-  if (!p || !sizes_valid(N, in_hw) || !host_images || !data) return MSCNN_ERR_INVALID;
-  size_t bytes = 0;
-  for (int n = 0; n < N; ++n) bytes += (size_t)in_hw[2 * n] * in_hw[2 * n + 1] * 3;
-  int rc = grow(&p->stage, &p->stage_cap, bytes);
-  if (rc != MSCNN_OK) return rc;
-  if (cudaMemcpyAsync(p->stage, host_images, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream) != cudaSuccess)
-    return MSCNN_ERR_CUDA;
-  return forward_sized(p, N, in_hw, p->stage, data, (cudaStream_t)stream);
+  return mscnn_preprocess_forward_sized_c_host(plan, N, in_hw, nullptr, host_images, data, stream);
 }
 
 // The uniform batch: every image has the plan's own input size.

@@ -44,6 +44,11 @@ def _declare(L):
     L.mscnn_net_set_blob.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long]
     L.mscnn_net_set_input_images.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_void_p]
     L.mscnn_net_set_input_images_sized.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    L.mscnn_net_set_input_images_sized_c.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int] + [C.c_void_p] * 3
+    L.mscnn_net_set_input_images_async.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_void_p]
+    L.mscnn_net_set_input_images_sized_async.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int] + [C.c_void_p] * 3
+    L.mscnn_net_copy_stream.restype = C.c_void_p
+    L.mscnn_net_copy_stream.argtypes = [C.c_void_p]
     L.mscnn_net_set_input_geometry.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.mscnn_net_set_blob_async.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long]
     L.mscnn_net_set_blob_device.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long]
@@ -228,22 +233,59 @@ class Net:
         """uint8 host images [N][h][w][3] (numpy or pinned CPU tensor) -> device pre-processing (`pre` = an
         ops.Preprocess plan) -> the input blob; the MATLAB code before net.forward, run_mscnn_detection.m:64-69.
         A list of host uint8 [h][w][3] frames may mix original sizes: their sizes become the geometry of the next
-        forward, whose detections are then rescaled and clipped per frame (run_mscnn_detection.m:64-65, 111-116)."""
+        forward, whose detections are then rescaled and clipped per frame (run_mscnn_detection.m:64-65, 111-116).
+        Gray frames ([N][h][w] / [N][h][w][1] arrays, [h][w] / [h][w][1] list entries, mixed with colour ones in a
+        list) give what their repmat to three channels gives (run_cascademscnn.m:76)."""
         from . import ops
         sized = isinstance(images, (list, tuple))
-        hw = ops.image_sizes(images) if sized else None
-        n = len(hw) if sized else images.shape[0]
+        n = len(images) if sized else images.shape[0]
         shp = (n, 3, *pre.out_hw)
         if self.blob_shape(name) != shp:
             capi.check(self._L.mscnn_net_reshape_blob(self._h, name.encode(), *shp), "reshape_blob")
-        if not sized:
+        if not sized and not ops.is_gray_batch(images):
             capi.check(self._L.mscnn_net_set_input_images(self._h, name.encode(), pre.handle, n, capi.ptr(images)),
                        "set_input_images")
             return
-        packed = pre.pack_host(images)
-        capi.check(self._L.mscnn_net_set_input_images_sized(self._h, name.encode(), pre.handle, n, hw.ctypes.data,
-                                                            capi.ptr(packed)), "set_input_images_sized")
+        hw, ch = ops.image_sizes_channels(images if sized else list(images))
+        packed = pre.pack_host(images if sized else [images])
+        gray = bool((ch == 1).any())
+        if gray:
+            rc = self._L.mscnn_net_set_input_images_sized_c(self._h, name.encode(), pre.handle, n, hw.ctypes.data,
+                                                            ch.ctypes.data, capi.ptr(packed))
+        else:
+            rc = self._L.mscnn_net_set_input_images_sized(self._h, name.encode(), pre.handle, n, hw.ctypes.data,
+                                                          capi.ptr(packed))
+        capi.check(rc, "set_input_images_sized")
         pre.host_copy_issued(_net_stream())
+        if not sized:          # an array batch records no sizes: the detect cfg's geometry applies, as for colour
+            self.set_input_geometry(None)
+
+    def set_input_images_async(self, name: str, pre, images) -> None:
+        """set_input_images for the NEXT forward while the current one runs: the frames are packed into the plan's
+        pinned buffer, then the H2D copy and both resize passes run on the net's copy stream once the forward in flight
+        has stopped reading `name`; the next forward waits for them on the device.  The blob must already have the
+        batch's shape (set_input_images reshapes, this does not).  Same frame forms and recorded sizes as
+        set_input_images, so "forward k, set k + 1, detect k" pairs each batch with its own sizes."""
+        from . import ops
+        import torch
+        sized = isinstance(images, (list, tuple))
+        n = len(images) if sized else images.shape[0]
+        if self.blob_shape(name) != (n, 3, *pre.out_hw):
+            raise capi.MscnnError("set_input_images_async does not reshape: call set_input_images with this batch "
+                                  "shape first")
+        frames = images if sized else [images]
+        packed = pre.pack_host(frames)
+        if sized or ops.is_gray_batch(images):
+            hw, ch = ops.image_sizes_channels(images if sized else list(images))
+            rc = self._L.mscnn_net_set_input_images_sized_async(self._h, name.encode(), pre.handle, n, hw.ctypes.data,
+                                                                ch.ctypes.data, capi.ptr(packed))
+        else:
+            assert tuple(images.shape[1:]) == (*pre.in_hw, 3), (images.shape, pre.in_hw)
+            rc = self._L.mscnn_net_set_input_images_async(self._h, name.encode(), pre.handle, n, capi.ptr(packed))
+        capi.check(rc, "set_input_images_async")
+        pre.host_copy_issued(torch.cuda.ExternalStream(self._L.mscnn_net_copy_stream(self._h)))
+        if not sized:
+            self.set_input_geometry(None)
 
     def set_input_geometry(self, org_hw_list) -> None:
         """Original (h, w) of each image the NEXT forward consumes, for inputs resized by the caller and set with

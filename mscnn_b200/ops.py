@@ -474,9 +474,14 @@ class Preprocess:
 
     def __call__(self, images, out: torch.Tensor | None = None) -> torch.Tensor:
         """images: uint8 [N][h][w][3], a torch.cuda tensor, or a host numpy array / CPU tensor (H2D inside); or a
-        list of uint8 [h][w][3] images of any sizes, all torch.cuda tensors or all on the host."""
+        list of uint8 [h][w][3] images of any sizes, all torch.cuda tensors or all on the host.  Gray images
+        ([N][h][w] or [N][h][w][1]; [h][w] or [h][w][1] in a list, mixed with colour ones) give what their repmat to
+        three channels gives (run_cascademscnn.m:76)."""
         if isinstance(images, (list, tuple)):
             return self._call_sized(images, out)
+        if is_gray_batch(images):
+            assert tuple(images.shape[1:3]) == self.in_hw, (images.shape, self.in_hw)
+            return self._call_sized(list(images), out)
         n = images.shape[0]
         assert tuple(images.shape[1:]) == (*self.in_hw, 3) and images.dtype in (torch.uint8, np.uint8)
         if out is None:
@@ -492,20 +497,22 @@ class Preprocess:
         return out
 
     def _call_sized(self, images, out):
-        n, hw = len(images), image_sizes(images)
+        n = len(images)
+        hw, ch = image_sizes_channels(images)
         if out is None:
             out = torch.empty((n, 3, *self.out_hw), dtype=torch.float32, device="cuda")
         L = capi.lib()
         on_device = [isinstance(im, torch.Tensor) and im.is_cuda for im in images]
         if all(on_device):
             packed = torch.cat([im.reshape(-1) for im in images])
-            capi.check(L.mscnn_preprocess_forward_sized(self.handle, n, hw.ctypes.data, capi.ptr(packed),
-                                                        capi.ptr(out), _stream()), "preprocess_forward_sized")
+            capi.check(L.mscnn_preprocess_forward_sized_c(self.handle, n, hw.ctypes.data, ch.ctypes.data,
+                                                          capi.ptr(packed), capi.ptr(out), _stream()),
+                       "preprocess_forward_sized_c")
         elif not any(on_device):
             packed = self.pack_host(images)
-            capi.check(L.mscnn_preprocess_forward_sized_host(self.handle, n, hw.ctypes.data, capi.ptr(packed),
-                                                             capi.ptr(out), _stream()),
-                       "preprocess_forward_sized_host")
+            capi.check(L.mscnn_preprocess_forward_sized_c_host(self.handle, n, hw.ctypes.data, ch.ctypes.data,
+                                                               capi.ptr(packed), capi.ptr(out), _stream()),
+                       "preprocess_forward_sized_c_host")
             self.host_copy_issued(torch.cuda.current_stream())
         else:
             raise ValueError("a list of images must be all on the device or all on the host")
@@ -533,8 +540,23 @@ class Preprocess:
 
 
 def image_sizes(images) -> np.ndarray:
-    """int32 [N][2] = h, w of a list of uint8 [h][w][3] images."""
+    """int32 [N][2] = h, w of a list of uint8 [h][w][3] images (or gray [h][w] / [h][w][1] ones)."""
+    return image_sizes_channels(images)[0]
+
+
+def image_sizes_channels(images) -> tuple[np.ndarray, np.ndarray]:
+    """int32 [N][2] = h, w and int32 [N] = channels (3, or 1 for a gray [h][w] / [h][w][1] image) of a list of uint8
+    images; any other shape is refused."""
     assert len(images) >= 1
     for im in images:
-        assert len(im.shape) == 3 and im.shape[2] == 3 and im.dtype in (torch.uint8, np.uint8), (im.shape, im.dtype)
-    return np.ascontiguousarray([im.shape[:2] for im in images], dtype=np.int32)
+        shp = tuple(im.shape)
+        assert (len(shp) == 2 or (len(shp) == 3 and shp[2] in (1, 3))) and im.dtype in (torch.uint8, np.uint8), \
+            (shp, im.dtype)
+    hw = np.ascontiguousarray([im.shape[:2] for im in images], dtype=np.int32)
+    ch = np.ascontiguousarray([im.shape[2] if len(im.shape) == 3 else 1 for im in images], dtype=np.int32)
+    return hw, ch
+
+
+def is_gray_batch(images) -> bool:
+    """True for a uint8 batch array of gray images, [N][h][w] or [N][h][w][1]."""
+    return len(images.shape) == 3 or (len(images.shape) == 4 and images.shape[3] == 1)
