@@ -69,17 +69,24 @@ MSCNN_API unsigned long long mscnn_kernel_launch_count(void);
 MSCNN_API void mscnn_config_reload(void);
 
 /* ------------------------------------------------------------------------------------
- * Convolution (stride 1) / InnerProduct with fused bias and optional ReLU.
+ * Convolution (stride, dilation, groups) / InnerProduct with fused bias and optional ReLU.
  * Replaces ConvolutionLayer::Forward_gpu (src/caffe/layers/conv_layer.cu:8-23,
  * cudnn_conv_layer.cu:11-46), InnerProductLayer::Forward_gpu (inner_product_layer.cu:10-31)
  * and the in-place ReLULayer::Forward_gpu that follows them (relu_layer.cu:9-26).
  *   x   : planes [N][H][W][C], C % 64 == 0
- *   w   : planes [Cout_pad][KH][KW][C]  (mscnn_pack_conv_weights / mscnn_pack_fc_weights)
+ *   w   : planes [Cout_pad][KH][KW][C / group]  (mscnn_pack_conv_weights / mscnn_pack_fc_weights)
  *   bias: fp32 [Cout_pad]
  *   out : MSCNN_OUT_NHWC_BF16 -> y planes [N][Ho][Wo][Cout_pad] (Cout_pad % 64 == 0)
  *         MSCNN_OUT_NCHW_F32  -> y_f32 [N][Cout][Ho][Wo]
  *         MSCNN_OUT_NHWC_F32  -> y_f32 [N][Ho][Wo][Cout_pad]
- *   Ho = H + 2 pad_h - KH + 1, Wo likewise.  InnerProduct = KH = KW = H = W = 1.
+ *   Ho = (H + 2 pad_h - (dil_h (KH - 1) + 1)) / stride_h + 1, Wo likewise (conv_layer.cpp:8-22); tap (dy, dx) of
+ *   output pixel (ho, wo) reads input pixel (ho stride_h + dy dil_h - pad_h, wo stride_w + dx dil_w - pad_w), zero
+ *   outside the image.  InnerProduct = KH = KW = H = W = 1.
+ *   group = g > 1 (base_conv_layer.cpp:108-120): output channels [k Cout/g, (k+1) Cout/g) see input channels
+ *   [k C/g, (k+1) C/g); C / g and Cout / g must be multiples of 64 and Cout_pad == Cout.  The weight planes are
+ *   mscnn_pack_conv_weights of the Caffe blob [Cout][C/g][KH][KW] with Cin = Cin_pad = C / g.
+ *   Served: strides 1..4, any dilation whose taps fit a tensor map's coordinate range; anything else returns
+ *   MSCNN_ERR_INVALID with a message on stderr.
  */
 typedef struct mscnn_conv_desc {
   const void* x_hi;
@@ -104,6 +111,9 @@ typedef struct mscnn_conv_desc {
    * on the device when the head is launched (the reference learns it on the host, box_output_layer.cpp:201): the
    * launch is sized for the cap N and R is read by the kernel. */
   const int* dyn_n;
+  /* Geometry beyond stride 1 / dilation 1 / group 1.  0 means 1, so a zero-initialised descriptor without these
+   * fields set is the plain convolution. */
+  int stride_h, stride_w, dil_h, dil_w, group;
 } mscnn_conv_desc;
 MSCNN_API int mscnn_conv_forward(const mscnn_conv_desc* d, void* stream);
 /* Host-only: the launch plan mscnn_conv_forward would use for `d` as one line of text (kernel instantiation, pixel box,
@@ -158,12 +168,25 @@ MSCNN_API int mscnn_planes_to_nchw_f32(const void* hi, const void* lo, float* y,
                              int Cpad, void* stream);
 
 /* ------------------------------------------------------------------------------------
- * Pooling, pad 0, ceil-mode output size.  Replaces PoolingLayer::Forward_gpu
+ * Pooling, ceil-mode output size.  Replaces PoolingLayer::Forward_gpu
  * (src/caffe/layers/pooling_layer.cu:158-190; shape pooling_layer.cpp:79-123).
  *   x planes [N][H][W][C] (C % 8 == 0) -> y planes [N][Ho][Wo][C],
- *   Ho = ceil((H - kernel) / stride) + 1.  mode = MSCNN_POOL_MAX | MSCNN_POOL_AVE. */
+ *   mode = MSCNN_POOL_MAX | MSCNN_POOL_AVE (STOCHASTIC is a training mode and is not served).
+ * mscnn_pool_output_size (host-only): Ho = ceil((H + 2 pad - kernel) / stride) + 1, one less when pad > 0 and that
+ *   last window would start in the bottom / right padding (pooling_layer.cpp:90-105); MSCNN_ERR_INVALID unless
+ *   kernel, stride > 0, 0 <= pad < kernel and Ho >= 1.
+ * mscnn_pool_forward: square kernel and stride, pad 0.
+ * mscnn_pool2d_forward_dyn: every PoolingParameter geometry.  Window (ho, wo) starts at (ho stride_h - pad_h,
+ *   wo stride_w - pad_w); MAX ignores padded positions; AVE divides by the window clipped to the padded extent
+ *   (pooling_layer.cpp:196-204), so padded positions count as zeros.  global_pooling is kernel = (H, W), stride 1,
+ *   pad 0: a single window over at least 32 pixels is reduced by a whole CTA per image and 64 channels.
+ *   dyn_n: see below (may be NULL). */
+MSCNN_API int mscnn_pool_output_size(int in, int kernel, int stride, int pad);
 MSCNN_API int mscnn_pool_forward(const void* x_hi, const void* x_lo, void* y_hi, void* y_lo, int N, int H, int W,
                        int C, int kernel, int stride, int mode, void* stream);
+MSCNN_API int mscnn_pool2d_forward_dyn(const void* x_hi, const void* x_lo, void* y_hi, void* y_lo, int N, int H, int W,
+                                       int C, int kernel_h, int kernel_w, int stride_h, int stride_w, int pad_h,
+                                       int pad_w, int mode, const int* dyn_n, void* stream);
 
 /* Data-dependent row counts.  The three per-ROI kernels behind BoxOutput (ROI pooling / ROI align / the pooling
  * that follows ROI align in the cascade nets) and mscnn_conv_desc.dyn_n take an optional DEVICE count: the launch is

@@ -43,6 +43,8 @@ class ConvDesc(C.Structure):
         ("y_hi", c_void_p), ("y_lo", c_void_p), ("y_f32", c_void_p),
         ("pool_hi", c_void_p), ("pool_lo", c_void_p),
         ("dyn_n", c_void_p),
+        # stride / dilation / groups; 0 means 1
+        ("stride_h", c_int), ("stride_w", c_int), ("dil_h", c_int), ("dil_w", c_int), ("group", c_int),
     ]
 
 
@@ -137,6 +139,10 @@ def _declare(L: C.CDLL) -> None:
     L.mscnn_planes_to_nchw_f32.argtypes = [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]
     L.mscnn_pool_forward.restype = c_int
     L.mscnn_pool_forward.argtypes = [c_void_p] * 4 + [c_int] * 7 + [c_void_p]
+    L.mscnn_pool_output_size.restype = c_int
+    L.mscnn_pool_output_size.argtypes = [c_int] * 4
+    L.mscnn_pool2d_forward_dyn.restype = c_int
+    L.mscnn_pool2d_forward_dyn.argtypes = [c_void_p] * 4 + [c_int] * 11 + [c_void_p, c_void_p]
     L.mscnn_deconv2x_forward.restype = c_int
     L.mscnn_deconv2x_forward.argtypes = [c_void_p] * 5 + [c_int] * 5 + [c_void_p]
     L.mscnn_box_output_workspace_bytes.restype = c_int

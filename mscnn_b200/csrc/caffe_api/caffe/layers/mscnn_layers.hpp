@@ -62,8 +62,8 @@ inline bool epilogue_pools(const Blob<Dtype>& conv_top) {
   return conv_top.height() % 2 == 0 && conv_top.width() % 2 == 0;
 }
 
-/// ConvolutionLayer: conv_layer.cpp:8-40 / base_conv_layer.cpp:15-254 (stride 1, group 1, dilation 1:
-/// every Convolution in the shipped deploy nets).  blobs_[0] = [Cout, Cin, kh, kw], blobs_[1] = [Cout].
+/// ConvolutionLayer: conv_layer.cpp:8-40 / base_conv_layer.cpp:15-254, 2-D, with stride, dilation and groups whose
+/// Cin / group and Cout / group are multiples of 64.  blobs_[0] = [Cout, Cin / group, kh, kw], blobs_[1] = [Cout].
 template <typename Dtype>
 class CAFFE_API ConvolutionLayer : public Layer<Dtype> {
  public:
@@ -84,12 +84,18 @@ class CAFFE_API ConvolutionLayer : public Layer<Dtype> {
   bool can_fuse_pool() const { return num_output_ % 64 == 0 && !is_conv1_1(); }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
+  // stride 1, dilation 1, one group: what conv1_1's kernel and the k x 1 head-tap route compute
+  bool plain_geometry() const {
+    return stride_h_ == 1 && stride_w_ == 1 && dilation_h_ == 1 && dilation_w_ == 1 && group_ == 1;
+  }
   bool is_conv1_1() const {
-    return channels_ == 3 && kernel_h_ == 3 && kernel_w_ == 3 && pad_h_ == 1 && pad_w_ == 1 && num_output_ == 64;
+    return channels_ == 3 && kernel_h_ == 3 && kernel_w_ == 3 && pad_h_ == 1 && pad_w_ == 1 && num_output_ == 64 &&
+           plain_geometry();
   }
   Blob<Dtype>* fused_pool_top_ = nullptr;
   bool fused_keep_full_ = true;
   int num_output_, channels_, kernel_h_, kernel_w_, pad_h_, pad_w_;
+  int stride_h_, stride_w_, dilation_h_, dilation_w_, group_;
   bool bias_term_, fuse_relu_;
   PackedParam packed_;
 };
@@ -129,7 +135,7 @@ class CAFFE_API ReLULayer : public Layer<Dtype> {
   bool fused_;
 };
 
-/// PoolingLayer: pooling_layer.cpp:16-220 (MAX / AVE, pad 0, ceil-mode output size).
+/// PoolingLayer: pooling_layer.cpp:16-220 (MAX / AVE; padding, rectangular kernel / stride, global_pooling).
 template <typename Dtype>
 class CAFFE_API PoolingLayer : public Layer<Dtype> {
  public:
@@ -140,14 +146,16 @@ class CAFFE_API PoolingLayer : public Layer<Dtype> {
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int MinTopBlobs() const { return 1; }
   virtual inline int MaxTopBlobs() const { return 1; }
-  int kernel() const { return kernel_; }
-  int stride() const { return stride_; }
-  int mode() const { return mode_; }
+  // the one geometry a convolution's epilogue computes: MAX over 2x2 windows, stride 2, no padding
+  bool is_max_2x2_s2() const {
+    return mode_ == MSCNN_POOL_MAX && !global_pooling_ && kernel_h_ == 2 && kernel_w_ == 2 && stride_h_ == 2 &&
+           stride_w_ == 2 && pad_h_ == 0 && pad_w_ == 0;
+  }
   void set_fused(bool f) { fused_ = f; }   // folded into the producing convolution: see epilogue_pools
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
-  int kernel_, stride_, mode_, pooled_h_, pooled_w_;
-  bool fused_;
+  int kernel_h_, kernel_w_, stride_h_, stride_w_, pad_h_, pad_w_, mode_, pooled_h_, pooled_w_;
+  bool global_pooling_, fused_;
 };
 
 /// SplitLayer: split_layer.cpp:9-31 (forward = share data).

@@ -117,27 +117,40 @@ void ConvolutionLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bottom, con
     pad_h_ = p.pad_size() > 0 ? p.pad(0) : 0;
     pad_w_ = p.pad_size() > 1 ? p.pad(1) : pad_h_;
   }
-  int stride_h = 1, stride_w = 1;
+  stride_h_ = stride_w_ = 1;
   if (p.has_stride_h() || p.has_stride_w()) {
-    stride_h = p.stride_h();
-    stride_w = p.stride_w();
+    stride_h_ = p.stride_h();
+    stride_w_ = p.stride_w();
   } else if (p.stride_size() > 0) {
-    stride_h = p.stride(0);
-    stride_w = p.stride_size() > 1 ? p.stride(1) : stride_h;
+    stride_h_ = p.stride(0);
+    stride_w_ = p.stride_size() > 1 ? p.stride(1) : stride_h_;
   }
-  CHECK(stride_h == 1 && stride_w == 1) << "mscnn_b200 Convolution supports stride 1 only (layer "
-                                        << this->layer_param_.name() << ")";
-  for (int i = 0; i < p.dilation_size(); ++i) CHECK_EQ(p.dilation(i), 1u) << "dilation is not supported";
-  CHECK_EQ(p.group(), 1u) << "mscnn_b200 Convolution supports group 1 only";
+  CHECK_GT(stride_h_, 0) << "Stride dimensions must be nonzero.";
+  CHECK_GT(stride_w_, 0) << "Stride dimensions must be nonzero.";
+  CHECK(stride_h_ <= 4 && stride_w_ <= 4) << "mscnn_b200 Convolution serves strides 1..4 (layer "
+                                          << this->layer_param_.name() << ")";
+  CHECK_LE(p.dilation_size(), 2) << "dilation must be specified once, or once per spatial dimension";
+  dilation_h_ = p.dilation_size() > 0 ? p.dilation(0) : 1;  // base_conv_layer.cpp:95-108
+  dilation_w_ = p.dilation_size() > 1 ? p.dilation(1) : dilation_h_;
+  CHECK_GT(dilation_h_, 0) << "dilation must be nonzero.";
+  CHECK_GT(dilation_w_, 0) << "dilation must be nonzero.";
   channels_ = bottom[0]->channels();
   num_output_ = p.num_output();
   CHECK_GT(num_output_, 0);
+  group_ = p.group();  // base_conv_layer.cpp:121-124
+  CHECK_GT(group_, 0);
+  CHECK_EQ(channels_ % group_, 0);
+  CHECK_EQ(num_output_ % group_, 0) << "Number of output should be multiples of group.";
+  CHECK(group_ == 1 || (channels_ / group_ % 64 == 0 && num_output_ / group_ % 64 == 0))
+      << "mscnn_b200 Convolution serves group > 1 only when the input and output channels of one group are multiples "
+         "of 64 (layer " << this->layer_param_.name() << ": " << channels_ << " -> " << num_output_ << ", group "
+      << group_ << ")";
   bias_term_ = p.bias_term();
   if (this->blobs_.size() > 0) {
     CHECK_EQ((int)this->blobs_.size(), 1 + (bias_term_ ? 1 : 0)) << "Incorrect number of weight blobs.";
   } else {
     this->blobs_.resize(bias_term_ ? 2 : 1);
-    this->blobs_[0].reset(new Blob<Dtype>(num_output_, channels_, kernel_h_, kernel_w_));
+    this->blobs_[0].reset(new Blob<Dtype>(num_output_, channels_ / group_, kernel_h_, kernel_w_));
     FillBlob(p.weight_filler(), this->blobs_[0].get());
     if (bias_term_) {
       this->blobs_[1].reset(new Blob<Dtype>(vector<int>(1, num_output_)));
@@ -149,9 +162,9 @@ void ConvolutionLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bottom, con
 template <typename Dtype>
 void ConvolutionLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   CHECK_EQ(bottom[0]->channels(), channels_) << "Input size incompatible with convolution kernel.";
-  // conv_layer.cpp:8-22 with stride 1, dilation 1
-  const int ho = bottom[0]->height() + 2 * pad_h_ - kernel_h_ + 1;
-  const int wo = bottom[0]->width() + 2 * pad_w_ - kernel_w_ + 1;
+  // conv_layer.cpp:8-22
+  const int ho = (bottom[0]->height() + 2 * pad_h_ - (dilation_h_ * (kernel_h_ - 1) + 1)) / stride_h_ + 1;
+  const int wo = (bottom[0]->width() + 2 * pad_w_ - (dilation_w_ * (kernel_w_ - 1) + 1)) / stride_w_ + 1;
   top[0]->Reshape(bottom[0]->num(), num_output_, ho, wo);
 }
 
@@ -165,7 +178,7 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
   // taps move into the GEMM's N dimension and a 1-D gather sums them (mscnn_head_gather in the C ABI).
   const bool head_path = (num_output_ == 9 || num_output_ == 6) && kernel_h_ == kernel_w_ && kernel_h_ > 1 &&
                          pad_h_ == pad_w_ && 2 * pad_h_ + 1 == kernel_h_ && !fuse_relu_ && channels_ % 64 == 0 &&
-                         !mscnn::config().no_head_taps;
+                         plain_geometry() && !mscnn::config().no_head_taps;
   if (head_path) {
     const int k = kernel_h_;
     const int n_pad = (k * num_output_ + 63) / 64 * 64;
@@ -201,11 +214,13 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
                                        split ? y.lo : nullptr, N, H, W, fuse_relu_ ? 1 : 0, Caffe::stream()));
     return;
   }
-  const int cout_pad = out_pad(num_output_), cin_pad = pad64(channels_);
+  // The blob [Cout][Cin / group][kh][kw] packs to planes [Cout_pad][kh][kw][cin_pad]: with groups, group k's rows are
+  // [k Cout / group, (k + 1) Cout / group) and their channels are the group's own.
+  const int cout_pad = out_pad(num_output_), cin_g = channels_ / group_, cin_pad = pad64(cin_g);
   const size_t bytes = (size_t)cout_pad * kernel_h_ * kernel_w_ * cin_pad * 2;
   packed_.update_weights(wb, {PackedParam::CONV, split, cout_pad, cin_pad, 0, 0, 0}, bytes,
                          [&](const float* w, void* hi, void* lo) {
-    MSCNN_CHECK(mscnn_pack_conv_weights(w, hi, lo, num_output_, channels_, kernel_h_, kernel_w_, cout_pad, cin_pad,
+    MSCNN_CHECK(mscnn_pack_conv_weights(w, hi, lo, num_output_, cin_g, kernel_h_, kernel_w_, cout_pad, cin_pad,
                                         Caffe::stream()));
   });
   packed_.bias.update(bias, num_output_, cout_pad);
@@ -213,6 +228,9 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
   mscnn_conv_desc d = conv_desc(x, packed_, N, H, W, x.cpad, num_output_, kernel_h_, kernel_w_, pad_h_, pad_w_,
                                 this->dyn_rows_device());
   d.relu = fuse_relu_ ? 1 : 0;
+  d.stride_h = stride_h_; d.stride_w = stride_w_;
+  d.dil_h = dilation_h_; d.dil_w = dilation_w_;
+  d.group = group_;
   if (cout_pad % 64 == 0) {
     d.out_mode = MSCNN_OUT_NHWC_BF16;
     const int ho = top[0]->height(), wo = top[0]->width();
@@ -289,26 +307,57 @@ void ReLULayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vec
 template <typename Dtype>
 void PoolingLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   const PoolingParameter& p = this->layer_param_.pooling_param();  // pooling_layer.cpp:16-77
-  CHECK(!p.global_pooling()) << "global pooling is not supported";
-  CHECK(p.has_kernel_size() || (p.has_kernel_h() && p.has_kernel_w())) << "kernel size is required";
-  const int kh = p.has_kernel_size() ? p.kernel_size() : p.kernel_h();
-  const int kw = p.has_kernel_size() ? p.kernel_size() : p.kernel_w();
-  const int sh = p.has_stride_h() ? p.stride_h() : p.stride();
-  const int sw = p.has_stride_w() ? p.stride_w() : p.stride();
-  CHECK(kh == kw && sh == sw) << "square kernel / stride only";
-  CHECK(p.pad() == 0 && p.pad_h() == 0 && p.pad_w() == 0) << "mscnn_b200 Pooling supports pad 0 only";
-  kernel_ = kh;
-  stride_ = sh;
+  global_pooling_ = p.global_pooling();
+  if (global_pooling_) {
+    CHECK(!(p.has_kernel_size() || p.has_kernel_h() || p.has_kernel_w()))
+        << "With Global_pooling: true Filter size cannot specified";
+  } else {
+    CHECK(!p.has_kernel_size() != !(p.has_kernel_h() && p.has_kernel_w()))
+        << "Filter size is kernel_size OR kernel_h and kernel_w; not both";
+    CHECK(p.has_kernel_size() || (p.has_kernel_h() && p.has_kernel_w()))
+        << "For non-square filters both kernel_h and kernel_w are required.";
+  }
+  CHECK((!p.has_pad() && p.has_pad_h() && p.has_pad_w()) || (!p.has_pad_h() && !p.has_pad_w()))
+      << "pad is pad OR pad_h and pad_w are required.";
+  CHECK((!p.has_stride() && p.has_stride_h() && p.has_stride_w()) || (!p.has_stride_h() && !p.has_stride_w()))
+      << "Stride is stride OR stride_h and stride_w are required.";
+  if (global_pooling_) {
+    kernel_h_ = bottom[0]->height();
+    kernel_w_ = bottom[0]->width();
+  } else {
+    kernel_h_ = p.has_kernel_size() ? p.kernel_size() : p.kernel_h();
+    kernel_w_ = p.has_kernel_size() ? p.kernel_size() : p.kernel_w();
+  }
+  CHECK_GT(kernel_h_, 0) << "Filter dimensions cannot be zero.";
+  CHECK_GT(kernel_w_, 0) << "Filter dimensions cannot be zero.";
+  pad_h_ = p.has_pad_h() ? p.pad_h() : p.pad();
+  pad_w_ = p.has_pad_h() ? p.pad_w() : p.pad();
+  stride_h_ = p.has_stride_h() ? p.stride_h() : p.stride();
+  stride_w_ = p.has_stride_h() ? p.stride_w() : p.stride();
+  CHECK_GT(stride_h_, 0) << "Stride cannot be zero.";
+  CHECK_GT(stride_w_, 0) << "Stride cannot be zero.";
+  if (global_pooling_)
+    CHECK(pad_h_ == 0 && pad_w_ == 0 && stride_h_ == 1 && stride_w_ == 1)
+        << "With Global_pooling: true; only pad = 0 and stride = 1";
+  CHECK_LT(pad_h_, kernel_h_);
+  CHECK_LT(pad_w_, kernel_w_);
   CHECK(p.pool() == PoolingParameter_PoolMethod_MAX || p.pool() == PoolingParameter_PoolMethod_AVE)
-      << "MAX and AVE pooling only";
+      << "MAX and AVE pooling only (STOCHASTIC is a training mode)";
   mode_ = p.pool() == PoolingParameter_PoolMethod_MAX ? MSCNN_POOL_MAX : MSCNN_POOL_AVE;
 }
 template <typename Dtype>
 void PoolingLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   CHECK_EQ(4, bottom[0]->num_axes()) << "Input must have 4 axes";
-  // pooling_layer.cpp:90-93 (pad 0)
-  pooled_h_ = (int)std::ceil((float)(bottom[0]->height() - kernel_) / stride_) + 1;
-  pooled_w_ = (int)std::ceil((float)(bottom[0]->width() - kernel_) / stride_) + 1;
+  if (global_pooling_) {  // pooling_layer.cpp:86-89: follows a net that changes its input size
+    kernel_h_ = bottom[0]->height();
+    kernel_w_ = bottom[0]->width();
+  }
+  // pooling_layer.cpp:90-105
+  pooled_h_ = mscnn_pool_output_size(bottom[0]->height(), kernel_h_, stride_h_, pad_h_);
+  pooled_w_ = mscnn_pool_output_size(bottom[0]->width(), kernel_w_, stride_w_, pad_w_);
+  CHECK(pooled_h_ > 0 && pooled_w_ > 0) << "Pooling layer " << this->layer_param_.name() << ": kernel " << kernel_h_
+                                        << "x" << kernel_w_ << " does not fit the " << bottom[0]->height() << "x"
+                                        << bottom[0]->width() << " bottom";
   top[0]->Reshape(bottom[0]->num(), bottom[0]->channels(), pooled_h_, pooled_w_);
 }
 template <typename Dtype>
@@ -317,8 +366,8 @@ void PoolingLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const 
   const bool split = Caffe::split();
   typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
   typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
-  MSCNN_CHECK(mscnn_pool_forward_dyn(x.hi, x.lo, y.hi, y.lo, x.n, x.h, x.w, x.cpad, kernel_, stride_, mode_,
-                                     this->dyn_rows_device(), Caffe::stream()));
+  MSCNN_CHECK(mscnn_pool2d_forward_dyn(x.hi, x.lo, y.hi, y.lo, x.n, x.h, x.w, x.cpad, kernel_h_, kernel_w_, stride_h_,
+                                       stride_w_, pad_h_, pad_w_, mode_, this->dyn_rows_device(), Caffe::stream()));
 }
 
 // ---------------------------------------------------------------------------------- Split

@@ -338,7 +338,7 @@ void Net<Dtype>::FusePooling() {
   const int L = (int)layers_.size();
   for (int i = 0; i < L; ++i) {
     PoolingLayer<Dtype>* pool = dynamic_cast<PoolingLayer<Dtype>*>(layers_[i].get());
-    if (!pool || pool->kernel() != 2 || pool->stride() != 2 || pool->mode() != MSCNN_POOL_MAX) continue;
+    if (!pool || !pool->is_max_2x2_s2()) continue;
     const int blob_id = bottom_id_vecs_[i][0];
     // walk back over the writers of the blob: [conv] or [conv, fused in-place relu]
     int conv_idx = -1;

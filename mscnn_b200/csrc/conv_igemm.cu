@@ -13,6 +13,11 @@
 //     An M tile is a TMA box {64 ch, bw, bh, bn} with bw*bh*bn <= 128 pixels; the tap
 //     (dy,dx) operand is the same box shifted by (dx-pad, dy-pad): TMA zero-fills out-of-
 //     bounds pixels, which *is* the convolution's zero padding.  No im2col buffer exists.
+//   * stride / dilation: the same box traversed with the tensor map's element strides {1, stride_w, stride_h, 1}
+//     (bw x bh pixels land in shared memory, bw stride_w x bh stride_h are spanned in the image), starting at
+//     (w0 stride_w + dx dil_w - pad_w, h0 stride_h + dy dil_h - pad_h).  Nothing else in the kernel knows about them.
+//   * groups: BLOCK_N divides Cout / group, so an n tile lies in one group k = n_base / (Cout / group); its
+//     activation chunks start at channel k Cin / group, its weight rows and output channels are n_base as always.
 //   * warp specialisation: warpgroup 0 = TMA producer (one warp issues, the others idle and hand
 //     their registers to the MMA warpgroups), warpgroups 1 and 2 = wgmma (m64 x BLOCK_N x k16,
 //     bf16 -> fp32) over rows [0, 64) and [64, 128) of the M tile, accumulators in registers, then
@@ -54,7 +59,9 @@ namespace mscnn {
 struct IgemmParams {
   int num_terms;   // 1: bf16; 3: split-bf16 (hi*hi, hi*lo, lo*hi)
   int taps_h, taps_w, pad_h, pad_w;
-  int cin_chunks;  // Cin_pad / 64
+  int stride_h, stride_w, dil_h, dil_w;
+  int cin_chunks;  // channels of one group / 64
+  int cin_g, cout_g;  // input / output channels of one group (the whole padded extents when group == 1)
   int tiles_w, tiles_h, tiles_n, n_tiles;
   int box_w, box_h, box_n;
   int relu;
@@ -186,7 +193,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
       const int n_tile = tile % p.n_tiles;
       int tw, th, tn;
       m_coords(tile / p.n_tiles, tw, th, tn);
-      const int w0 = tw * p.box_w - p.pad_w, h0 = th * p.box_h - p.pad_h, n0 = tn * p.box_n;
+      const int w0 = tw * p.box_w * p.stride_w - p.pad_w, h0 = th * p.box_h * p.stride_h - p.pad_h, n0 = tn * p.box_n;
+      const int c_base = n_tile * BLOCK_N / p.cout_g * p.cin_g;  // first input channel of the tile's group
       for (int term = 0; term < terms; ++term) {
         const CUtensorMap* mapA = (term == 2) ? &tmA_lo : &tmA_hi;
         const CUtensorMap* mapB = (term == 1) ? &tmB_lo : &tmB_hi;
@@ -197,8 +205,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
               if (ptx::elect_one()) {
                 const uint32_t a0 = sA + a_ring.slot * a_stride;
                 ptx::mbar_expect_tx(a_ring.full_bar(), a_tx);
-                ptx::tma_load_4d(a0, mapA, a_ring.full_bar(), cc * kBlockK, w0, h0 + dy, n0);
-                if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, a_ring.full_bar(), cc * kBlockK, w0, h0 + dy, n0);
+                const int c0 = c_base + cc * kBlockK, h = h0 + dy * p.dil_h;
+                ptx::tma_load_4d(a0, mapA, a_ring.full_bar(), c0, w0, h, n0);
+                if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, a_ring.full_bar(), c0, w0, h, n0);
               }
               __syncwarp();
               a_ring.advance();
@@ -212,8 +221,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
                 ptx::tma_load_2d(b0, mapB, ring.full_bar(), kcol, n_tile * BLOCK_N);
                 if (FAT) ptx::tma_load_2d(b0 + kBBytes, &tmB_lo, ring.full_bar(), kcol, n_tile * BLOCK_N);
                 if (!p.rowshare) {
-                  ptx::tma_load_4d(a0, mapA, ring.full_bar(), cc * kBlockK, w0 + dx, h0 + dy, n0);
-                  if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, ring.full_bar(), cc * kBlockK, w0 + dx, h0 + dy, n0);
+                  const int c0 = c_base + cc * kBlockK, w = w0 + dx * p.dil_w, h = h0 + dy * p.dil_h;
+                  ptx::tma_load_4d(a0, mapA, ring.full_bar(), c0, w, h, n0);
+                  if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, ring.full_bar(), c0, w, h, n0);
                 }
               }
               __syncwarp();
@@ -422,12 +432,13 @@ static int pick_block_n(int cout_pad) {
   return 32;
 }
 
-// Choose the pixel box (bw, bh, bn), bw*bh*bn <= 128, that wastes the fewest MMA rows.
-static void pick_box(int N, int Ho, int Wo, bool even, int* bw_o, int* bh_o, int* bn_o) {
+// Choose the pixel box (bw, bh, bn), bw*bh*bn <= 128, that wastes the fewest MMA rows.  The activation box spans
+// bw stride_w x bh stride_h image pixels, and a tensor map's box dimension is at most 256 elements.
+static void pick_box(int N, int Ho, int Wo, bool even, int stride_h, int stride_w, int* bw_o, int* bh_o, int* bn_o) {
   double best = -1.0;
   int b_w = 1, b_h = 1, b_n = 1;
-  for (int bw = 1; bw <= 128 && bw <= Wo; ++bw) {
-    for (int bh = 1; bh * bw <= 128 && bh <= Ho; ++bh) {
+  for (int bw = 1; bw <= 128 && bw <= Wo && bw * stride_w <= 256; ++bw) {
+    for (int bh = 1; bh * bw <= 128 && bh <= Ho && bh * stride_h <= 256; ++bh) {
       if (even && ((bw & 1) || (bh & 1))) continue;  // 2x2 pooling windows must not straddle tiles
       int bn = 128 / (bw * bh);
       if (bn > N) bn = N;
@@ -487,7 +498,7 @@ struct ConvPlan {
 
 struct PlanKey {
   const void* ptr[11];
-  int v[15];
+  int v[20];
   bool operator==(const PlanKey& o) const { return memcmp(this, &o, sizeof(PlanKey)) == 0; }
 };
 struct PlanKeyHash {
@@ -521,8 +532,9 @@ extern "C" int mscnn_conv_forward(const mscnn_conv_desc* d, void* stream_v) {
   memset(&key, 0, sizeof(key));
   const void* ptrs[11] = {d->x_hi, d->x_lo, d->w_hi, d->w_lo, d->bias, d->y_hi, d->y_lo, d->y_f32, d->pool_hi, d->pool_lo, d->dyn_n};
   memcpy(key.ptr, ptrs, sizeof(ptrs));
-  const int vals[15] = {d->N, d->H, d->W, d->C, d->Cout, d->Cout_pad, d->KH, d->KW, d->pad_h, d->pad_w, d->relu,
-                        d->out_mode, device, static_cast<int>(config().epoch), 0};
+  const int vals[20] = {d->N, d->H, d->W, d->C, d->Cout, d->Cout_pad, d->KH, d->KW, d->pad_h, d->pad_w, d->relu,
+                        d->out_mode, device, static_cast<int>(config().epoch), 0,
+                        d->stride_h, d->stride_w, d->dil_h, d->dil_w, d->group};
   memcpy(key.v, vals, sizeof(vals));
   ConvPlan plan;
   bool hit = false;
@@ -582,16 +594,37 @@ static void fit_rings(IgemmParams& p, int block_n) {
   p.stages = deepest_ring(p, block_n);
 }
 
+// A geometry field of mscnn_conv_desc: 0 means 1.
+static inline int or1(int v) { return v == 0 ? 1 : v; }
+
+static int unsupported(const mscnn_conv_desc* d, const char* rule) {
+  fprintf(stderr, "mscnn_conv_forward: stride %dx%d, dilation %dx%d, group %d, C=%d Cout=%d Cout_pad=%d: %s\n",
+          or1(d->stride_h), or1(d->stride_w), or1(d->dil_h), or1(d->dil_w), or1(d->group), d->C, d->Cout, d->Cout_pad,
+          rule);
+  return MSCNN_ERR_INVALID;
+}
+
 static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps) {
   const Config& cfg = config();
   if (!d->x_hi || !d->w_hi || !d->bias) return MSCNN_ERR_INVALID;
   if (d->C % 64 != 0) return MSCNN_ERR_INVALID;
   const bool split = (d->x_lo != nullptr);
   if (split && !d->w_lo) return MSCNN_ERR_INVALID;
-  const int Ho = d->H + 2 * d->pad_h - d->KH + 1;
-  const int Wo = d->W + 2 * d->pad_w - d->KW + 1;
-  if (Ho <= 0 || Wo <= 0 || d->N <= 0) return MSCNN_ERR_INVALID;
-  const int BN = pick_block_n(d->Cout_pad);
+  const int sh = or1(d->stride_h), sw = or1(d->stride_w), dh = or1(d->dil_h), dw = or1(d->dil_w), g = or1(d->group);
+  if (d->KH <= 0 || d->KW <= 0 || d->pad_h < 0 || d->pad_w < 0) return MSCNN_ERR_INVALID;
+  if (sh < 1 || sh > 4 || sw < 1 || sw > 4) return unsupported(d, "strides 1..4 are served");
+  // the furthest tap coordinate, pad + extent + reach, has to stay far inside a tensor map's int32 coordinates
+  if (dh < 1 || dw < 1 || dh > (1 << 20) / d->KH || dw > (1 << 20) / d->KW)
+    return unsupported(d, "the dilated kernel reach must be in 1..2^20");
+  if (g < 1) return unsupported(d, "group must be positive");
+  if (g > 1 && (d->C % g || d->Cout % g || d->C / g % 64 || d->Cout / g % 64 || d->Cout_pad != d->Cout))
+    return unsupported(d, "a grouped convolution needs C / group and Cout / group to be multiples of 64");
+  const int ext_h = dh * (d->KH - 1) + 1, ext_w = dw * (d->KW - 1) + 1;  // conv_layer.cpp:8-22
+  if (d->H + 2 * d->pad_h < ext_h || d->W + 2 * d->pad_w < ext_w || d->N <= 0) return MSCNN_ERR_INVALID;
+  const int Ho = (d->H + 2 * d->pad_h - ext_h) / sh + 1;
+  const int Wo = (d->W + 2 * d->pad_w - ext_w) / sw + 1;
+  const int cin_g = d->C / g, cout_g = d->Cout_pad / g;
+  const int BN = pick_block_n(cout_g);
   if (d->Cout_pad % BN != 0 || d->Cout > d->Cout_pad) return MSCNN_ERR_INVALID;
   const bool pool = (d->out_mode == MSCNN_OUT_NHWC_BF16 && d->pool_hi != nullptr);
   if (d->out_mode == MSCNN_OUT_NHWC_BF16 && (BN < 64 || (!d->y_hi && !pool))) return MSCNN_ERR_INVALID;
@@ -605,8 +638,14 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
   p.taps_w = d->KW;
   p.pad_h = d->pad_h;
   p.pad_w = d->pad_w;
-  p.cin_chunks = d->C / 64;
-  pick_box(d->N, Ho, Wo, pool, &p.box_w, &p.box_h, &p.box_n);
+  p.stride_h = sh;
+  p.stride_w = sw;
+  p.dil_h = dh;
+  p.dil_w = dw;
+  p.cin_g = cin_g;
+  p.cout_g = cout_g;
+  p.cin_chunks = cin_g / 64;
+  pick_box(d->N, Ho, Wo, pool, sh, sw, &p.box_w, &p.box_h, &p.box_n);
   p.tiles_w = (Wo + p.box_w - 1) / p.box_w;
   p.tiles_h = (Ho + p.box_h - 1) / p.box_h;
   p.tiles_n = (d->N + p.box_n - 1) / p.box_n;
@@ -645,9 +684,10 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
   // taps dx of a (term, dy, chunk) are the same activation rows shifted by one pixel: fetch them once with a one-pixel
   // halo per side into an A ring, and deliver only the weight tiles per tap on the B ring.  The MMAs, their order and
   // hence the results are those of the per-tap plan; L2->SM bytes per k-block drop from A + B to A / 3 + B.  The B ring
-  // has to be at least as deep (in taps) as the per-tap ring it replaces, else the per-tap plan stays.
+  // has to be at least as deep (in taps) as the per-tap ring it replaces, else the per-tap plan stays.  The haloed
+  // row serves neighbouring taps only when they are neighbouring columns: stride and dilation 1 in W.
   const bool rs_box = p.box_n == 1 && ((p.box_w == 64 && p.box_h == 2) || (p.box_w == 128 && p.box_h == 1));
-  if (!cfg.no_rowshare && d->KW == 3 && BN <= 128 && rs_box) {
+  if (!cfg.no_rowshare && d->KW == 3 && sw == 1 && dw == 1 && BN <= 128 && rs_box) {
     IgemmParams rs = p;
     rs.rowshare = 1;
     rs.a_stages = 2;
@@ -684,18 +724,20 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
                                {},
                                {(uint64_t)d->Cout_pad, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)d->N},
                                {(uint64_t)d->Cout_pad, (uint64_t)(Wo / 2), (uint64_t)(Ho / 2), (uint64_t)d->N}};
-  const uint32_t boxes[4][4] = {{64u, (uint32_t)(p.box_w + (p.rowshare ? 2 : 0)), (uint32_t)p.box_h, (uint32_t)p.box_n},
+  // the activation box in image pixels: with element strides TMA loads ceil(box / stride) = box_w x box_h of them
+  const uint32_t boxes[4][4] = {{64u, (uint32_t)((p.box_w + (p.rowshare ? 2 : 0)) * sw), (uint32_t)(p.box_h * sh), (uint32_t)p.box_n},
                                 {},
                                 {64u, (uint32_t)p.box_w, (uint32_t)p.box_h, (uint32_t)p.box_n},
                                 {64u, (uint32_t)(p.box_w / 2), (uint32_t)(p.box_h / 2), (uint32_t)p.box_n}};
+  const uint32_t a_strides[4] = {1u, (uint32_t)sw, (uint32_t)sh, 1u};
   for (int i = 0; i < 8; ++i) {
     if (!src[i]) {
       maps[i] = maps[(i & 1) ? i - 1 : 0];
       continue;
     }
     const int rc = (i >> 1) == 1
-                       ? tmap_2d_bf16(&maps[i], src[i], (uint64_t)d->KH * d->KW * d->C, (uint64_t)d->Cout_pad, 64u, (uint32_t)BN)
-                       : tmap_nhwc_bf16(&maps[i], src[i], dims[i >> 1], boxes[i >> 1]);
+                       ? tmap_2d_bf16(&maps[i], src[i], (uint64_t)d->KH * d->KW * cin_g, (uint64_t)d->Cout_pad, 64u, (uint32_t)BN)
+                       : tmap_nhwc_bf16(&maps[i], src[i], dims[i >> 1], boxes[i >> 1], (i >> 1) == 0 ? a_strides : nullptr);
     if (rc) return rc;
   }
 
@@ -717,11 +759,18 @@ extern "C" int mscnn_conv_plan_describe(const mscnn_conv_desc* d, char* buf, int
   const int rc = mscnn::build_plan(d, &plan, false);
   if (rc != MSCNN_OK) return rc;
   const mscnn::IgemmParams& p = plan.p;
-  const int n = snprintf(buf, (size_t)cap,
+  int n = snprintf(buf, (size_t)cap,
                          "kernel=conv_igemm_kernel<%d, %s> box=%dx%dx%d terms=%d fat=%d pool=%d stages=%d epi_bufs=%d "
                          "smem=%zu dyn=%d rowshare=%d a_stages=%d",
                          plan.BN, p.fat ? "true" : "false", p.box_w, p.box_h, p.box_n, p.num_terms, p.fat, p.pool, p.stages, p.epi_bufs,
                          plan.smem, p.dyn_n ? 1 : 0, p.rowshare, p.a_stages);
+  // stride / dilation / groups only where a layer has them: the plain convolution's line stays as it was
+  const int group = d->Cout_pad / p.cout_g;
+  if (n > 0 && n < cap && (p.stride_h != 1 || p.stride_w != 1 || p.dil_h != 1 || p.dil_w != 1 || group != 1)) {
+    const int m = snprintf(buf + n, (size_t)(cap - n), " stride=%dx%d dil=%dx%d group=%d", p.stride_h, p.stride_w,
+                           p.dil_h, p.dil_w, group);
+    n = m > 0 ? n + m : -1;
+  }
   return (n > 0 && n < cap) ? MSCNN_OK : MSCNN_ERR_INVALID;
 }
 

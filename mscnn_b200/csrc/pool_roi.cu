@@ -61,12 +61,16 @@ __device__ __forceinline__ void store8(__nv_bfloat16* hi, __nv_bfloat16* lo, siz
 }
 
 // ------------------------------------------------------------------------------- Pooling
-// PoolingLayer::Forward_cpu (src/caffe/layers/pooling_layer.cpp:128-220) with pad = 0:
-// output size in ceil mode (:90-93), windows clipped to the image, AVE divides by the clipped
-// window size (pad 0 => pool_size = (hend-hstart)*(wend-wstart), :196-203).
+// PoolingLayer::Forward_cpu (src/caffe/layers/pooling_layer.cpp:128-220): windows start at o * stride - pad and are
+// clipped to the image, so MAX never sees a padded position.  AVE divides by the window clipped to the PADDED extent
+// (pool_size is taken with hend = min(hstart + kh, H + pad_h) before hstart / hend are clipped to [0, H], :196-204):
+// padded positions count as zeros in the mean.  With pad 0 that is the clipped window itself.
+struct PoolGeom {
+  int kh, kw, sh, sw, ph, pw;
+};
 __global__ void pool_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl,
                             __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl, int N, int H,
-                            int W, int C, int Ho, int Wo, int k, int s, int mode, const int* __restrict__ dyn_n) {
+                            int W, int C, int Ho, int Wo, PoolGeom q, int mode, const int* __restrict__ dyn_n) {
   const int cg = C / 8;
   if (dyn_n) N = max(0, min(N, *dyn_n));  // data-dependent row count (mscnn_pool_forward_dyn)
   const size_t total = (size_t)N * Ho * Wo * cg;
@@ -77,8 +81,11 @@ __global__ void pool_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfl
     const int ow = r % Wo; r /= Wo;
     const int oh = r % Ho;
     const int n = r / Ho;
-    const int hs = oh * s, ws = ow * s;
-    const int he = min(hs + k, H), we = min(ws + k, W);
+    int hs = oh * q.sh - q.ph, ws = ow * q.sw - q.pw;
+    int he = min(hs + q.kh, H + q.ph), we = min(ws + q.kw, W + q.pw);
+    const float sz = (float)((he - hs) * (we - ws));
+    hs = max(hs, 0); ws = max(ws, 0);
+    he = min(he, H); we = min(we, W);
     Vec8 acc;
 #pragma unroll
     for (int i = 0; i < 8; ++i) acc.v[i] = (mode == MSCNN_POOL_MAX) ? -3.402823466e+38f : 0.f;
@@ -92,12 +99,61 @@ __global__ void pool_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfl
         }
       }
     if (mode == MSCNN_POOL_AVE) {
-      const float sz = (float)((he - hs) * (we - ws));
 #pragma unroll
       for (int i = 0; i < 8; ++i) acc.v[i] = acc.v[i] / sz;
     }
     store8(yh, yl, ((size_t)(n * Ho + oh) * Wo + ow) * C + g * 8, acc);
   }
+}
+
+// Pooling whose one window is the whole image (global_pooling, or any kernel that covers the bottom): pool_kernel
+// would walk a plane per thread.  Here a CTA owns one image and 8 consecutive 8-channel groups (128 contiguous bytes
+// per pixel and plane); its 256 threads are 32 pixel slices x 8 groups, slice s taking pixels s, s + 32, ... with
+// four loads in flight, and slice 0 then folds the 32 partial results in slice order.  MAX is exact in any order.
+// AVE sums hi + lo in fp32 in that fixed order (deterministic), not the reference's row-major one: the two differ by
+// at most (H W - 1) 2^-24 sum|x| / (H W) in the mean, far inside the planes' own 2^-17 relative rounding.
+constexpr int kGlobalSlices = 32, kGlobalGroups = 8;
+__global__ void __launch_bounds__(kGlobalSlices * kGlobalGroups)
+global_pool_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl,
+                   __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl, int N, int HW, int C, int mode,
+                   const int* __restrict__ dyn_n) {
+  __shared__ Vec8 part[kGlobalSlices][kGlobalGroups];
+  const int n = blockIdx.y;
+  if (dyn_n && n >= *dyn_n) return;
+  const int gl = threadIdx.x % kGlobalGroups, slice = threadIdx.x / kGlobalGroups;
+  const int g = blockIdx.x * kGlobalGroups + gl;
+  const bool live = g < C / 8;
+  const bool is_max = mode == MSCNN_POOL_MAX;
+  Vec8 acc;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) acc.v[i] = is_max ? -3.402823466e+38f : 0.f;
+  auto fold = [&](const Vec8& v) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc.v[i] = is_max ? ((v.v[i] > acc.v[i]) ? v.v[i] : acc.v[i]) : acc.v[i] + v.v[i];
+  };
+  if (live) {
+    const size_t base = (size_t)n * HW * C + g * 8;
+    int px = slice;
+    for (; px + 3 * kGlobalSlices < HW; px += 4 * kGlobalSlices) {
+      Vec8 v[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) v[u] = load8(xh, xl, base + (size_t)(px + u * kGlobalSlices) * C);
+#pragma unroll
+      for (int u = 0; u < 4; ++u) fold(v[u]);
+    }
+    for (; px < HW; px += kGlobalSlices) fold(load8(xh, xl, base + (size_t)px * C));
+  }
+  part[slice][gl] = acc;
+  __syncthreads();
+  if (slice != 0 || !live) return;
+  const int used = min(HW, kGlobalSlices);  // slices beyond the pixel count hold the neutral element only
+  for (int sl = 1; sl < used; ++sl) fold(part[sl][gl]);
+  if (!is_max) {
+    const float sz = (float)HW;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc.v[i] = acc.v[i] / sz;
+  }
+  store8(yh, yl, (size_t)n * C + g * 8, acc);
 }
 
 // --------------------------------------------------------------------------- ROIPooling
@@ -405,21 +461,44 @@ static int grid_for(size_t total, int threads) {
 
 using namespace mscnn;
 
-extern "C" int mscnn_pool_forward_dyn(const void* x_hi, const void* x_lo, void* y_hi, void* y_lo, int N, int H,
-                                      int W, int C, int kernel, int stride, int mode, const int* dyn_n, void* stream) {
-  if (!x_hi || !y_hi || N <= 0 || H <= 0 || W <= 0 || C % 8 || kernel <= 0 || stride <= 0)
-    return MSCNN_ERR_INVALID;
+extern "C" int mscnn_pool_output_size(int in, int kernel, int stride, int pad) {
+  if (in <= 0 || kernel <= 0 || stride <= 0 || pad < 0 || pad >= kernel) return MSCNN_ERR_INVALID;
+  int out = (in + 2 * pad - kernel + stride - 1) / stride + 1;
+  if (pad > 0 && (out - 1) * stride >= in + pad) --out;  // the last window must start in the image or the left padding
+  return out >= 1 ? out : MSCNN_ERR_INVALID;
+}
+
+extern "C" int mscnn_pool2d_forward_dyn(const void* x_hi, const void* x_lo, void* y_hi, void* y_lo, int N, int H,
+                                        int W, int C, int kernel_h, int kernel_w, int stride_h, int stride_w,
+                                        int pad_h, int pad_w, int mode, const int* dyn_n, void* stream) {
+  if (!x_hi || !y_hi || N <= 0 || C <= 0 || C % 8) return MSCNN_ERR_INVALID;
   if ((x_lo == nullptr) != (y_lo == nullptr)) return MSCNN_ERR_INVALID;
   if (mode != MSCNN_POOL_MAX && mode != MSCNN_POOL_AVE) return MSCNN_ERR_INVALID;
-  // pooling_layer.cpp:90-93 with pad 0
-  const int Ho = (H - kernel + stride - 1) / stride + 1;
-  const int Wo = (W - kernel + stride - 1) / stride + 1;
-  const size_t total = (size_t)N * Ho * Wo * (C / 8);
+  const int Ho = mscnn_pool_output_size(H, kernel_h, stride_h, pad_h);
+  const int Wo = mscnn_pool_output_size(W, kernel_w, stride_w, pad_w);
+  if (Ho <= 0 || Wo <= 0) return MSCNN_ERR_INVALID;
+  const __nv_bfloat16 *xh = (const __nv_bfloat16*)x_hi, *xl = (const __nv_bfloat16*)x_lo;
+  __nv_bfloat16 *yh = (__nv_bfloat16*)y_hi, *yl = (__nv_bfloat16*)y_lo;
   mscnn::note_launch();
-  pool_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
-      (const __nv_bfloat16*)x_hi, (const __nv_bfloat16*)x_lo, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, N,
-      H, W, C, Ho, Wo, kernel, stride, mode, dyn_n);
+  // one unpadded window over a whole image of at least a pixel per slice: the CTA-wide reduction
+  if (Ho == 1 && Wo == 1 && pad_h == 0 && pad_w == 0 && (long long)H * W >= kGlobalSlices && N <= 65535 &&
+      (long long)H * W <= 2147483647ll) {
+    const dim3 grid((C / 8 + kGlobalGroups - 1) / kGlobalGroups, N);
+    global_pool_kernel<<<grid, kGlobalSlices * kGlobalGroups, 0, (cudaStream_t)stream>>>(xh, xl, yh, yl, N, H * W, C,
+                                                                                         mode, dyn_n);
+    return launch_check("global_pool");
+  }
+  const size_t total = (size_t)N * Ho * Wo * (C / 8);
+  const PoolGeom q = {kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w};
+  pool_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(xh, xl, yh, yl, N, H, W, C, Ho, Wo, q, mode,
+                                                                     dyn_n);
   return launch_check("pool");
+}
+
+extern "C" int mscnn_pool_forward_dyn(const void* x_hi, const void* x_lo, void* y_hi, void* y_lo, int N, int H,
+                                      int W, int C, int kernel, int stride, int mode, const int* dyn_n, void* stream) {
+  return mscnn_pool2d_forward_dyn(x_hi, x_lo, y_hi, y_lo, N, H, W, C, kernel, kernel, stride, stride, 0, 0, mode,
+                                  dyn_n, stream);
 }
 
 extern "C" int mscnn_pool_forward(const void* x_hi, const void* x_lo, void* y_hi, void* y_lo, int N, int H,

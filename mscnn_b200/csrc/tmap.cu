@@ -28,23 +28,24 @@ static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
 }
 
 int tmap_nhwc_bf16(CUtensorMap* out, const void* base, const uint64_t dims[4],
-                   const uint32_t box[4]) {
+                   const uint32_t box[4], const uint32_t elem_strides[4]) {
   auto enc = get_encode();
   if (!enc) return MSCNN_ERR_CUDA;
   cuuint64_t gdim[4] = {dims[0], dims[1], dims[2], dims[3]};
   cuuint64_t gstride[3] = {dims[0] * 2, dims[0] * dims[1] * 2, dims[0] * dims[1] * dims[2] * 2};
   cuuint32_t b[4] = {box[0], box[1], box[2], box[3]};
   cuuint32_t estr[4] = {1, 1, 1, 1};
+  for (int i = 0; elem_strides && i < 4; ++i) estr[i] = elem_strides[i];
   CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), gdim, gstride,
                    b, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     fprintf(stderr,
             "mscnn: cuTensorMapEncodeTiled(4d) failed rc=%d dims={%llu,%llu,%llu,%llu} "
-            "box={%u,%u,%u,%u} base=%p\n",
+            "box={%u,%u,%u,%u} strides={%u,%u,%u,%u} base=%p\n",
             (int)r, (unsigned long long)dims[0], (unsigned long long)dims[1],
             (unsigned long long)dims[2], (unsigned long long)dims[3], box[0], box[1], box[2],
-            box[3], base);
+            box[3], estr[0], estr[1], estr[2], estr[3], base);
     return MSCNN_ERR_CUDA;
   }
   return MSCNN_OK;

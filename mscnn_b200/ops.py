@@ -75,7 +75,8 @@ def planes_to_nchw(p: Planes) -> torch.Tensor:
 
 def pack_conv_weights(w: torch.Tensor, b: torch.Tensor | None, split: bool,
                       cout_pad: int | None = None, cin_pad: int | None = None) -> PackedWeights:
-    """w: [Cout][Cin][KH][KW] fp32 (Caffe blob 0), b: [Cout] fp32 (blob 1) or None."""
+    """w: [Cout][Cin][KH][KW] fp32 (Caffe blob 0; [Cout][Cin / group][KH][KW] of a grouped layer packs the same way),
+    b: [Cout] fp32 (blob 1) or None."""
     assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and w.dim() == 4
     cout, cin, kh, kw = w.shape
     cout_pad = cout_pad or (pad64(cout) if cout > 32 else 32)
@@ -109,20 +110,25 @@ def pack_fc_weights(w: torch.Tensor, b: torch.Tensor | None, split: bool, c: int
     return PackedWeights(hi, lo, bias, nout, 1, 1)
 
 
+def _pair(v) -> tuple[int, int]:
+    return (int(v), int(v)) if isinstance(v, int) else (int(v[0]), int(v[1]))
+
+
 def conv_forward(x: Planes, w: PackedWeights, pad, relu: bool, out_f32: bool = False,
                  out_split: bool | None = None, pool: str | None = None, dyn: torch.Tensor | None = None,
-                 out_mode: int | None = None, out=None):
-    """Convolution (stride 1) + bias (+ReLU).  Returns Planes, or an NCHW fp32 tensor when
+                 out_mode: int | None = None, out=None, stride=1, dilation=1, group: int = 1):
+    """Convolution + bias (+ReLU).  Returns Planes, or an NCHW fp32 tensor when
     ``out_f32``.  An InnerProduct is the KH=KW=H=W=1 case.
 
-    pad: an int, or (pad_h, pad_w).  out_mode = capi.OUT_NHWC_F32 returns pixel-major fp32 rows
+    pad, stride, dilation: an int, or (h, w).  group > 1: ``w`` packed from the blob [Cout][Cin / group][KH][KW].  out_mode = capi.OUT_NHWC_F32 returns pixel-major fp32 rows
     [N][Ho][Wo][Cout_pad] (the head-tap partial sums).  dyn: a device int32 tensor of one element, the
     number of images / rows to compute (rows at or above it are left as they were).  out: a tensor or
     Planes of the returned kind to write into instead of a new one."""
     n, h, wd, c = x.hi.shape
-    assert w.hi.shape[3] == c, (w.hi.shape, x.hi.shape)
-    pad_h, pad_w = (pad, pad) if isinstance(pad, int) else pad
-    ho, wo = h + 2 * pad_h - w.kh + 1, wd + 2 * pad_w - w.kw + 1
+    assert w.hi.shape[3] * group == c, (w.hi.shape, x.hi.shape, group)
+    (pad_h, pad_w), (s_h, s_w), (d_h, d_w) = _pair(pad), _pair(stride), _pair(dilation)
+    ho = (h + 2 * pad_h - (d_h * (w.kh - 1) + 1)) // s_h + 1
+    wo = (wd + 2 * pad_w - (d_w * (w.kw - 1) + 1)) // s_w + 1
     cout_pad = w.hi.shape[0]
     if out_mode is None:
         out_mode = capi.OUT_NCHW_F32 if out_f32 else capi.OUT_NHWC_BF16
@@ -132,6 +138,7 @@ def conv_forward(x: Planes, w: PackedWeights, pad, relu: bool, out_f32: bool = F
     d.w_hi, d.w_lo, d.bias = capi.ptr(w.hi), capi.ptr(w.lo), capi.ptr(w.bias)
     d.Cout, d.Cout_pad, d.KH, d.KW, d.pad_h, d.pad_w = w.cout, cout_pad, w.kh, w.kw, pad_h, pad_w
     d.relu = int(relu)
+    d.stride_h, d.stride_w, d.dil_h, d.dil_w, d.group = s_h, s_w, d_h, d_w, group
     if dyn is not None:
         assert dyn.is_cuda and dyn.dtype == torch.int32 and dyn.numel() == 1
         d.dyn_n = capi.ptr(dyn)
@@ -167,11 +174,16 @@ def conv_forward(x: Planes, w: PackedWeights, pad, relu: bool, out_f32: bool = F
     return out
 
 
-def pool_forward(x: Planes, kernel: int, stride: int, mode: int = capi.POOL_MAX, dyn: torch.Tensor | None = None,
-                 out: Planes | None = None) -> Planes:
-    """dyn: a device int32 tensor of one element, the number of images to pool (mscnn_pool_forward_dyn);
+def pool_forward(x: Planes, kernel, stride, mode: int = capi.POOL_MAX, dyn: torch.Tensor | None = None,
+                 out: Planes | None = None, pad=0) -> Planes:
+    """kernel, stride, pad: an int, or (h, w); kernel = None pools each whole image (global_pooling).
+    dyn: a device int32 tensor of one element, the number of images to pool (mscnn_pool_forward_dyn);
     out: planes to write into instead of new ones."""
     n, h, w, c = x.hi.shape
+    if kernel is None:
+        kernel = (h, w)
+    if not (isinstance(kernel, int) and isinstance(stride, int) and pad == 0):
+        return _pool2d_forward(x, _pair(kernel), _pair(stride), _pair(pad), mode, dyn, out)
     ho = -(-(h - kernel) // stride) + 1
     wo = -(-(w - kernel) // stride) + 1
     if out is None:
@@ -185,6 +197,24 @@ def pool_forward(x: Planes, kernel: int, stride: int, mode: int = capi.POOL_MAX,
     else:
         assert dyn.is_cuda and dyn.dtype == torch.int32 and dyn.numel() == 1
         capi.check(capi.lib().mscnn_pool_forward_dyn(*args, capi.ptr(dyn), _stream()), "pool_forward_dyn")
+    return out
+
+
+def _pool2d_forward(x: Planes, kernel, stride, pad, mode, dyn, out) -> Planes:
+    n, h, w, c = x.hi.shape
+    ho = capi.lib().mscnn_pool_output_size(h, kernel[0], stride[0], pad[0])
+    wo = capi.lib().mscnn_pool_output_size(w, kernel[1], stride[1], pad[1])
+    if ho <= 0 or wo <= 0:
+        raise capi.MscnnError(f"pooling kernel {kernel} stride {stride} pad {pad} does not fit a {h}x{w} map")
+    if out is None:
+        y_hi = torch.empty((n, ho, wo, c), dtype=torch.bfloat16, device=x.hi.device)
+        out = Planes(y_hi, torch.empty_like(y_hi) if x.lo is not None else None, x.channels)
+    assert out.shape == (n, ho, wo, c)
+    if dyn is not None:
+        assert dyn.is_cuda and dyn.dtype == torch.int32 and dyn.numel() == 1
+    capi.check(capi.lib().mscnn_pool2d_forward_dyn(capi.ptr(x.hi), capi.ptr(x.lo), capi.ptr(out.hi), capi.ptr(out.lo),
+                                                   n, h, w, c, *kernel, *stride, *pad, mode, capi.ptr(dyn), _stream()),
+               "pool2d_forward_dyn")
     return out
 
 
