@@ -134,6 +134,39 @@ MSCNN_API int mscnn_pack_conv_weights(const float* w_f32, void* w_hi, void* w_lo
 MSCNN_API int mscnn_pack_fc_weights(const float* w_f32, void* w_hi, void* w_lo, int Nout, int C, int H, int W,
                           int Nout_pad, int Cpad, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Deconvolution (transposed convolution) with any kernel, stride, pad, dilation and group whose channels are 64-aligned,
+ * with fused bias and optional ReLU.  Replaces DeconvolutionLayer::Forward_gpu (src/caffe/layers/deconv_layer.cu,
+ * deconv_layer.cpp:25-40: col2im of w^T x, then the bias) for every layer but the depthwise ones
+ * (mscnn_deconv_depthwise_forward).
+ *   The descriptor is the convolution's: KH, KW, pad_*, stride_*, dil_*, group are the Deconvolution's parameters,
+ *   N, H, W, C the input planes [N][H][W][C] (C % 64 == 0), w_* the planes of mscnn_pack_deconv_weights, bias fp32
+ *   [Cout_pad], y planes [N][Ho][Wo][Cout_pad] (Cout_pad % 64 == 0, out_mode MSCNN_OUT_NHWC_BF16), with
+ *   Ho = stride_h (H - 1) + dil_h (KH - 1) + 1 - 2 pad_h, Wo likewise (deconv_layer.cpp:8-22):
+ *     y[n][i stride_h - pad_h + ky dil_h][j stride_w - pad_w + kx dil_w][co] += x[n][i][j][ci] w[ci][co][ky][kx].
+ *   The output is computed by phase (ho mod stride_h, wo mod stride_w): each phase is a stride-1 convolution with its
+ *   own sub-kernel, signed pad and extent, one conv_igemm_kernel launch writing that phase's pixels; a phase no tap
+ *   reaches holds the bias (plus ReLU).  The sums run in the convolution kernel's K order, not col2im's.
+ *   group = g > 1: C / g and Cout / g must be multiples of 64 and Cout_pad == Cout.
+ *   Served: strides 1..8, pad >= 0, dilation >= 1, pad and dilated kernel reach up to 2^20, a positive output extent;
+ *   pool_*, y_f32 and dyn_n unused (NULL).  Anything else returns MSCNN_ERR_INVALID with a message on stderr and
+ *   writes nothing. */
+MSCNN_API int mscnn_deconv_forward(const mscnn_conv_desc* d, void* stream);
+/* Host-only: one line per output phase, in (r_h, r_w) row-major order,
+ *   "phase=<r_h>x<r_w> taps=<m_h>x<m_w> dil=<d_h>x<d_w> pad=<P_h>x<P_w> out=<Q_h>x<Q_w> plan=<plan>\n"
+ * with the sub-convolution's taps, dilation, signed pad and extent, and as <plan> the mscnn_conv_plan_describe text of
+ * its launch, "bias_fill" where no tap reaches the phase or "none" where it has no output pixel.  No CUDA call. */
+MSCNN_API int mscnn_deconv_plan_describe(const mscnn_conv_desc* d, char* buf, int cap);
+/* Weight packing for mscnn_deconv_forward: the Caffe blob [Cin][Cout / group][KH][KW] (deconv blob layout,
+ * base_conv_layer.cpp:135-142 with the channel axes reversed) -> every phase's sub-kernel, phases (r_h, r_w) in row-major
+ * order, each [Cout_pad][m_h][m_w][cin_g] (mscnn_pack_conv_weights' layout; cin_g = Cin / group padded to 64), taps
+ * reversed.  mscnn_deconv_packed_elems (host-only): elements of one plane (w_hi or w_lo), -1 for a geometry not served. */
+MSCNN_API long long mscnn_deconv_packed_elems(int Cin, int Cout, int group, int KH, int KW, int stride_h, int stride_w,
+                                              int pad_h, int pad_w, int dil_h, int dil_w, int Cout_pad);
+MSCNN_API int mscnn_pack_deconv_weights(const float* w_f32, void* w_hi, void* w_lo, int Cin, int Cout, int group,
+                                        int KH, int KW, int stride_h, int stride_w, int pad_h, int pad_w, int dil_h,
+                                        int dil_w, int Cout_pad, void* stream);
+
 /* conv1_1 as one tensor-core kernel (mscnn_b200/csrc/conv_c3_tc.cu): 3 -> 64 channels, 3x3, pad 1, straight
  * from the fp32 NCHW input blob to NHWC bf16 planes [N][H][W][64] (+ReLU).  Same reference call sites as
  * mscnn_conv_forward (conv_layer.cpp:25-40, relu_layer.cpp:9-19).  The horizontal taps are overlapping views
@@ -211,10 +244,18 @@ MSCNN_API int mscnn_relu_planes(void* hi, void* lo, size_t count, void* stream);
 MSCNN_API int mscnn_relu_f32(float* x, size_t count, void* stream);
 MSCNN_API int mscnn_concat_planes(const void* x, void* y, size_t pixels, int C, int Ctot, int offset, void* stream);
 
-/* Depthwise transposed convolution, kernel 4 / stride 2 / pad 1 / group == channels / no bias:
- * the "conv4_3_2x" layer of the -2x nets.  Replaces DeconvolutionLayer::Forward_gpu
- * (src/caffe/layers/deconv_layer.cu) for that shape.  w: fp32 [Creal][1][4][4] (layer blob 0).
- *   x planes [N][H][W][C] -> y planes [N][2H][2W][C]. */
+/* Depthwise transposed convolution (group == channels == num_output): DeconvolutionLayer::Forward_gpu
+ * (src/caffe/layers/deconv_layer.cu) for those layers, any kernel, stride 1..8, pad >= 0 and dilation >= 1 per axis.
+ *   w: fp32 [Creal][1][KH][KW] (layer blob 0), bias: fp32 [Creal] (blob 1) or NULL.
+ *   x planes [N][H][W][C] -> y planes [N][Ho][Wo][C], Ho = stride_h (H - 1) + dil_h (KH - 1) + 1 - 2 pad_h, Wo likewise;
+ *   channels from Creal up to C are zero.  Each output sums its taps in col2im's increasing (ky, kx) order
+ *   (util/im2col.cpp:col2im_cpu), then adds the bias.
+ * mscnn_deconv2x_forward: kernel 4 / stride 2 / pad 1 / no bias, the "conv4_3_2x" layer of the -2x nets
+ *   (y planes [N][2H][2W][C]). */
+MSCNN_API int mscnn_deconv_depthwise_forward(const void* x_hi, const void* x_lo, const float* w, const float* bias,
+                                             void* y_hi, void* y_lo, int N, int H, int W, int C, int Creal, int KH,
+                                             int KW, int stride_h, int stride_w, int pad_h, int pad_w, int dil_h,
+                                             int dil_w, void* stream);
 MSCNN_API int mscnn_deconv2x_forward(const void* x_hi, const void* x_lo, const float* w, void* y_hi, void* y_lo,
                            int N, int H, int W, int C, int Creal, void* stream);
 

@@ -145,6 +145,16 @@ def _declare(L: C.CDLL) -> None:
     L.mscnn_pool2d_forward_dyn.argtypes = [c_void_p] * 4 + [c_int] * 11 + [c_void_p, c_void_p]
     L.mscnn_deconv2x_forward.restype = c_int
     L.mscnn_deconv2x_forward.argtypes = [c_void_p] * 5 + [c_int] * 5 + [c_void_p]
+    L.mscnn_deconv_depthwise_forward.restype = c_int
+    L.mscnn_deconv_depthwise_forward.argtypes = [c_void_p] * 6 + [c_int] * 13 + [c_void_p]
+    L.mscnn_deconv_forward.restype = c_int
+    L.mscnn_deconv_forward.argtypes = [C.POINTER(ConvDesc), c_void_p]
+    L.mscnn_deconv_plan_describe.restype = c_int
+    L.mscnn_deconv_plan_describe.argtypes = [C.POINTER(ConvDesc), C.c_char_p, c_int]
+    L.mscnn_deconv_packed_elems.restype = C.c_longlong
+    L.mscnn_deconv_packed_elems.argtypes = [c_int] * 12
+    L.mscnn_pack_deconv_weights.restype = c_int
+    L.mscnn_pack_deconv_weights.argtypes = [c_void_p, c_void_p, c_void_p] + [c_int] * 12 + [c_void_p]
     L.mscnn_box_output_workspace_bytes.restype = c_int
     L.mscnn_box_output_workspace_bytes.argtypes = [C.POINTER(BoxOutputCfg), c_int, C.POINTER(C.c_size_t)]
     L.mscnn_box_output_forward.restype = c_int

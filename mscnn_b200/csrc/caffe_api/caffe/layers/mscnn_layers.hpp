@@ -29,7 +29,7 @@ struct PackedBias {
   void update(Blob<float>* b, int n, int n_pad);  // b[0:n], then zeros up to n_pad (b == NULL: all zeros)
 };
 struct PackedParam {
-  enum Route { CONV, HEAD, CONV1_1, FC };
+  enum Route { CONV, HEAD, CONV1_1, FC, DECONV };
   // what `w` holds: the route that packed it, its padding and (fc) the bottom's C, H, W
   struct Layout { int route, split, out_pad, in_pad, c, h, w; };
   PlaneStore w;  // bf16 hi (+ lo when layout.split)
@@ -100,8 +100,10 @@ class CAFFE_API ConvolutionLayer : public Layer<Dtype> {
   PackedParam packed_;
 };
 
-/// DeconvolutionLayer: deconv_layer.cpp:8-40, restricted to the depthwise 4/2/1 bilinear-upsampling
-/// shape of the "-2x" nets.
+/// DeconvolutionLayer: deconv_layer.cpp:8-40 / base_conv_layer.cpp:15-254, 2-D, with stride, pad, dilation, groups and
+/// bias.  blobs_[0] = [Cin, Cout / group, kh, kw], blobs_[1] = [Cout].  Depthwise layers (group == Cin == Cout) run
+/// mscnn_deconv_depthwise_forward on the blob as it is; the others mscnn_deconv_forward on weights packed by phase,
+/// which needs Cin / group and Cout / group to be multiples of 64 when group > 1.
 template <typename Dtype>
 class CAFFE_API DeconvolutionLayer : public Layer<Dtype> {
  public:
@@ -113,7 +115,11 @@ class CAFFE_API DeconvolutionLayer : public Layer<Dtype> {
   virtual inline int ExactNumTopBlobs() const { return 1; }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
-  int channels_;
+  bool depthwise() const { return group_ == channels_ && num_output_ == channels_; }
+  int num_output_, channels_, kernel_h_, kernel_w_, pad_h_, pad_w_;
+  int stride_h_, stride_w_, dilation_h_, dilation_w_, group_;
+  bool bias_term_;
+  PackedParam packed_;
 };
 
 /// ReLULayer: relu_layer.cpp:9-19 (negative_slope 0), in place.

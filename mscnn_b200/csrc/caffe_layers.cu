@@ -6,6 +6,7 @@
 
 #include "caffe/layers/mscnn_layers.hpp"
 #include "config.h"
+#include "deconv_phase.h"
 
 namespace caffe {
 
@@ -93,47 +94,55 @@ void InputLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vec
   }
 }
 
+// Kernel, pad, stride and dilation of a 2-D ConvolutionParameter (base_conv_layer.cpp:27-108), shared by Convolution
+// and Deconvolution.
+static void ParseConvGeometry(const ConvolutionParameter& p, int* kh, int* kw, int* ph, int* pw, int* sh, int* sw,
+                              int* dh, int* dw) {
+  if (p.has_kernel_h() || p.has_kernel_w()) {
+    CHECK_EQ(0, p.kernel_size_size()) << "Either kernel_size or kernel_h/w should be specified; not both.";
+    *kh = p.kernel_h();
+    *kw = p.kernel_w();
+  } else {
+    CHECK(p.kernel_size_size() == 1 || p.kernel_size_size() == 2) << "kernel_size must be specified once or twice";
+    *kh = p.kernel_size(0);
+    *kw = p.kernel_size(p.kernel_size_size() == 1 ? 0 : 1);
+  }
+  CHECK_GT(*kh, 0) << "Filter dimensions must be nonzero.";
+  CHECK_GT(*kw, 0) << "Filter dimensions must be nonzero.";
+  if (p.has_pad_h() || p.has_pad_w()) {
+    *ph = p.pad_h();
+    *pw = p.pad_w();
+  } else {
+    *ph = p.pad_size() > 0 ? p.pad(0) : 0;
+    *pw = p.pad_size() > 1 ? p.pad(1) : *ph;
+  }
+  *sh = 1;
+  *sw = 1;
+  if (p.has_stride_h() || p.has_stride_w()) {
+    *sh = p.stride_h();
+    *sw = p.stride_w();
+  } else if (p.stride_size() > 0) {
+    *sh = p.stride(0);
+    *sw = p.stride_size() > 1 ? p.stride(1) : *sh;
+  }
+  CHECK_GT(*sh, 0) << "Stride dimensions must be nonzero.";
+  CHECK_GT(*sw, 0) << "Stride dimensions must be nonzero.";
+  CHECK_LE(p.dilation_size(), 2) << "dilation must be specified once, or once per spatial dimension";
+  *dh = p.dilation_size() > 0 ? p.dilation(0) : 1;  // base_conv_layer.cpp:95-108
+  *dw = p.dilation_size() > 1 ? p.dilation(1) : *dh;
+  CHECK_GT(*dh, 0) << "dilation must be nonzero.";
+  CHECK_GT(*dw, 0) << "dilation must be nonzero.";
+}
+
 // ---------------------------------------------------------------------------- Convolution
 template <typename Dtype>
 void ConvolutionLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   // base_conv_layer.cpp:15-180, 2-D case
   const ConvolutionParameter& p = this->layer_param_.convolution_param();
   CHECK_EQ(bottom[0]->num_axes(), 4) << "mscnn_b200 Convolution takes 4-D bottoms";
-  if (p.has_kernel_h() || p.has_kernel_w()) {
-    CHECK_EQ(0, p.kernel_size_size()) << "Either kernel_size or kernel_h/w should be specified; not both.";
-    kernel_h_ = p.kernel_h();
-    kernel_w_ = p.kernel_w();
-  } else {
-    CHECK(p.kernel_size_size() == 1 || p.kernel_size_size() == 2) << "kernel_size must be specified once or twice";
-    kernel_h_ = p.kernel_size(0);
-    kernel_w_ = p.kernel_size(p.kernel_size_size() == 1 ? 0 : 1);
-  }
-  CHECK_GT(kernel_h_, 0) << "Filter dimensions must be nonzero.";
-  CHECK_GT(kernel_w_, 0) << "Filter dimensions must be nonzero.";
-  if (p.has_pad_h() || p.has_pad_w()) {
-    pad_h_ = p.pad_h();
-    pad_w_ = p.pad_w();
-  } else {
-    pad_h_ = p.pad_size() > 0 ? p.pad(0) : 0;
-    pad_w_ = p.pad_size() > 1 ? p.pad(1) : pad_h_;
-  }
-  stride_h_ = stride_w_ = 1;
-  if (p.has_stride_h() || p.has_stride_w()) {
-    stride_h_ = p.stride_h();
-    stride_w_ = p.stride_w();
-  } else if (p.stride_size() > 0) {
-    stride_h_ = p.stride(0);
-    stride_w_ = p.stride_size() > 1 ? p.stride(1) : stride_h_;
-  }
-  CHECK_GT(stride_h_, 0) << "Stride dimensions must be nonzero.";
-  CHECK_GT(stride_w_, 0) << "Stride dimensions must be nonzero.";
+  ParseConvGeometry(p, &kernel_h_, &kernel_w_, &pad_h_, &pad_w_, &stride_h_, &stride_w_, &dilation_h_, &dilation_w_);
   CHECK(stride_h_ <= 4 && stride_w_ <= 4) << "mscnn_b200 Convolution serves strides 1..4 (layer "
                                           << this->layer_param_.name() << ")";
-  CHECK_LE(p.dilation_size(), 2) << "dilation must be specified once, or once per spatial dimension";
-  dilation_h_ = p.dilation_size() > 0 ? p.dilation(0) : 1;  // base_conv_layer.cpp:95-108
-  dilation_w_ = p.dilation_size() > 1 ? p.dilation(1) : dilation_h_;
-  CHECK_GT(dilation_h_, 0) << "dilation must be nonzero.";
-  CHECK_GT(dilation_w_, 0) << "dilation must be nonzero.";
   channels_ = bottom[0]->channels();
   num_output_ = p.num_output();
   CHECK_GT(num_output_, 0);
@@ -256,33 +265,92 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
 // -------------------------------------------------------------------------- Deconvolution
 template <typename Dtype>
 void DeconvolutionLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
+  // base_conv_layer.cpp:15-180, 2-D case, with the channel axes reversed (deconv_layer.hpp: reverse_dimensions)
   const ConvolutionParameter& p = this->layer_param_.convolution_param();
+  const std::string& name = this->layer_param_.name();
+  CHECK_EQ(bottom[0]->num_axes(), 4) << "mscnn_b200 Deconvolution takes 4-D bottoms";
+  ParseConvGeometry(p, &kernel_h_, &kernel_w_, &pad_h_, &pad_w_, &stride_h_, &stride_w_, &dilation_h_, &dilation_w_);
   channels_ = bottom[0]->channels();
-  const int k = p.kernel_size_size() ? (int)p.kernel_size(0) : (int)p.kernel_h();
-  const int s = p.stride_size() ? (int)p.stride(0) : (p.has_stride_h() ? (int)p.stride_h() : 1);
-  const int pd = p.pad_size() ? (int)p.pad(0) : (int)p.pad_h();
-  CHECK(k == 4 && s == 2 && pd == 1 && (int)p.group() == channels_ && (int)p.num_output() == channels_ &&
-        !p.bias_term())
-      << "mscnn_b200 Deconvolution supports the depthwise kernel 4 / stride 2 / pad 1 / no-bias shape of the "
-         "MS-CNN -2x nets only (layer " << this->layer_param_.name() << ")";
-  if (this->blobs_.empty()) {
-    this->blobs_.resize(1);
-    this->blobs_[0].reset(new Blob<Dtype>(channels_, 1, 4, 4));  // deconv: [Cin, Cout/group, kh, kw]
+  num_output_ = p.num_output();
+  CHECK_GT(num_output_, 0);
+  group_ = p.group();  // base_conv_layer.cpp:121-124
+  CHECK_GT(group_, 0);
+  CHECK_EQ(channels_ % group_, 0);
+  CHECK_EQ(num_output_ % group_, 0) << "Number of output should be multiples of group.";
+  CHECK(stride_h_ <= mscnn::kDeconvMaxStride && stride_w_ <= mscnn::kDeconvMaxStride)
+      << "mscnn_b200 Deconvolution serves strides 1..8 (layer " << name << ")";
+  CHECK(mscnn::deconv_axis_ok(kernel_h_, stride_h_, pad_h_, dilation_h_) &&
+        mscnn::deconv_axis_ok(kernel_w_, stride_w_, pad_w_, dilation_w_))
+      << "mscnn_b200 Deconvolution serves pads and dilated kernel reaches up to 2^20 (layer " << name << ")";
+  CHECK(!(group_ == channels_ && group_ > 1 && num_output_ != channels_))
+      << "mscnn_b200 Deconvolution does not serve a depthwise layer with a channel multiplier (layer " << name << ": "
+      << channels_ << " -> " << num_output_ << ", group " << group_ << ")";
+  CHECK(group_ == 1 || depthwise() || (channels_ / group_ % 64 == 0 && num_output_ / group_ % 64 == 0))
+      << "mscnn_b200 Deconvolution serves group > 1 only when the input and output channels of one group are 1 "
+         "(depthwise) or multiples of 64 (layer " << name << ": " << channels_ << " -> " << num_output_ << ", group "
+      << group_ << ")";
+  bias_term_ = p.bias_term();
+  if (this->blobs_.size() > 0) {
+    CHECK_EQ((int)this->blobs_.size(), 1 + (bias_term_ ? 1 : 0)) << "Incorrect number of weight blobs.";
+  } else {
+    this->blobs_.resize(bias_term_ ? 2 : 1);
+    this->blobs_[0].reset(new Blob<Dtype>(channels_, num_output_ / group_, kernel_h_, kernel_w_));
     FillBlob(p.weight_filler(), this->blobs_[0].get());
+    if (bias_term_) {
+      this->blobs_[1].reset(new Blob<Dtype>(vector<int>(1, num_output_)));
+      FillBlob(p.bias_filler(), this->blobs_[1].get());
+    }
   }
 }
+
 template <typename Dtype>
 void DeconvolutionLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
-  // deconv_layer.cpp:8-22: stride*(in-1) + kernel - 2*pad = 2*in
-  top[0]->Reshape(bottom[0]->num(), channels_, 2 * bottom[0]->height(), 2 * bottom[0]->width());
+  CHECK_EQ(bottom[0]->channels(), channels_) << "Input size incompatible with convolution kernel.";
+  // deconv_layer.cpp:8-22
+  const int ho = mscnn::deconv_out_size(bottom[0]->height(), kernel_h_, stride_h_, pad_h_, dilation_h_);
+  const int wo = mscnn::deconv_out_size(bottom[0]->width(), kernel_w_, stride_w_, pad_w_, dilation_w_);
+  CHECK(ho > 0 && wo > 0) << "mscnn_b200 Deconvolution: the output extent " << ho << " x " << wo
+                          << " is not positive (layer " << this->layer_param_.name() << ")";
+  top[0]->Reshape(bottom[0]->num(), num_output_, ho, wo);
 }
+
 template <typename Dtype>
 void DeconvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   const bool split = Caffe::split();
+  Blob<Dtype>* wb = this->blobs_[0].get();
+  Blob<Dtype>* bias = bias_term_ ? this->blobs_[1].get() : nullptr;
   typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
+  // group == channels == num_output: a gather per output pixel straight from the blob [C][1][kh][kw]
+  if (depthwise()) {
+    typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
+    MSCNN_CHECK(mscnn_deconv_depthwise_forward(x.hi, x.lo, wb->gpu_data(), bias ? bias->gpu_data() : nullptr, y.hi,
+                                               y.lo, x.n, x.h, x.w, x.cpad, channels_, kernel_h_, kernel_w_, stride_h_,
+                                               stride_w_, pad_h_, pad_w_, dilation_h_, dilation_w_, Caffe::stream()));
+    return;
+  }
+  // The blob [Cin][Cout / group][kh][kw] packs into one stride-1 sub-kernel per output phase
+  // (mscnn_pack_deconv_weights), each [Cout_pad][m_h][m_w][cin_pad].
+  const int cout_pad = pad64(num_output_), cin_pad = pad64(channels_ / group_);
+  const long long elems = mscnn_deconv_packed_elems(channels_, num_output_, group_, kernel_h_, kernel_w_, stride_h_,
+                                                    stride_w_, pad_h_, pad_w_, dilation_h_, dilation_w_, cout_pad);
+  CHECK_GE(elems, 0);
+  packed_.update_weights(wb, {PackedParam::DECONV, split, cout_pad, cin_pad, 0, 0, 0}, (size_t)elems * 2,
+                         [&](const float* w, void* hi, void* lo) {
+    MSCNN_CHECK(mscnn_pack_deconv_weights(w, hi, lo, channels_, num_output_, group_, kernel_h_, kernel_w_, stride_h_,
+                                          stride_w_, pad_h_, pad_w_, dilation_h_, dilation_w_, cout_pad,
+                                          Caffe::stream()));
+  });
+  packed_.bias.update(bias, num_output_, cout_pad);
+  mscnn_conv_desc d = conv_desc(x, packed_, x.n, x.h, x.w, x.cpad, num_output_, kernel_h_, kernel_w_, pad_h_, pad_w_,
+                                nullptr);
+  d.stride_h = stride_h_; d.stride_w = stride_w_;
+  d.dil_h = dilation_h_; d.dil_w = dilation_w_;
+  d.group = group_;
+  d.out_mode = MSCNN_OUT_NHWC_BF16;
   typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
-  MSCNN_CHECK(mscnn_deconv2x_forward(x.hi, x.lo, this->blobs_[0]->gpu_data(), y.hi, y.lo, x.n, x.h, x.w, x.cpad,
-                                     channels_, Caffe::stream()));
+  d.y_hi = y.hi;
+  d.y_lo = y.lo;
+  MSCNN_CHECK(mscnn_deconv_forward(&d, Caffe::stream()));
 }
 
 // ----------------------------------------------------------------------------------- ReLU

@@ -47,8 +47,10 @@
 
 #include <mutex>
 #include <unordered_map>
+#include <vector>
 
 #include "config.h"
+#include "deconv_phase.h"
 #include "mscnn_b200.h"
 #include "ptx_sm90.cuh"
 #include "tmap.h"
@@ -496,9 +498,16 @@ struct ConvPlan {
   size_t smem;
 };
 
+// The output a launch writes instead of the dense planes [N][Ho][Wo][Cout_pad]: pixels (q_h step_h + r_h,
+// q_w step_w + r_w), q in [0, ho) x [0, wo), of planes [N][full_h][full_w][Cout_pad] -- one output phase of a
+// deconvolution (mscnn_deconv_forward), whose stride-1 sub-convolution may also have a negative pad.
+struct OutView {
+  int ho, wo, step_h, step_w, r_h, r_w, full_h, full_w;
+};
+
 struct PlanKey {
   const void* ptr[11];
-  int v[20];
+  int v[28];
   bool operator==(const PlanKey& o) const { return memcmp(this, &o, sizeof(PlanKey)) == 0; }
 };
 struct PlanKeyHash {
@@ -517,7 +526,51 @@ void conv_plan_cache_clear() {
   g_plans.clear();
 }
 
-static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps = true);
+static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps = true,
+                      const OutView* view = nullptr);
+
+// The cached launch plan of (d, view), built and cached on a miss.
+static int resolve_plan(const mscnn_conv_desc* d, const OutView* view, int device, ConvPlan* plan) {
+  PlanKey key;
+  memset(&key, 0, sizeof(key));
+  const void* ptrs[11] = {d->x_hi, d->x_lo, d->w_hi, d->w_lo, d->bias, d->y_hi, d->y_lo, d->y_f32, d->pool_hi, d->pool_lo, d->dyn_n};
+  memcpy(key.ptr, ptrs, sizeof(ptrs));
+  const OutView dense = {0, 0, 0, 0, 0, 0, 0, 0};
+  const OutView& v = view ? *view : dense;
+  const int vals[28] = {d->N, d->H, d->W, d->C, d->Cout, d->Cout_pad, d->KH, d->KW, d->pad_h, d->pad_w, d->relu,
+                        d->out_mode, device, static_cast<int>(config().epoch), 0,
+                        d->stride_h, d->stride_w, d->dil_h, d->dil_w, d->group,
+                        v.ho, v.wo, v.step_h, v.step_w, v.r_h, v.r_w, v.full_h, v.full_w};
+  memcpy(key.v, vals, sizeof(vals));
+  {
+    std::lock_guard<std::mutex> lk(g_plan_mu);
+    auto it = g_plans.find(key);
+    if (it != g_plans.end()) {
+      *plan = it->second;
+      return MSCNN_OK;
+    }
+  }
+  const int rc = build_plan(d, plan, true, view);
+  if (rc != MSCNN_OK) return rc;
+  std::lock_guard<std::mutex> lk(g_plan_mu);
+  if (g_plans.size() >= 4096) g_plans.clear();  // blobs that keep moving (re-allocation): bound the table
+  g_plans.emplace(key, *plan);
+  return MSCNN_OK;
+}
+
+static int launch_plan(const ConvPlan& plan, int device, cudaStream_t stream, const char* who) {
+  // [BLOCK_N = 32 << i][fat]; fat stages only below BLOCK_N = 256 (build_plan): no <256, true> instantiation
+  static const decltype(&launch_igemm<32, false>) launch[4][2] = {
+      {launch_igemm<32, false>, launch_igemm<32, true>}, {launch_igemm<64, false>, launch_igemm<64, true>},
+      {launch_igemm<128, false>, launch_igemm<128, true>}, {launch_igemm<256, false>, nullptr}};
+  const cudaError_t e =
+      launch[__builtin_ctz(plan.BN) - 5][plan.p.fat](plan.maps, plan.p, plan.grid, plan.smem, device, stream);
+  if (e != cudaSuccess) {
+    fprintf(stderr, "%s: launch failed: %s\n", who, cudaGetErrorString(e));
+    return MSCNN_ERR_CUDA;
+  }
+  return MSCNN_OK;
+}
 
 }  // namespace mscnn
 
@@ -528,42 +581,10 @@ extern "C" int mscnn_conv_forward(const mscnn_conv_desc* d, void* stream_v) {
   if (!d) return MSCNN_ERR_INVALID;
   int device = 0;
   if (cudaGetDevice(&device) != cudaSuccess) return MSCNN_ERR_CUDA;
-  PlanKey key;
-  memset(&key, 0, sizeof(key));
-  const void* ptrs[11] = {d->x_hi, d->x_lo, d->w_hi, d->w_lo, d->bias, d->y_hi, d->y_lo, d->y_f32, d->pool_hi, d->pool_lo, d->dyn_n};
-  memcpy(key.ptr, ptrs, sizeof(ptrs));
-  const int vals[20] = {d->N, d->H, d->W, d->C, d->Cout, d->Cout_pad, d->KH, d->KW, d->pad_h, d->pad_w, d->relu,
-                        d->out_mode, device, static_cast<int>(config().epoch), 0,
-                        d->stride_h, d->stride_w, d->dil_h, d->dil_w, d->group};
-  memcpy(key.v, vals, sizeof(vals));
   ConvPlan plan;
-  bool hit = false;
-  {
-    std::lock_guard<std::mutex> lk(g_plan_mu);
-    auto it = g_plans.find(key);
-    if (it != g_plans.end()) {
-      plan = it->second;
-      hit = true;
-    }
-  }
-  if (!hit) {
-    const int rc = build_plan(d, &plan);
-    if (rc != MSCNN_OK) return rc;
-    std::lock_guard<std::mutex> lk(g_plan_mu);
-    if (g_plans.size() >= 4096) g_plans.clear();  // blobs that keep moving (re-allocation): bound the table
-    g_plans.emplace(key, plan);
-  }
-  // [BLOCK_N = 32 << i][fat]; fat stages only below BLOCK_N = 256 (build_plan): no <256, true> instantiation
-  static const decltype(&launch_igemm<32, false>) launch[4][2] = {
-      {launch_igemm<32, false>, launch_igemm<32, true>}, {launch_igemm<64, false>, launch_igemm<64, true>},
-      {launch_igemm<128, false>, launch_igemm<128, true>}, {launch_igemm<256, false>, nullptr}};
-  const cudaError_t e =
-      launch[__builtin_ctz(plan.BN) - 5][plan.p.fat](plan.maps, plan.p, plan.grid, plan.smem, device, stream);
-  if (e != cudaSuccess) {
-    fprintf(stderr, "mscnn_conv_forward: launch failed: %s\n", cudaGetErrorString(e));
-    return MSCNN_ERR_CUDA;
-  }
-  return MSCNN_OK;
+  const int rc = resolve_plan(d, nullptr, device, &plan);
+  if (rc != MSCNN_OK) return rc;
+  return launch_plan(plan, device, stream, "mscnn_conv_forward");
 }
 
 namespace mscnn {
@@ -604,14 +625,18 @@ static int unsupported(const mscnn_conv_desc* d, const char* rule) {
   return MSCNN_ERR_INVALID;
 }
 
-static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps) {
+// view != NULL (a deconvolution phase): the output extents are the view's, the pad may be negative (the extents are
+// not derived from it), and only NHWC_BF16 planes without pooling or dyn_n are written.
+static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps, const OutView* view) {
   const Config& cfg = config();
   if (!d->x_hi || !d->w_hi || !d->bias) return MSCNN_ERR_INVALID;
   if (d->C % 64 != 0) return MSCNN_ERR_INVALID;
   const bool split = (d->x_lo != nullptr);
   if (split && !d->w_lo) return MSCNN_ERR_INVALID;
   const int sh = or1(d->stride_h), sw = or1(d->stride_w), dh = or1(d->dil_h), dw = or1(d->dil_w), g = or1(d->group);
-  if (d->KH <= 0 || d->KW <= 0 || d->pad_h < 0 || d->pad_w < 0) return MSCNN_ERR_INVALID;
+  if (d->KH <= 0 || d->KW <= 0 || (!view && (d->pad_h < 0 || d->pad_w < 0))) return MSCNN_ERR_INVALID;
+  if (view && (view->ho <= 0 || view->wo <= 0 || d->out_mode != MSCNN_OUT_NHWC_BF16 || d->pool_hi || d->dyn_n))
+    return MSCNN_ERR_INVALID;
   if (sh < 1 || sh > 4 || sw < 1 || sw > 4) return unsupported(d, "strides 1..4 are served");
   // the furthest tap coordinate, pad + extent + reach, has to stay far inside a tensor map's int32 coordinates
   if (dh < 1 || dw < 1 || dh > (1 << 20) / d->KH || dw > (1 << 20) / d->KW)
@@ -620,9 +645,9 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
   if (g > 1 && (d->C % g || d->Cout % g || d->C / g % 64 || d->Cout / g % 64 || d->Cout_pad != d->Cout))
     return unsupported(d, "a grouped convolution needs C / group and Cout / group to be multiples of 64");
   const int ext_h = dh * (d->KH - 1) + 1, ext_w = dw * (d->KW - 1) + 1;  // conv_layer.cpp:8-22
-  if (d->H + 2 * d->pad_h < ext_h || d->W + 2 * d->pad_w < ext_w || d->N <= 0) return MSCNN_ERR_INVALID;
-  const int Ho = (d->H + 2 * d->pad_h - ext_h) / sh + 1;
-  const int Wo = (d->W + 2 * d->pad_w - ext_w) / sw + 1;
+  if (d->N <= 0 || (!view && (d->H + 2 * d->pad_h < ext_h || d->W + 2 * d->pad_w < ext_w))) return MSCNN_ERR_INVALID;
+  const int Ho = view ? view->ho : (d->H + 2 * d->pad_h - ext_h) / sh + 1;
+  const int Wo = view ? view->wo : (d->W + 2 * d->pad_w - ext_w) / sw + 1;
   const int cin_g = d->C / g, cout_g = d->Cout_pad / g;
   const int BN = pick_block_n(cout_g);
   if (d->Cout_pad % BN != 0 || d->Cout > d->Cout_pad) return MSCNN_ERR_INVALID;
@@ -717,8 +742,16 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
   // The kernel's maps A_hi, A_lo, B_hi, B_lo, O_hi, O_lo, P_hi, P_lo (P: fused pooling output).  One the launch does
   // not use is a copy of its primary (a lo plane of its hi plane, a hi plane of A_hi), so every argument is valid.
   const bool lo_out = staged && p.has_lo_out;
+  // a view starts at pixel (r_h, r_w) of the full planes and steps (step_h, step_w) pixels: every byte stride is a
+  // multiple of Cout_pad * 2 = 128 B
+  const size_t pix = (size_t)d->Cout_pad * 2;
+  const size_t view_off = view ? ((size_t)view->r_h * view->full_w + view->r_w) * pix : 0;
+  const uint64_t view_strides[3] = {view ? view->step_w * pix : 0, view ? (size_t)view->step_h * view->full_w * pix : 0,
+                                    view ? (size_t)view->full_h * view->full_w * pix : 0};
+  void* y_hi = d->y_hi ? static_cast<uint8_t*>(d->y_hi) + view_off : nullptr;
+  void* y_lo = d->y_lo ? static_cast<uint8_t*>(d->y_lo) + view_off : nullptr;
   const void* src[8] = {d->x_hi, split ? d->x_lo : nullptr, d->w_hi, split ? d->w_lo : nullptr,
-                        staged ? d->y_hi : nullptr, lo_out ? d->y_lo : nullptr,
+                        staged ? y_hi : nullptr, lo_out ? y_lo : nullptr,
                         p.pool ? d->pool_hi : nullptr, p.pool && lo_out ? d->pool_lo : nullptr};
   const uint64_t dims[4][4] = {{(uint64_t)d->C, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->N},
                                {},
@@ -737,7 +770,8 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
     }
     const int rc = (i >> 1) == 1
                        ? tmap_2d_bf16(&maps[i], src[i], (uint64_t)d->KH * d->KW * cin_g, (uint64_t)d->Cout_pad, 64u, (uint32_t)BN)
-                       : tmap_nhwc_bf16(&maps[i], src[i], dims[i >> 1], boxes[i >> 1], (i >> 1) == 0 ? a_strides : nullptr);
+                       : tmap_nhwc_bf16(&maps[i], src[i], dims[i >> 1], boxes[i >> 1], (i >> 1) == 0 ? a_strides : nullptr,
+                                        (i >> 1) == 2 && view ? view_strides : nullptr);
     if (rc) return rc;
   }
 
@@ -753,12 +787,10 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
 // the pointers in `d` only have to be non-NULL where the call would require them): which instantiation, pixel box,
 // operand staging and pipeline depth (`stages` = depth of the ring carrying the weights; with rowshare=1 the
 // activation tiles have their own ring of a_stages slots).  Host-side tests pin the variant every full-size layer takes.
-extern "C" int mscnn_conv_plan_describe(const mscnn_conv_desc* d, char* buf, int cap) {
-  if (!d || !buf || cap <= 0) return MSCNN_ERR_INVALID;
-  mscnn::ConvPlan plan;
-  const int rc = mscnn::build_plan(d, &plan, false);
-  if (rc != MSCNN_OK) return rc;
-  const mscnn::IgemmParams& p = plan.p;
+namespace mscnn {
+
+static int format_plan(const ConvPlan& plan, const mscnn_conv_desc* d, char* buf, int cap) {
+  const IgemmParams& p = plan.p;
   int n = snprintf(buf, (size_t)cap,
                          "kernel=conv_igemm_kernel<%d, %s> box=%dx%dx%d terms=%d fat=%d pool=%d stages=%d epi_bufs=%d "
                          "smem=%zu dyn=%d rowshare=%d a_stages=%d",
@@ -774,10 +806,193 @@ extern "C" int mscnn_conv_plan_describe(const mscnn_conv_desc* d, char* buf, int
   return (n > 0 && n < cap) ? MSCNN_OK : MSCNN_ERR_INVALID;
 }
 
+}  // namespace mscnn
+
+extern "C" int mscnn_conv_plan_describe(const mscnn_conv_desc* d, char* buf, int cap) {
+  if (!d || !buf || cap <= 0) return MSCNN_ERR_INVALID;
+  mscnn::ConvPlan plan;
+  const int rc = mscnn::build_plan(d, &plan, false);
+  if (rc != MSCNN_OK) return rc;
+  return mscnn::format_plan(plan, d, buf, cap);
+}
+
 // Entries in the launch-plan cache.  A net adds one per convolution for every new combination of input shape and blob
 // addresses it runs with; the table is emptied when it reaches 4096 entries, so it stays bounded however many input
 // sizes a process goes through.
 extern "C" int mscnn_conv_plan_count(void) {
   std::lock_guard<std::mutex> lk(mscnn::g_plan_mu);
   return (int)mscnn::g_plans.size();
+}
+
+// ------------------------------------------------------------------ deconvolution by output phase
+// DeconvolutionLayer::Forward_gpu (deconv_layer.cu) for dense and 64-aligned grouped layers: the output is split by
+// phase (deconv_phase.h) and each phase is a stride-1 convolution of the input with its own sub-kernel, signed pad and
+// extent, run by conv_igemm_kernel with the phase's pixels of the full output planes as its output tensor map.
+
+namespace mscnn {
+
+// A phase no tap reaches holds the bias alone (col2im leaves it zero, the bias is added after): one channel pair of
+// one pixel of the view per thread, bias + ReLU split into (hi, lo) as the GEMM epilogue does with a zero sum.
+__global__ void deconv_bias_fill_kernel(const float* __restrict__ bias, __nv_bfloat16* __restrict__ yh,
+                                        __nv_bfloat16* __restrict__ yl, int N, int Ho, int Wo, int cpad, int r_h,
+                                        int r_w, int s_h, int s_w, int q_h, int q_w, int relu) {
+  const int pairs = cpad / 2;
+  const size_t total = (size_t)N * q_h * q_w * pairs;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = 2 * (int)(i % pairs);
+    size_t r = i / pairs;
+    const int qw = (int)(r % q_w);
+    r /= q_w;
+    const int qh = (int)(r % q_h);
+    const size_t n = r / q_h;
+    const float2 f = ptx::bias_relu(0.f, 0.f, bias[c], bias[c + 1], relu);
+    const uint32_t h = ptx::pack_bf16x2(f.x, f.y);
+    const uint32_t l = ptx::pack_bf16x2(f.x - __uint_as_float(h << 16), f.y - __uint_as_float(h & 0xFFFF0000u));
+    const size_t o = ((n * Ho + (size_t)qh * s_h + r_h) * Wo + (size_t)qw * s_w + r_w) * cpad + c;
+    *reinterpret_cast<uint32_t*>(yh + o) = h;
+    if (yl) *reinterpret_cast<uint32_t*>(yl + o) = l;
+  }
+}
+
+struct DeconvGeom {
+  int sh, sw, dh, dw, g, Ho, Wo;
+};
+
+static int deconv_unsupported(const mscnn_conv_desc* d, const char* rule) {
+  fprintf(stderr,
+          "mscnn_deconv_forward: kernel %dx%d, stride %dx%d, pad %dx%d, dilation %dx%d, group %d, C=%d Cout=%d "
+          "Cout_pad=%d, input %dx%d: %s\n",
+          d->KH, d->KW, or1(d->stride_h), or1(d->stride_w), d->pad_h, d->pad_w, or1(d->dil_h), or1(d->dil_w),
+          or1(d->group), d->C, d->Cout, d->Cout_pad, d->H, d->W, rule);
+  return MSCNN_ERR_INVALID;
+}
+
+// The geometry of a deconvolution descriptor; MSCNN_ERR_INVALID, with a message for a geometry not served.
+static int deconv_geometry(const mscnn_conv_desc* d, DeconvGeom* q) {
+  if (!d->x_hi || !d->w_hi || !d->bias || !d->y_hi || d->N <= 0 || d->H <= 0 || d->W <= 0) return MSCNN_ERR_INVALID;
+  if (d->x_lo && !d->w_lo) return MSCNN_ERR_INVALID;
+  if (d->out_mode != MSCNN_OUT_NHWC_BF16) return deconv_unsupported(d, "the output is served as NHWC_BF16 planes only");
+  if (d->pool_hi || d->pool_lo) return deconv_unsupported(d, "no fused pooling is served");
+  if (d->dyn_n) return deconv_unsupported(d, "dyn_n must be NULL");
+  q->sh = or1(d->stride_h);
+  q->sw = or1(d->stride_w);
+  q->dh = or1(d->dil_h);
+  q->dw = or1(d->dil_w);
+  q->g = or1(d->group);
+  if (q->sh < 1 || q->sh > kDeconvMaxStride || q->sw < 1 || q->sw > kDeconvMaxStride)
+    return deconv_unsupported(d, "strides 1..8 are served");
+  if (!deconv_axis_ok(d->KH, q->sh, d->pad_h, q->dh) || !deconv_axis_ok(d->KW, q->sw, d->pad_w, q->dw))
+    return deconv_unsupported(d, "kernel >= 1, pad in 0..2^20 and dilation >= 1 with a kernel reach up to 2^20 are served");
+  if (q->g < 1 || d->C % 64 || d->Cout < 1 || d->Cout_pad % 64 || d->Cout > d->Cout_pad)
+    return deconv_unsupported(d, "C and Cout_pad must be multiples of 64 and Cout_pad >= Cout >= 1");
+  if (q->g > 1 && (d->C % q->g || d->Cout % q->g || d->C / q->g % 64 || d->Cout / q->g % 64 || d->Cout_pad != d->Cout))
+    return deconv_unsupported(d, "a grouped deconvolution needs C / group and Cout / group to be multiples of 64 "
+                                 "(group == channels: mscnn_deconv_depthwise_forward)");
+  q->Ho = deconv_out_size(d->H, d->KH, q->sh, d->pad_h, q->dh);
+  q->Wo = deconv_out_size(d->W, d->KW, q->sw, d->pad_w, q->dw);
+  if (q->Ho <= 0 || q->Wo <= 0) return deconv_unsupported(d, "the output extent must be positive");
+  return MSCNN_OK;
+}
+
+// Phase i = r_h s_w + r_w: its axes, its stride-1 sub-convolution and the view of the output it writes.
+struct DeconvPhase {
+  DeconvAxis h, w;
+  mscnn_conv_desc sub;
+  OutView view;
+  bool launches() const { return h.taps > 0 && w.taps > 0 && view.ho > 0 && view.wo > 0; }
+  bool fills() const { return (h.taps == 0 || w.taps == 0) && view.ho > 0 && view.wo > 0; }
+};
+
+static DeconvPhase deconv_phase(const mscnn_conv_desc* d, const DeconvGeom& q, int i) {
+  DeconvPhase ph;
+  ph.h = deconv_axis(d->KH, q.sh, d->pad_h, q.dh, q.Ho, i / q.sw);
+  ph.w = deconv_axis(d->KW, q.sw, d->pad_w, q.dw, q.Wo, i % q.sw);
+  const long long off =
+      deconv_phase_offset(d->C, q.g, d->KH, d->KW, q.sh, q.sw, d->pad_h, d->pad_w, q.dh, q.dw, d->Cout_pad, i);
+  ph.sub = *d;
+  ph.sub.w_hi = static_cast<const __nv_bfloat16*>(d->w_hi) + off;
+  ph.sub.w_lo = d->w_lo ? static_cast<const __nv_bfloat16*>(d->w_lo) + off : nullptr;
+  ph.sub.KH = ph.h.taps;
+  ph.sub.KW = ph.w.taps;
+  ph.sub.pad_h = ph.h.pad;
+  ph.sub.pad_w = ph.w.pad;
+  ph.sub.stride_h = ph.sub.stride_w = 1;
+  ph.sub.dil_h = ph.h.dil;
+  ph.sub.dil_w = ph.w.dil;
+  ph.sub.group = q.g;
+  ph.view = {ph.h.ext, ph.w.ext, q.sh, q.sw, i / q.sw, i % q.sw, q.Ho, q.Wo};
+  return ph;
+}
+
+}  // namespace mscnn
+
+extern "C" int mscnn_deconv_forward(const mscnn_conv_desc* d, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (!d) return MSCNN_ERR_INVALID;
+  DeconvGeom q;
+  int rc = deconv_geometry(d, &q);
+  if (rc != MSCNN_OK) return rc;
+  int device = 0;
+  if (cudaGetDevice(&device) != cudaSuccess) return MSCNN_ERR_CUDA;
+  // every phase's plan before the first launch: a descriptor that any phase refuses writes nothing
+  const int phases = q.sh * q.sw;
+  std::vector<DeconvPhase> ph(phases);
+  std::vector<ConvPlan> plans(phases);
+  for (int i = 0; i < phases; ++i) {
+    ph[i] = deconv_phase(d, q, i);
+    if (ph[i].launches() && (rc = resolve_plan(&ph[i].sub, &ph[i].view, device, &plans[i])) != MSCNN_OK) return rc;
+  }
+  for (int i = 0; i < phases; ++i) {
+    if (ph[i].launches()) {
+      if ((rc = launch_plan(plans[i], device, stream, "mscnn_deconv_forward")) != MSCNN_OK) return rc;
+    } else if (ph[i].fills()) {
+      const OutView& v = ph[i].view;
+      const size_t total = (size_t)d->N * v.ho * v.wo * (d->Cout_pad / 2);
+      const size_t cap = (size_t)mscnn_sm_count() * 16;
+      const int grid = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
+      mscnn::note_launch();
+      deconv_bias_fill_kernel<<<grid, 256, 0, stream>>>(d->bias, static_cast<__nv_bfloat16*>(d->y_hi),
+                                                         static_cast<__nv_bfloat16*>(d->y_lo), d->N, q.Ho, q.Wo,
+                                                         d->Cout_pad, v.r_h, v.r_w, v.step_h, v.step_w, v.ho, v.wo,
+                                                         d->relu);
+      const cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) {
+        fprintf(stderr, "mscnn_deconv_forward: bias fill launch failed: %s\n", cudaGetErrorString(e));
+        return MSCNN_ERR_CUDA;
+      }
+    }
+  }
+  return MSCNN_OK;
+}
+
+// One line per output phase: its taps, sub-dilation, signed pad and extent, and the launch plan it runs
+// (mscnn_conv_plan_describe's text), "bias_fill" where no tap reaches it, "none" where it holds no output pixel.
+extern "C" int mscnn_deconv_plan_describe(const mscnn_conv_desc* d, char* buf, int cap) {
+  if (!d || !buf || cap <= 0) return MSCNN_ERR_INVALID;
+  DeconvGeom q;
+  int rc = deconv_geometry(d, &q);
+  if (rc != MSCNN_OK) return rc;
+  int n = 0;
+  buf[0] = '\0';
+  for (int i = 0; i < q.sh * q.sw; ++i) {
+    const DeconvPhase ph = deconv_phase(d, q, i);
+    int m = snprintf(buf + n, (size_t)(cap - n), "phase=%dx%d taps=%dx%d dil=%dx%d pad=%dx%d out=%dx%d plan=",
+                     ph.view.r_h, ph.view.r_w, ph.h.taps, ph.w.taps, ph.h.dil, ph.w.dil, ph.h.pad, ph.w.pad, ph.view.ho,
+                     ph.view.wo);
+    if (m < 0 || m >= cap - n) return MSCNN_ERR_INVALID;
+    n += m;
+    if (ph.launches()) {
+      ConvPlan plan;
+      if ((rc = build_plan(&ph.sub, &plan, false, &ph.view)) != MSCNN_OK) return rc;
+      if ((rc = format_plan(plan, &ph.sub, buf + n, cap - n)) != MSCNN_OK) return rc;
+      m = (int)strlen(buf + n);
+    } else {
+      m = snprintf(buf + n, (size_t)(cap - n), "%s", ph.fills() ? "bias_fill" : "none");
+    }
+    if (m < 0 || m + 1 >= cap - n) return MSCNN_ERR_INVALID;
+    n += m;
+    buf[n++] = '\n';
+    buf[n] = '\0';
+  }
+  return MSCNN_OK;
 }

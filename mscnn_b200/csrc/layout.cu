@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "deconv_phase.h"
 #include "mscnn_b200.h"
 #include "launch_count.h"
 
@@ -87,6 +88,35 @@ __global__ void planes_to_nchw_kernel(const __nv_bfloat16* __restrict__ hi,
   for (int cc = warp; cc < 64; cc += 8) {
     const int c = c0 + cc, w = w0 + lane;
     if (c < C && w < W) y[((size_t)(n * C + c) * H + h) * W + w] = tile[cc][lane];
+  }
+}
+
+// One deconvolution output phase's sub-kernel (deconv_phase.h) from the Caffe blob [Cin][Cout / group][KH][KW]:
+//   out[((co m_h + uh) m_w + uw) cin_gp + ci] = w[k cin_g + ci][co - k cout_g][t0_h + (m_h - 1 - uh) step_h]
+//                                                [t0_w + (m_w - 1 - uw) step_w],   k = co / cout_g,
+// input and output channels swapped and the taps reversed; zero for co >= Cout or ci >= cin_g.
+__global__ void pack_deconv_w_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ hi,
+                                     __nv_bfloat16* __restrict__ lo, int Cout, int cin_g, int cout_g, int KH, int KW,
+                                     int Cout_pad, int cin_gp, DeconvAxis ah, DeconvAxis aw) {
+  const size_t total = (size_t)Cout_pad * ah.taps * aw.taps * cin_gp;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (size_t)gridDim.x * blockDim.x) {
+    const int ci = i % cin_gp;
+    size_t r = i / cin_gp;
+    const int uw = r % aw.taps;
+    r /= aw.taps;
+    const int uh = r % ah.taps;
+    const int co = r / ah.taps;
+    float v = 0.f;
+    if (co < Cout && ci < cin_g) {
+      const int k = co / cout_g;
+      const int th = ah.t0 + (ah.taps - 1 - uh) * ah.tstep, tw = aw.t0 + (aw.taps - 1 - uw) * aw.tstep;
+      v = w[(((size_t)(k * cin_g + ci) * cout_g + (co - k * cout_g)) * KH + th) * KW + tw];
+    }
+    __nv_bfloat16 h, l;
+    split_bf16(v, h, l);
+    hi[i] = h;
+    if (lo) lo[i] = l;
   }
 }
 
@@ -227,6 +257,38 @@ extern "C" int mscnn_pack_conv_weights(const float* w, void* hi, void* lo, int C
   pack_conv_w_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
       w, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, Cout, Cin, KH * KW, Cout_pad, Cin_pad);
   return check_launch("pack_conv_w");
+}
+
+extern "C" long long mscnn_deconv_packed_elems(int Cin, int Cout, int group, int KH, int KW, int stride_h, int stride_w,
+                                               int pad_h, int pad_w, int dil_h, int dil_w, int Cout_pad) {
+  if (Cout < 1 || group < 1 || Cout % group || Cout_pad < Cout) return -1;
+  return mscnn::deconv_phase_offset(Cin, group, KH, KW, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, Cout_pad,
+                                    stride_h * stride_w);
+}
+
+extern "C" int mscnn_pack_deconv_weights(const float* w, void* hi, void* lo, int Cin, int Cout, int group, int KH,
+                                         int KW, int stride_h, int stride_w, int pad_h, int pad_w, int dil_h,
+                                         int dil_w, int Cout_pad, void* stream) {
+  if (!w || !hi || mscnn_deconv_packed_elems(Cin, Cout, group, KH, KW, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w,
+                                             Cout_pad) < 0)
+    return MSCNN_ERR_INVALID;
+  const int cin_g = Cin / group, cin_gp = (cin_g + 63) / 64 * 64;
+  for (int i = 0; i < stride_h * stride_w; ++i) {
+    const DeconvAxis ah = deconv_axis(KH, stride_h, pad_h, dil_h, 0, i / stride_w);
+    const DeconvAxis aw = deconv_axis(KW, stride_w, pad_w, dil_w, 0, i % stride_w);
+    if (ah.taps == 0 || aw.taps == 0) continue;
+    const long long off = deconv_phase_offset(Cin, group, KH, KW, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w,
+                                              Cout_pad, i);
+    const size_t total = (size_t)Cout_pad * ah.taps * aw.taps * cin_gp;
+    const int blocks = (int)((total + 255) / 256 > 132 * 16 ? 132 * 16 : (total + 255) / 256);
+    mscnn::note_launch();
+    pack_deconv_w_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
+        w, (__nv_bfloat16*)hi + off, lo ? (__nv_bfloat16*)lo + off : nullptr, Cout, cin_g, Cout / group, KH, KW,
+        Cout_pad, cin_gp, ah, aw);
+    const int rc = check_launch("pack_deconv_w");
+    if (rc != MSCNN_OK) return rc;
+  }
+  return MSCNN_OK;
 }
 
 extern "C" int mscnn_pack_fc_weights(const float* w, void* hi, void* lo, int Nout, int C, int H,

@@ -1,4 +1,4 @@
-// HBM-bound plane kernels: Pooling, ROIPooling (+ fused Concat), depthwise 2x Deconvolution.
+// HBM-bound plane kernels: Pooling, ROIPooling (+ fused Concat), depthwise Deconvolution.
 // All work on NHWC bf16 planes with 16-byte (8-channel) vector accesses, so a warp touches
 // 512 contiguous bytes per pixel; values of split tensors are hi + lo evaluated in fp32.
 #include <cuda_bf16.h>
@@ -6,6 +6,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "deconv_phase.h"
 #include "mscnn_b200.h"
 #include "launch_count.h"
 
@@ -355,52 +356,78 @@ __global__ void roi_align_kernel(const __nv_bfloat16* __restrict__ xh, const __n
   }
 }
 
-// ------------------------------------------------------------ depthwise Deconvolution 2x
-// DeconvolutionLayer::Forward_cpu (src/caffe/layers/deconv_layer.cpp:25-40) for the shape the
-// MS-CNN "-2x" nets use: group == channels, kernel 4, stride 2, pad 1, no bias
-// (examples/kitti_car/mscnn-7s-576-2x/mscnn_deploy.prototxt:452-466):
-//   y[n, c, 2*iy - 1 + ky, 2*ix - 1 + kx] += x[n, c, iy, ix] * w[c, ky, kx]
-// Gather form: each output pixel has exactly 2 x 2 contributing taps.  Weights are read from
-// the layer blob (the bilinear filler is just the usual content, filler.hpp:248-258).
-__global__ void deconv2x_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl,
-                                const float* __restrict__ wt /*[C][4][4]*/, __nv_bfloat16* __restrict__ yh,
-                                __nv_bfloat16* __restrict__ yl, int N, int H, int W, int C, int Creal) {
-  // The 16 taps of every channel, staged once per block as w_s[(tap * 8 + i) * cg + g] (channel c = 8 g + i): a warp
-  // reads consecutive g, so the reads are conflict-free.  (Reading wt[(c * 4 + ky) * 4 + kx] from global memory cost 32
-  // scattered 4-byte loads per thread, many times the layer's HBM time.)
+// ------------------------------------------------------------ depthwise Deconvolution
+// DeconvolutionLayer::Forward_cpu (src/caffe/layers/deconv_layer.cpp:25-40) with group == channels == num_output,
+// e.g. the bilinear up-sampling of the MS-CNN "-2x" nets (kernel 4, stride 2, pad 1, no bias;
+// examples/kitti_car/mscnn-7s-576-2x/mscnn_deploy.prototxt:452-466):
+//   y[n, c, s_h iy - p_h + ky d_h, s_w ix - p_w + kx d_w] += x[n, c, iy, ix] * w[c, ky, kx],  then + bias[c]
+// Gather form: output row oy is reached by the taps ky with (oy + p_h - ky d_h) mod s_h == 0, which start at
+// ky0[(oy + p_h) mod s_h] and lie s_h / gcd(s_h, d_h) apart (likewise in x).  Weights are read from the layer blob
+// (the bilinear filler is just the usual content, filler.hpp:248-258).
+struct DwDeconvGeom {
+  int KH, KW, sh, sw, ph, pw, dh, dw;
+  int step_h, step_w;                          // s / gcd(s, d): distance between the taps of one output phase
+  int ky0[8], kx0[8];                          // first tap of phase (o + p) mod s; KH / KW when none reaches it
+};
+
+// Every block stages the taps of its slice of channel groups [g0, g0 + cgs) (blockIdx.y) as
+// w_s[(tap * 8 + i) * cgs + g - g0] (channel c = 8 g + i): a warp reads consecutive g, so the reads are
+// conflict-free.  (Reading wt[c * taps + tap] from global memory cost scattered 4-byte loads per thread, many times
+// the layer's HBM time.)  Wide kernels on many channels take several slices, so the staging fits shared memory.
+// K > 0: the geometry is fixed at compile time to K x K, stride S, pad P, dilation 1 (the -2x nets' 4 / 2 / 1 layer):
+// constant divisors and tap steps keep its index arithmetic as cheap as a kernel written for that shape alone.
+template <int K, int S, int P>
+__global__ void deconv_depthwise_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl,
+                                        const float* __restrict__ wt /*[Creal][KH][KW]*/,
+                                        const float* __restrict__ bias /*[Creal] or NULL*/,
+                                        __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl, int N, int H,
+                                        int W, int C, int Creal, int Ho, int Wo, int cgs, const DwDeconvGeom q) {
+  constexpr bool kFixed = K > 0;
+  const int KH = kFixed ? K : q.KH, KW = kFixed ? K : q.KW, sh = kFixed ? S : q.sh, sw = kFixed ? S : q.sw;
+  const int ph = kFixed ? P : q.ph, pw = kFixed ? P : q.pw, dh = kFixed ? 1 : q.dh, dw = kFixed ? 1 : q.dw;
+  const int step_h = kFixed ? S : q.step_h, step_w = kFixed ? S : q.step_w;
   extern __shared__ float w_s[];
-  const int cg = C / 8;
-  for (int j = threadIdx.x; j < 16 * C; j += blockDim.x) {
-    const int g = j % cg, i = (j / cg) % 8, tap = j / (8 * cg);
+  const int cg = C / 8, taps = KH * KW;
+  const int g0 = blockIdx.y * cgs;
+  for (int j = threadIdx.x; j < taps * 8 * cgs; j += blockDim.x) {
+    const int g = g0 + j % cgs, i = (j / cgs) % 8, tap = j / (8 * cgs);
     const int c = g * 8 + i;
-    w_s[j] = (c < Creal) ? wt[c * 16 + tap] : 0.f;
+    w_s[j] = (g < cg && c < Creal) ? wt[c * taps + tap] : 0.f;
   }
   __syncthreads();
-  const int Ho = 2 * H, Wo = 2 * W;
-  const size_t total = (size_t)N * Ho * Wo * cg;
+  const size_t total = (size_t)N * Ho * Wo * cgs;
   for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (size_t)gridDim.x * blockDim.x) {
-    const int g = idx % cg;
-    size_t r = idx / cg;
+    const int gl = idx % cgs, g = g0 + gl;
+    size_t r = idx / cgs;
     const int ox = r % Wo; r /= Wo;
     const int oy = r % Ho;
     const int n = r / Ho;
+    if (g >= cg) continue;
     Vec8 acc;
 #pragma unroll
     for (int i = 0; i < 8; ++i) acc.v[i] = 0.f;
-    // ky has the parity of oy+1; iy = (oy + 1 - ky) / 2.  The reference's col2im adds the
-    // kernel offsets in increasing (ky, kx) order (util/im2col.cpp:col2im_cpu), so do we.
-    for (int ky = (oy + 1) & 1; ky < 4; ky += 2) {
-      const int iy = (oy + 1 - ky) / 2;
-      if (oy + 1 - ky < 0 || iy >= H) continue;
-      for (int kx = (ox + 1) & 1; kx < 4; kx += 2) {
-        const int ix = (ox + 1 - kx) / 2;
-        if (ox + 1 - kx < 0 || ix >= W) continue;
+    // The reference's col2im adds the kernel offsets in increasing (ky, kx) order (util/im2col.cpp:col2im_cpu), so
+    // do we; taps that fall outside the input are skipped.  With dilation 1 the first tap of output row oy is
+    // (oy + p) mod s.
+    for (int ky = kFixed ? (int)((unsigned)(oy + P) % S) : q.ky0[(oy + ph) % sh]; ky < KH; ky += step_h) {
+      const int ny = oy + ph - ky * dh;
+      const int iy = ny / sh;
+      if (ny < 0 || iy >= H) continue;
+      for (int kx = kFixed ? (int)((unsigned)(ox + P) % S) : q.kx0[(ox + pw) % sw]; kx < KW; kx += step_w) {
+        const int nx = ox + pw - kx * dw;
+        const int ix = nx / sw;
+        if (nx < 0 || ix >= W) continue;
         const Vec8 v = load8(xh, xl, ((size_t)(n * H + iy) * W + ix) * C + g * 8);
-        const float* wp = w_s + (size_t)((ky * 4 + kx) * 8) * cg + g;
+        const float* wp = w_s + (size_t)((ky * KW + kx) * 8) * cgs + gl;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) acc.v[i] = acc.v[i] + v.v[i] * wp[i * cg];
+        for (int i = 0; i < 8; ++i) acc.v[i] = acc.v[i] + v.v[i] * wp[i * cgs];
       }
+    }
+    if (bias != nullptr) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        if (g * 8 + i < Creal) acc.v[i] = acc.v[i] + __ldg(bias + g * 8 + i);
     }
     store8(yh, yl, ((size_t)(n * Ho + oy) * Wo + ox) * C + g * 8, acc);
   }
@@ -579,21 +606,57 @@ extern "C" int mscnn_roi_align_forward(const void* x_hi, const void* x_lo, int N
                                      y_hi, y_lo, out_channels_total, out_channel_offset, nullptr, stream);
 }
 
+extern "C" int mscnn_deconv_depthwise_forward(const void* x_hi, const void* x_lo, const float* w, const float* bias,
+                                              void* y_hi, void* y_lo, int N, int H, int W, int C, int Creal, int KH,
+                                              int KW, int stride_h, int stride_w, int pad_h, int pad_w, int dil_h,
+                                              int dil_w, void* stream) {
+  if (!x_hi || !y_hi || !w || N <= 0 || H <= 0 || W <= 0 || C <= 0 || C % 8 || Creal <= 0 || Creal > C)
+    return MSCNN_ERR_INVALID;
+  if ((x_lo == nullptr) != (y_lo == nullptr)) return MSCNN_ERR_INVALID;
+  if (!deconv_axis_ok(KH, stride_h, pad_h, dil_h) || !deconv_axis_ok(KW, stride_w, pad_w, dil_w)) {
+    fprintf(stderr, "mscnn_deconv_depthwise_forward: kernel %dx%d, stride %dx%d, pad %dx%d, dilation %dx%d: strides "
+            "1..8, pad >= 0 and dilation >= 1 with a reach up to 2^20 are served\n", KH, KW, stride_h, stride_w, pad_h,
+            pad_w, dil_h, dil_w);
+    return MSCNN_ERR_INVALID;
+  }
+  const int Ho = deconv_out_size(H, KH, stride_h, pad_h, dil_h), Wo = deconv_out_size(W, KW, stride_w, pad_w, dil_w);
+  if (Ho <= 0 || Wo <= 0) return MSCNN_ERR_INVALID;
+  DwDeconvGeom q = {KH, KW, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, 1, 1, {}, {}};
+  for (int r = 0; r < 8; ++r) {
+    // phase r of (o + p) mod s: the axes' first taps (deconv_axis with p = 0 counts phases of o + p)
+    const DeconvAxis ay = deconv_axis(KH, stride_h, 0, dil_h, 0, r % stride_h);
+    const DeconvAxis ax = deconv_axis(KW, stride_w, 0, dil_w, 0, r % stride_w);
+    q.ky0[r] = ay.taps ? ay.t0 : KH;
+    q.kx0[r] = ax.taps ? ax.t0 : KW;
+    q.step_h = ay.tstep;
+    q.step_w = ax.tstep;
+  }
+  // channel-group slices whose staged taps fit 64 KB
+  const int cg = C / 8, taps = KH * KW;
+  const long long per_group = (long long)taps * 8 * sizeof(float);
+  if (per_group > 64 * 1024) return MSCNN_ERR_INVALID;  // a kernel of more than 2048 taps
+  const int max_groups = (int)((64 * 1024) / per_group);
+  const int slices = (cg + max_groups - 1) / max_groups, cgs = (cg + slices - 1) / slices;
+  if (slices > 65535) return MSCNN_ERR_INVALID;
+  const size_t w_smem = (size_t)per_group * cgs;
+  const bool shipped = KH == 4 && KW == 4 && stride_h == 2 && stride_w == 2 && pad_h == 1 && pad_w == 1 && dil_h == 1 &&
+                       dil_w == 1;
+  auto kern = shipped ? deconv_depthwise_kernel<4, 2, 1> : deconv_depthwise_kernel<0, 0, 0>;
+  if (w_smem > 48 * 1024 &&
+      cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024) != cudaSuccess)
+    return MSCNN_ERR_CUDA;
+  const size_t total = (size_t)N * Ho * Wo * cgs;
+  mscnn::note_launch();
+  kern<<<dim3(grid_for(total, 256), slices), 256, w_smem, (cudaStream_t)stream>>>(
+      (const __nv_bfloat16*)x_hi, (const __nv_bfloat16*)x_lo, w, bias, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, N,
+      H, W, C, Creal, Ho, Wo, cgs, q);
+  return launch_check("deconv_depthwise");
+}
+
 extern "C" int mscnn_deconv2x_forward(const void* x_hi, const void* x_lo, const float* w, void* y_hi,
                                       void* y_lo, int N, int H, int W, int C, int Creal, void* stream) {
-  if (!x_hi || !y_hi || !w || N <= 0 || H <= 0 || W <= 0 || C % 8 || Creal > C) return MSCNN_ERR_INVALID;
-  if ((x_lo == nullptr) != (y_lo == nullptr)) return MSCNN_ERR_INVALID;
-  const size_t total = (size_t)N * 2 * H * 2 * W * (C / 8);
-  mscnn::note_launch();
-  const size_t w_smem = (size_t)16 * C * sizeof(float);
-  if (w_smem > 200 * 1024) return MSCNN_ERR_INVALID;
-  if (w_smem > 48 * 1024 &&
-      cudaFuncSetAttribute(deconv2x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w_smem) != cudaSuccess)
-    return MSCNN_ERR_CUDA;
-  deconv2x_kernel<<<grid_for(total, 256), 256, w_smem, (cudaStream_t)stream>>>(
-      (const __nv_bfloat16*)x_hi, (const __nv_bfloat16*)x_lo, w, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo,
-      N, H, W, C, Creal);
-  return launch_check("deconv2x");
+  return mscnn_deconv_depthwise_forward(x_hi, x_lo, w, nullptr, y_hi, y_lo, N, H, W, C, Creal, 4, 4, 2, 2, 1, 1, 1, 1,
+                                        stream);
 }
 
 extern "C" int mscnn_relu_planes(void* hi, void* lo, size_t count, void* stream) {

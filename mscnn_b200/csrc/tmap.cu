@@ -28,11 +28,12 @@ static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
 }
 
 int tmap_nhwc_bf16(CUtensorMap* out, const void* base, const uint64_t dims[4],
-                   const uint32_t box[4], const uint32_t elem_strides[4]) {
+                   const uint32_t box[4], const uint32_t elem_strides[4], const uint64_t byte_strides[3]) {
   auto enc = get_encode();
   if (!enc) return MSCNN_ERR_CUDA;
   cuuint64_t gdim[4] = {dims[0], dims[1], dims[2], dims[3]};
   cuuint64_t gstride[3] = {dims[0] * 2, dims[0] * dims[1] * 2, dims[0] * dims[1] * dims[2] * 2};
+  for (int i = 0; byte_strides && i < 3; ++i) gstride[i] = byte_strides[i];
   cuuint32_t b[4] = {box[0], box[1], box[2], box[3]};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   for (int i = 0; elem_strides && i < 4; ++i) estr[i] = elem_strides[i];
@@ -42,10 +43,11 @@ int tmap_nhwc_bf16(CUtensorMap* out, const void* base, const uint64_t dims[4],
   if (r != CUDA_SUCCESS) {
     fprintf(stderr,
             "mscnn: cuTensorMapEncodeTiled(4d) failed rc=%d dims={%llu,%llu,%llu,%llu} "
-            "box={%u,%u,%u,%u} strides={%u,%u,%u,%u} base=%p\n",
+            "box={%u,%u,%u,%u} strides={%u,%u,%u,%u} byte strides={%llu,%llu,%llu} base=%p\n",
             (int)r, (unsigned long long)dims[0], (unsigned long long)dims[1],
             (unsigned long long)dims[2], (unsigned long long)dims[3], box[0], box[1], box[2],
-            box[3], estr[0], estr[1], estr[2], estr[3], base);
+            box[3], estr[0], estr[1], estr[2], estr[3], (unsigned long long)gstride[0],
+            (unsigned long long)gstride[1], (unsigned long long)gstride[2], base);
     return MSCNN_ERR_CUDA;
   }
   return MSCNN_OK;

@@ -230,6 +230,101 @@ def deconv2x_forward(x: Planes, w: torch.Tensor) -> Planes:
     return Planes(y_hi, y_lo, x.channels)
 
 
+def deconv_out_size(size: int, k: int, stride: int, pad: int, dilation: int = 1) -> int:
+    """DeconvolutionLayer::compute_output_shape (deconv_layer.cpp:8-22)."""
+    return stride * (size - 1) + dilation * (k - 1) + 1 - 2 * pad
+
+
+@dataclass
+class PackedDeconvWeights:
+    """Weights packed by output phase for mscnn_deconv_forward (mscnn_pack_deconv_weights)."""
+    hi: torch.Tensor          # [elems] bf16, the phases' sub-kernels one after another
+    lo: torch.Tensor | None
+    bias: torch.Tensor        # fp32 [Cout_pad]
+    cin: int
+    cout: int
+    cout_pad: int
+    kernel: tuple[int, int]
+    stride: tuple[int, int]
+    pad: tuple[int, int]
+    dilation: tuple[int, int]
+    group: int
+
+
+def pack_deconv_weights(w: torch.Tensor, b: torch.Tensor | None, split: bool, stride, pad, dilation=1,
+                        group: int = 1) -> PackedDeconvWeights:
+    """w: [Cin][Cout / group][KH][KW] fp32 (the Deconvolution layer's blob 0), b: [Cout] fp32 (blob 1) or None.
+    stride, pad, dilation: an int, or (h, w); the phase split depends on them, so they are fixed at packing."""
+    assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and w.dim() == 4
+    cin, cout_g, kh, kw = w.shape
+    cout = cout_g * group
+    cout_pad = pad64(cout)
+    (s_h, s_w), (p_h, p_w), (d_h, d_w) = _pair(stride), _pair(pad), _pair(dilation)
+    geom = (cin, cout, group, kh, kw, s_h, s_w, p_h, p_w, d_h, d_w, cout_pad)
+    elems = capi.lib().mscnn_deconv_packed_elems(*geom)
+    if elems < 0:
+        raise capi.MscnnError(f"deconvolution weights {tuple(w.shape)} stride {stride} pad {pad} dilation {dilation} "
+                              f"group {group}: geometry not served")
+    hi = torch.empty((elems,), dtype=torch.bfloat16, device=w.device)
+    lo = torch.empty_like(hi) if split else None
+    capi.check(capi.lib().mscnn_pack_deconv_weights(capi.ptr(w), capi.ptr(hi), capi.ptr(lo), cin, cout, group, kh, kw,
+                                                    s_h, s_w, p_h, p_w, d_h, d_w, cout_pad, _stream()),
+               "pack_deconv_weights")
+    bias = torch.zeros(cout_pad, dtype=torch.float32, device=w.device)
+    if b is not None:
+        bias[:cout] = b
+    return PackedDeconvWeights(hi, lo, bias, cin, cout, cout_pad, (kh, kw), (s_h, s_w), (p_h, p_w), (d_h, d_w), group)
+
+
+def deconv_desc(x: Planes, w: PackedDeconvWeights, relu: bool = False) -> capi.ConvDesc:
+    """The mscnn_deconv_forward descriptor of x through w, outputs unset."""
+    n, h, wd, c = x.hi.shape
+    d = capi.ConvDesc()
+    d.x_hi, d.x_lo = capi.ptr(x.hi), capi.ptr(x.lo)
+    d.N, d.H, d.W, d.C = n, h, wd, c
+    d.w_hi, d.w_lo, d.bias = capi.ptr(w.hi), capi.ptr(w.lo), capi.ptr(w.bias)
+    d.Cout, d.Cout_pad, (d.KH, d.KW), (d.pad_h, d.pad_w) = w.cout, w.cout_pad, w.kernel, w.pad
+    d.relu = int(relu)
+    d.out_mode = capi.OUT_NHWC_BF16
+    (d.stride_h, d.stride_w), (d.dil_h, d.dil_w), d.group = w.stride, w.dilation, w.group
+    return d
+
+
+def deconv_forward(x: Planes, w: PackedDeconvWeights, relu: bool = False, out: Planes | None = None) -> Planes:
+    """Deconvolution + bias (+ReLU) of planes through weights packed by pack_deconv_weights (whose kernel, stride, pad,
+    dilation and group it uses): planes [N][Ho][Wo][Cout_pad].  out: planes to write into instead of new ones."""
+    n, h, wd, c = x.hi.shape
+    assert c == pad64(w.cin), (x.hi.shape, w.cin)
+    ho = deconv_out_size(h, w.kernel[0], w.stride[0], w.pad[0], w.dilation[0])
+    wo = deconv_out_size(wd, w.kernel[1], w.stride[1], w.pad[1], w.dilation[1])
+    if out is None:
+        y_hi = torch.empty((n, max(ho, 0), max(wo, 0), w.cout_pad), dtype=torch.bfloat16, device=x.hi.device)
+        out = Planes(y_hi, torch.empty_like(y_hi) if x.lo is not None else None, w.cout)
+    assert out.shape == (n, ho, wo, w.cout_pad)
+    d = deconv_desc(x, w, relu)
+    d.y_hi, d.y_lo = capi.ptr(out.hi), capi.ptr(out.lo)
+    capi.check(capi.lib().mscnn_deconv_forward(d, _stream()), "deconv_forward")
+    return out
+
+
+def deconv_depthwise_forward(x: Planes, w: torch.Tensor, b: torch.Tensor | None, stride, pad, dilation=1) -> Planes:
+    """Depthwise deconvolution (group == channels == num_output): w fp32 [C][1][KH][KW] (blob 0), b fp32 [C] or None.
+    kernel from w; stride, pad, dilation: an int, or (h, w)."""
+    n, h, wd, c = x.hi.shape
+    assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and w.dim() == 4 and w.shape[1] == 1
+    assert b is None or (b.is_cuda and b.dtype == torch.float32 and b.is_contiguous() and b.numel() == w.shape[0])
+    kh, kw = w.shape[2:]
+    (s_h, s_w), (p_h, p_w), (d_h, d_w) = _pair(stride), _pair(pad), _pair(dilation)
+    ho, wo = deconv_out_size(h, kh, s_h, p_h, d_h), deconv_out_size(wd, kw, s_w, p_w, d_w)
+    y_hi = torch.empty((n, max(ho, 0), max(wo, 0), c), dtype=torch.bfloat16, device=x.hi.device)
+    y_lo = torch.empty_like(y_hi) if x.lo is not None else None
+    capi.check(capi.lib().mscnn_deconv_depthwise_forward(capi.ptr(x.hi), capi.ptr(x.lo), capi.ptr(w), capi.ptr(b),
+                                                         capi.ptr(y_hi), capi.ptr(y_lo), n, h, wd, c, w.shape[0], kh,
+                                                         kw, s_h, s_w, p_h, p_w, d_h, d_w, _stream()),
+               "deconv_depthwise_forward")
+    return Planes(y_hi, y_lo, x.channels)
+
+
 def make_box_cfg(maps_shapes, field_w, field_h, rate, fg_thr, iou_thr, nms_type="IOU", field_whr=2.0,
                  field_xyr=2.0, min_size=15.0, max_nms_num=2000, max_post_nms_num=0, bbox_mean=None,
                  bbox_std=None) -> capi.BoxOutputCfg:

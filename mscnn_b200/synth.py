@@ -18,7 +18,8 @@ Weights  : per-layer numpy PCG64 stream seeded with 1706 + crc32(layer name):
     (tools/calibrate_synth.py) so that ~3/4 of the anchors pass fg_thr = -5, the top-2000 cap is
     hit, and the dx/dy/dw/dh clamps (box_output_layer.cpp:145-151) trigger on a few percent.
   * cls_pred* / bbox_pred* (every cascade stage): N(0, target/sqrt(K * M2_FC)), bias 0.
-  * Deconvolution (conv4_3_2x): the exact BilinearFiller weights (include/caffe/filler.hpp:248-258).
+  * Deconvolution with a square kernel (conv4_3_2x): the exact BilinearFiller weights (include/caffe/filler.hpp:248-258),
+    zero bias with bias_term; a rectangular kernel takes the MSRA rule of the trunk.
 """
 from __future__ import annotations
 
@@ -67,10 +68,10 @@ def make_weights(layers: list[tuple[str, str, list[tuple[int, ...]]]]) -> dict[s
         wshape = tuple(shapes[0])
         fan_in = int(np.prod(wshape[1:]))
         blobs: list[np.ndarray]
-        if ltype == "Deconvolution":
+        if ltype == "Deconvolution" and wshape[-1] == wshape[-2]:
             k = wshape[-1]
             w = np.broadcast_to(bilinear_kernel(k), wshape).astype(np.float32).copy()
-            blobs = [w]
+            blobs = [w] + [np.zeros(s, dtype=np.float32) for s in shapes[1:]]   # bias_term: zero bias
         elif ltype == "Convolution" and name.startswith("LFCN"):
             cout = wshape[0]
             cls = cout - 4
@@ -84,10 +85,10 @@ def make_weights(layers: list[tuple[str, str, list[tuple[int, ...]]]]) -> dict[s
             std = PRED_CLS_STD if name.startswith("cls_pred") else PRED_BOX_STD
             w = (rng.standard_normal(wshape) * (std / np.sqrt(fan_in * M2_FC))).astype(np.float32)
             blobs = [w, np.zeros(wshape[0], dtype=np.float32)]
-        else:  # MSRA
+        else:  # MSRA (a Deconvolution with a non-square kernel too; its bias blob is [Cout], not wshape[0])
             w = (rng.standard_normal(wshape) * np.sqrt(2.0 / fan_in)).astype(np.float32)
             if ltype == "Convolution" and wshape[1] == 3:
                 w *= np.float32(FIRST_CONV_GAIN)
-            blobs = [w, np.zeros(wshape[0], dtype=np.float32)]
+            blobs = [w, np.zeros(shapes[1] if len(shapes) > 1 else wshape[0], dtype=np.float32)]
         out[name] = blobs[: len(shapes)]
     return out
