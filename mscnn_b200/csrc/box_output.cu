@@ -12,7 +12,8 @@
 //   * ranking is std::sort with std::greater<pair<score,idx>> (box_output_layer.cpp:168): score
 //     descending, ties broken by the LARGER candidate index.  Candidate indices grow with the
 //     anchor scan order (scale j, then row-major position), so the 64-bit key
-//     (orderable(score) << 32 | anchor_index) sorted descending gives the same permutation;
+//     (orderable(score) << 32 | anchor_index) sorted descending gives the same permutation
+//     (-0 and +0 compare equal there, so they share one key: score_key);
 //   * NMS is nmsMax(greedy) over the top max_nms_num boxes of an image, all scales together
 //     (box_output_layer.cpp:38-63,176-182), IoU by BoxIOU (util/math_functions.cpp:13-35) with
 //     the strict `>` test.
@@ -48,6 +49,11 @@ __device__ __forceinline__ uint32_t float_orderable(float f) {
   const uint32_t u = __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
+// The sort key of a score.  -0.0f and +0.0f get one key: fg + 0.0f is +0.0f for both (round to nearest), so a run of
+// zero scores is ranked by the index word alone, as std::greater<pair<float,int>> (BoxOutput) and MATLAB's stable
+// sort (final detections) rank it, where the raw bits would put every +0 above every -0.  The score written back from
+// the key is therefore +0.0f for a zero score of either sign.
+__device__ __forceinline__ uint32_t score_key(float f) { return float_orderable(f + 0.0f); }
 __device__ __forceinline__ float orderable_float(uint32_t o) {
   const uint32_t u = (o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o;
   return __uint_as_float(u);
@@ -101,7 +107,7 @@ __global__ void box_decode_kernel(const DecodeParams p, int N, unsigned long lon
     bw = (rw < bw) ? rw : bw;  // std::min(bbw, img_width - bbx)
     bh = (rh < bh) ? rh : bh;
     if (bw >= p.min_size && bh >= p.min_size) {
-      key = ((unsigned long long)float_orderable(fg) << 32) | (unsigned int)a;
+      key = ((unsigned long long)score_key(fg) << 32) | (unsigned int)a;
       boxes[(size_t)n * p.anchors_per_image + a] = make_float4(bx, by, bw, bh);
     }
   }
@@ -481,7 +487,7 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
       if (prob != prob) continue;  // bbNms: kp = bbs(:,5) > -inf drops NaN
       if (prob < p.det_thr) continue;  // widerface/run_cascademscnn.m:130-131
       dboxes[(size_t)s * Kpad + i] = make_float4(x1, y1, w, h);
-      sk[i] = ((unsigned long long)float_orderable(prob) << 32) | (unsigned int)(0xFFFFFFFFu - (unsigned)i);
+      sk[i] = ((unsigned long long)score_key(prob) << 32) | (unsigned int)(0xFFFFFFFFu - (unsigned)i);
       atomicAdd(&s_valid, 1);
       continue;
     }
@@ -510,7 +516,7 @@ detect_decode_sort_kernel(const DetectParams p, const DetectGeom geom, const flo
     if (prob != prob) continue;  // bbNms: kp = bbs(:,5) > -inf drops NaN
     if (prob < p.det_thr) continue;  // widerface/run_mscnn_detection.m:139-143
     dboxes[(size_t)s * Kpad + i] = make_float4(tx, ty, tw, th);
-    sk[i] = ((unsigned long long)float_orderable(prob) << 32) | (unsigned int)(0xFFFFFFFFu - (unsigned)i);
+    sk[i] = ((unsigned long long)score_key(prob) << 32) | (unsigned int)(0xFFFFFFFFu - (unsigned)i);
     atomicAdd(&s_valid, 1);
   }
   __syncthreads();
