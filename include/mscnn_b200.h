@@ -63,6 +63,9 @@ MSCNN_API const char* mscnn_version(void);
 MSCNN_API int mscnn_sm_count(void);
 /* Number of CUDA kernels this library has launched in this process so far (all entry points). */
 MSCNN_API unsigned long long mscnn_kernel_launch_count(void);
+/* Number of packed weight images this process has (re-)packed so far: nets that share their weights
+ * (mscnn_net_share_trained_layers) pack each image once between them. */
+MSCNN_API unsigned long long mscnn_weight_pack_count(void);
 /* The MSCNN_* environment switches (DESIGN.md 4.1c) are read once, not per launch.  This re-reads them and drops the
  * cached convolution launch plans; mscnn_net_create calls it.  The reference reads its switches (Caffe::mode, cuDNN
  * engine choice) at layer set-up too (src/caffe/layer_factory.cpp:37-65). */
@@ -554,6 +557,15 @@ MSCNN_API int mscnn_net_param_shape(void* net, const char* layer, int idx, int* 
 MSCNN_API int mscnn_net_set_param(void* net, const char* layer, int idx, const float* host, long count);
 MSCNN_API int mscnn_net_get_param(void* net, const char* layer, int idx, float* host, long count);
 MSCNN_API int mscnn_net_copy_trained(void* net, const char* caffemodel_path); /* Net::CopyTrainedLayersFrom */
+/* Net::ShareTrainedLayersWith (net.cpp:682-712, pycaffe's share_with): every parameter blob of `net` whose layer name
+ * `other` also has shares `other`'s storage (ShareData); layers `net` lacks are ignored.  Afterwards a write through
+ * either net is seen by both, and both read one packed image of each weight, so the second net allocates no weight
+ * memory.  The nets may then run forwards concurrently from different host threads, each on its own stream; write
+ * parameters only while no forward of a sharing net is in flight.  MSCNN_ERR_INVALID, with the reference's message
+ * on stderr and nothing shared, when a layer's blob count or a blob's shape differs, or the nets were created on
+ * different devices. */
+MSCNN_API int mscnn_net_share_trained_layers(void* net, const void* other);
+MSCNN_API int mscnn_net_device(void* net);   /* the device current when the net was created (-1: none) */
 MSCNN_API int mscnn_net_num_blobs(void* net);
 MSCNN_API const char* mscnn_net_blob_name(void* net, int i);
 MSCNN_API int mscnn_net_num_inputs(void* net);

@@ -1,5 +1,6 @@
 // Implementation of the Caffe-API mirror's core types: Caffe context, SyncedMemory, Blob.
 // Semantics follow /root/reference/src/caffe/{common,syncedmem,blob}.cpp; citations inline.
+#include <algorithm>
 #include <cstring>
 
 #include "caffe/blob.hpp"
@@ -13,8 +14,13 @@ namespace caffe {
 // ------------------------------------------------------------------------------- Caffe
 Caffe& Caffe::Get() {
   // one context per thread, like boost::thread_specific_ptr<Caffe> in common.cpp:13-22
-  static thread_local Caffe* instance = new Caffe();
+  // (a host thread per net, started and joined per call, must not leave its scratch behind)
+  static thread_local std::unique_ptr<Caffe> instance(new Caffe());
   return *instance;
+}
+
+Caffe::~Caffe() {
+  if (scratch_) cudaFree(scratch_);  // not checked: at process exit the runtime may already be gone
 }
 
 Caffe::Caffe() : mode_(Caffe::GPU), precision_(Caffe::FP32_SPLIT), stream_(0), scratch_(nullptr), scratch_bytes_(0) {
@@ -66,9 +72,28 @@ static void host_free(void* p) {
   else free(p);
 }
 
+static std::atomic<unsigned long> g_storage_clock{0};
+unsigned long next_storage_version() { return g_storage_clock.fetch_add(1, std::memory_order_relaxed) + 1; }
+
 SyncedMemory::~SyncedMemory() {
   if (cpu_ptr_ && own_cpu_data_) host_free(cpu_ptr_);
   if (gpu_ptr_ && own_gpu_data_) cudaFree(gpu_ptr_);
+  if (upload_) cudaEventDestroy(upload_);
+}
+
+inline void SyncedMemory::wait_upload() {
+  if (!upload_pending_) return;
+  const cudaStream_t s = Caffe::stream();
+  if (s == upload_stream_ || std::find(upload_waited_.begin(), upload_waited_.end(), s) != upload_waited_.end()) return;
+  CUDA_CHECK(cudaStreamWaitEvent(s, upload_, 0));
+  upload_waited_.push_back(s);
+}
+
+shared_ptr<PackedImage> SyncedMemory::packed_image(const std::string& key) {
+  std::lock_guard<std::mutex> lk(packed_mu_);
+  shared_ptr<PackedImage>& p = packed_[key];
+  if (!p) p.reset(new PackedImage());
+  return p;
 }
 
 inline void SyncedMemory::to_cpu() {  // syncedmem.cpp:25-49
@@ -84,6 +109,7 @@ inline void SyncedMemory::to_cpu() {  // syncedmem.cpp:25-49
         cpu_ptr_ = host_alloc(size_ ? size_ : 1);
         own_cpu_data_ = true;
       }
+      wait_upload();
       CUDA_CHECK(cudaMemcpyAsync(cpu_ptr_, gpu_ptr_, size_, cudaMemcpyDeviceToHost, Caffe::stream()));
       CUDA_CHECK(cudaStreamSynchronize(Caffe::stream()));
       head_ = SYNCED;
@@ -108,6 +134,18 @@ inline void SyncedMemory::to_gpu() {  // syncedmem.cpp:51-77
         own_gpu_data_ = true;
       }
       CUDA_CHECK(cudaMemcpyAsync(gpu_ptr_, cpu_ptr_, size_, cudaMemcpyHostToDevice, Caffe::stream()));
+      {
+        // another thread's stream may read these bytes next (storage shared between nets): mark where they land
+        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+        CUDA_CHECK(cudaStreamIsCapturing(Caffe::stream(), &cap));
+        if (cap == cudaStreamCaptureStatusNone) {
+          if (!upload_) CUDA_CHECK(cudaEventCreateWithFlags(&upload_, cudaEventDisableTiming));
+          CUDA_CHECK(cudaEventRecord(upload_, Caffe::stream()));
+          upload_stream_ = Caffe::stream();
+          upload_pending_ = true;
+          upload_waited_.clear();
+        }
+      }
       head_ = SYNCED;
       break;
     case HEAD_AT_GPU:
@@ -117,34 +155,43 @@ inline void SyncedMemory::to_gpu() {  // syncedmem.cpp:51-77
 }
 
 const void* SyncedMemory::cpu_data() {
+  std::lock_guard<std::mutex> lk(mu_);
   to_cpu();
   return (const void*)cpu_ptr_;
 }
 void SyncedMemory::set_cpu_data(void* data) {
   CHECK(data);
+  std::lock_guard<std::mutex> lk(mu_);
   if (own_cpu_data_) host_free(cpu_ptr_);
   cpu_ptr_ = data;
   head_ = HEAD_AT_CPU;
   own_cpu_data_ = false;
 }
 const void* SyncedMemory::gpu_data() {
+  std::lock_guard<std::mutex> lk(mu_);
   to_gpu();
+  wait_upload();
   return (const void*)gpu_ptr_;
 }
 void SyncedMemory::set_gpu_data(void* data) {
   CHECK(data);
+  std::lock_guard<std::mutex> lk(mu_);
   if (own_gpu_data_) cudaFree(gpu_ptr_);
   gpu_ptr_ = data;
   head_ = HEAD_AT_GPU;
   own_gpu_data_ = false;
+  upload_pending_ = false;
 }
 void* SyncedMemory::mutable_cpu_data() {
+  std::lock_guard<std::mutex> lk(mu_);
   to_cpu();
   head_ = HEAD_AT_CPU;
   return cpu_ptr_;
 }
 void* SyncedMemory::mutable_gpu_data() {
+  std::lock_guard<std::mutex> lk(mu_);
   to_gpu();
+  wait_upload();
   head_ = HEAD_AT_GPU;
   return gpu_ptr_;
 }
@@ -167,15 +214,19 @@ void PlaneStore::reserve(size_t bytes, bool need_lo) {
   }
 }
 
+PackedImage::~PackedImage() {
+  if (ready) cudaEventDestroy(ready);
+}
+
 // ---------------------------------------------------------------------------------- Blob
 template <typename Dtype>
 Blob<Dtype>::Blob(const int num, const int channels, const int height, const int width)
-    : count_(0), capacity_(0), layout_head_(HEAD_NCHW), planes_split_(false), version_(0) {
+    : count_(0), capacity_(0), layout_head_(HEAD_NCHW), planes_split_(false) {
   Reshape(num, channels, height, width);
 }
 template <typename Dtype>
 Blob<Dtype>::Blob(const vector<int>& shape)
-    : count_(0), capacity_(0), layout_head_(HEAD_NCHW), planes_split_(false), version_(0) {
+    : count_(0), capacity_(0), layout_head_(HEAD_NCHW), planes_split_(false) {
   Reshape(shape);
 }
 
@@ -265,7 +316,7 @@ void Blob<Dtype>::set_cpu_data(Dtype* data) {
   CHECK(data);
   data_->set_cpu_data(data);
   layout_head_ = HEAD_NCHW;
-  ++version_;
+  bump_version();
 }
 template <typename Dtype>
 const Dtype* Blob<Dtype>::gpu_data() {
@@ -278,7 +329,7 @@ Dtype* Blob<Dtype>::mutable_cpu_data() {
   CHECK(data_);
   sync_to_nchw();
   layout_head_ = HEAD_NCHW;
-  ++version_;
+  bump_version();
   return static_cast<Dtype*>(data_->mutable_cpu_data());
 }
 template <typename Dtype>
@@ -286,7 +337,7 @@ Dtype* Blob<Dtype>::mutable_gpu_data() {
   CHECK(data_);
   sync_to_nchw();
   layout_head_ = HEAD_NCHW;
-  ++version_;
+  bump_version();
   return static_cast<Dtype*>(data_->mutable_gpu_data());
 }
 
@@ -326,7 +377,7 @@ typename Blob<Dtype>::Planes Blob<Dtype>::mutable_planes(bool split) {
   planes_->reserve(bytes ? bytes : 2, split);
   planes_split_ = split;
   layout_head_ = HEAD_PLANES;
-  ++version_;
+  bump_version();
   Planes p;
   p.hi = planes_->hi;
   p.lo = split ? planes_->lo : nullptr;
@@ -341,7 +392,8 @@ void Blob<Dtype>::ShareData(const Blob& other) {  // blob.cpp:149-153
   planes_ = other.planes_;
   layout_head_ = other.layout_head_;
   planes_split_ = other.planes_split_;
-  ++version_;
+  // the version now is the shared storage's (a value this blob never had: the clock never repeats), so every cache
+  // keyed on it, packed weights and CUDA graphs included, sees the change without a write
 }
 
 template <typename Dtype>

@@ -9,8 +9,17 @@
 // demand (mscnn_planes_to_nchw_f32), planes() converts from NCHW on demand
 // (mscnn_nchw_f32_to_planes), so user code that inspects any blob by name sees ordinary Caffe
 // data while layers hand planes to each other with no conversion.
+//
+// Versions follow the storage.  version() is the counter of the SyncedMemory holding the NCHW bytes, not of the Blob:
+// blobs that ShareData (within a net by ParamSpec name, or across nets by Net::ShareTrainedLayersWith) read one
+// counter, so a write through any of them (mutable_cpu_data / mutable_gpu_data / mutable_planes / set_cpu_data, and
+// so CopyTrainedLayersFrom and mscnn_net_set_param) is seen by every layer that caches something derived from the
+// data.  Values come from one process-wide clock and never repeat, so ShareData itself changes the version a blob
+// reports.  The packed weight images live next to that counter (packed_image), one per packing key, so layers whose
+// weight blobs share storage pack once and read one image.
 #pragma once
 #include <algorithm>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -32,10 +41,22 @@ struct CAFFE_API PlaneStore {
   void reserve(size_t bytes, bool need_lo);
 };
 
+// A packed device image of a parameter blob's bytes (the weights a Convolution / InnerProduct / Deconvolution kernel
+// reads), kept with the storage (SyncedMemory::packed_image).  A layer that finds it stale re-packs it under `mu` on
+// its own stream and records `ready` there; a layer on another stream that finds it current waits for `ready` on the
+// device before its first launch that reads this version.  No host thread waits for the device.
+struct CAFFE_API PackedImage {
+  std::mutex mu;
+  PlaneStore w;                      // bf16 hi (+ lo on the fp32-faithful path)
+  unsigned long version = ~0ul;      // the storage version it holds (~0: never packed)
+  cudaEvent_t ready = nullptr;       // recorded after the last pack, on the stream that ran it
+  ~PackedImage();
+};
+
 template <typename Dtype>
 class CAFFE_API Blob {
  public:
-  Blob() : data_(), count_(0), capacity_(0), layout_head_(HEAD_NCHW), planes_split_(false), version_(0) {}
+  Blob() : data_(), count_(0), capacity_(0), layout_head_(HEAD_NCHW), planes_split_(false) {}
   explicit Blob(const int num, const int channels, const int height, const int width);
   explicit Blob(const vector<int>& shape);
 
@@ -110,13 +131,22 @@ class CAFFE_API Blob {
   // Storage for a producer to fill: sets the head to planes and invalidates the NCHW copy.
   Planes mutable_planes(bool split);
   bool head_is_planes() const { return layout_head_ == HEAD_PLANES; }
-  // Bumped by every mutable_* accessor; layers use it to re-pack cached weights lazily.
-  unsigned long version() const { return version_; }
+  // The storage's version (see the file comment): changed by every mutable_* accessor and by ShareData; layers use it
+  // to re-pack cached weights lazily.
+  unsigned long version() const { return data_ ? data_->version() : 0; }
+  // The packed image of this blob's storage under `key` (see PackedImage); the blob must have storage.
+  shared_ptr<PackedImage> packed_image(const std::string& key) {
+    CHECK(data_);
+    return data_->packed_image(key);
+  }
 
  protected:
   enum LayoutHead { HEAD_NCHW, HEAD_PLANES, HEAD_BOTH };
   void planes_dims(int* n, int* c, int* h, int* w) const;
   void sync_to_nchw();
+  void bump_version() {
+    if (data_) data_->bump_version();
+  }
   shared_ptr<SyncedMemory> data_;
   shared_ptr<PlaneStore> planes_;
   vector<int> shape_;
@@ -124,7 +154,6 @@ class CAFFE_API Blob {
   int capacity_;
   LayoutHead layout_head_;
   bool planes_split_;
-  unsigned long version_;
   DISABLE_COPY_AND_ASSIGN(Blob);
 };
 

@@ -73,7 +73,8 @@ class CAFFE_API Caffe {
  public:
   enum Brew { CPU, GPU };
   enum Precision { FP32_SPLIT, BF16 };
-  static Caffe& Get();  // thread-local, like common.cpp:13-22
+  static Caffe& Get();  // thread-local, like common.cpp:13-22; freed when its thread ends
+  ~Caffe();
   inline static Brew mode() { return Get().mode_; }
   inline static void set_mode(Brew mode) { Get().mode_ = mode; }
   inline static Precision precision() { return Get().precision_; }

@@ -30,14 +30,18 @@ struct PackedBias {
 };
 struct PackedParam {
   enum Route { CONV, HEAD, CONV1_1, FC, DECONV };
-  // what `w` holds: the route that packed it, its padding and (fc) the bottom's C, H, W
-  struct Layout { int route, split, out_pad, in_pad, c, h, w; };
-  PlaneStore w;  // bf16 hi (+ lo when layout.split)
+  // how the image was packed: the route, the precision (split), its padding, (fc) the bottom's C, H, W and (deconv)
+  // the stride, pad and dilation per axis.  With the blob's storage it names one image (Blob::packed_image).
+  struct Layout { int route, split, out_pad, in_pad, c, h, w, geom[6]; };
+  shared_ptr<PackedImage> img;  // the image the kernels read; it lives with the weight blob's storage
   Layout layout = {-1};
-  unsigned long w_version = ~0ul;
+  unsigned long w_version = ~0ul;  // the storage version img held when this layer last made its stream wait for it
   PackedBias bias, gather_bias;  // [layout.out_pad] for the kernel; k x k heads: [Cout] for the tap gather
-  // re-packs with pack(w_f32, hi, lo) when wb's version or the layout changed; lo = NULL unless l.split
+  // Makes img the image of wb's storage under l, current for wb's version: packs it with pack(w_f32, hi, lo) on this
+  // thread's stream when stale (lo = NULL unless l.split), else orders this stream after its last pack.
   template <typename Pack> void update_weights(Blob<float>* wb, const Layout& l, size_t bytes, Pack pack);
+  void* hi() const { return img->w.hi; }
+  void* lo() const { return layout.split ? img->w.lo : nullptr; }
 };
 
 /// InputLayer: /root/reference/src/caffe/layers/input_layer.cpp:8-22

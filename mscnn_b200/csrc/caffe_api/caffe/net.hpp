@@ -48,6 +48,15 @@ class CAFFE_API Net {
   void CopyTrainedLayersFrom(const NetParameter& param);
   // Binary .caffemodel (NetParameter wire format, net.cpp:787-803).
   void CopyTrainedLayersFrom(const string trained_filename);
+  // Share other's trained parameters by layer name (net.cpp:682-712): each parameter blob of a layer other also has
+  // ShareData's other's blob; layers this net lacks are ignored.  Blob counts and shapes must match.  The storage
+  // carries the version and the packed weight images (blob.hpp), so both nets see every write and pack each image
+  // once.  Both nets must live on one device (mscnn_b200: the reference has no multi-device case).
+  void ShareTrainedLayersWith(const Net* other);
+  // mscnn_b200 extension: the message ShareTrainedLayersWith(other) would abort with, or "" when it would succeed.
+  string ShareTrainedLayersError(const Net* other) const;
+  // mscnn_b200 extension: the device current when the net was built (-1: none), where its storage lives
+  int device() const { return device_; }
 
   inline const string& name() const { return name_; }
   inline const vector<string>& layer_names() const { return layer_names_; }
@@ -130,6 +139,7 @@ class CAFFE_API Net {
   vector<int> dyn_layers_;      // layers whose row count derives from it, in execution order
   set<string> dyn_blob_names_;  // blobs whose row count derives from it
   bool lazy_rows_ = false;
+  int device_ = -1;
   bool graph_mode_ = false, graph_replayed_ = false;
   struct GraphState;
   shared_ptr<GraphState> graph_;

@@ -7,6 +7,7 @@
 #include "caffe/layers/mscnn_layers.hpp"
 #include "config.h"
 #include "deconv_phase.h"
+#include "launch_count.h"
 
 namespace caffe {
 
@@ -30,11 +31,27 @@ void PackedBias::update(Blob<float>* b, int n, int n_pad) {
 }
 template <typename Pack>
 void PackedParam::update_weights(Blob<float>* wb, const Layout& l, size_t bytes, Pack pack) {
-  if (w_version == wb->version() && memcmp(&layout, &l, sizeof(l)) == 0) return;
-  w.reserve(bytes, l.split);
-  pack(wb->gpu_data(), w.hi, l.split ? w.lo : nullptr);
-  w_version = wb->version();
+  const unsigned long ver = wb->version();
+  if (img && w_version == ver && memcmp(&layout, &l, sizeof(l)) == 0) return;
+  shared_ptr<PackedImage> im = wb->packed_image(std::string(reinterpret_cast<const char*>(&l), sizeof(l)));
+  const cudaStream_t s = Caffe::stream();
+  {
+    std::lock_guard<std::mutex> lk(im->mu);  // one thread packs a given version
+    if (im->version != ver) {
+      im->w.reserve(bytes, l.split);
+      pack(wb->gpu_data(), im->w.hi, l.split ? im->w.lo : nullptr);
+      if (!im->ready) CUDA_CHECK(cudaEventCreateWithFlags(&im->ready, cudaEventDisableTiming));
+      CUDA_CHECK(cudaEventRecord(im->ready, s));
+      im->version = ver;
+      mscnn::g_weight_packs.fetch_add(1, std::memory_order_relaxed);
+    } else {
+      // packed by a layer that shares the storage, maybe on another thread's stream
+      CUDA_CHECK(cudaStreamWaitEvent(s, im->ready, 0));
+    }
+  }
+  img = im;
   layout = l;
+  w_version = ver;
 }
 
 // The mscnn_conv_desc fields every route through mscnn_conv_forward shares; the caller sets out_mode, the outputs,
@@ -45,7 +62,7 @@ static mscnn_conv_desc conv_desc(const Blob<float>::Planes& x, const PackedParam
   memset(&d, 0, sizeof(d));
   d.x_hi = x.hi; d.x_lo = x.lo;
   d.N = N; d.H = H; d.W = W; d.C = C;
-  d.w_hi = pk.w.hi; d.w_lo = pk.layout.split ? pk.w.lo : nullptr;
+  d.w_hi = pk.hi(); d.w_lo = pk.lo();
   d.bias = pk.bias.data;
   d.Cout = cout; d.Cout_pad = pk.layout.out_pad;
   d.KH = kh; d.KW = kw;
@@ -219,7 +236,7 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
     });
     packed_.bias.update(bias, 64, 64);
     typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
-    MSCNN_CHECK(mscnn_conv1_tc_forward(bottom[0]->gpu_data(), packed_.w.hi, packed_.bias.data, y.hi,
+    MSCNN_CHECK(mscnn_conv1_tc_forward(bottom[0]->gpu_data(), packed_.hi(), packed_.bias.data, y.hi,
                                        split ? y.lo : nullptr, N, H, W, fuse_relu_ ? 1 : 0, Caffe::stream()));
     return;
   }
@@ -334,7 +351,8 @@ void DeconvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, 
   const long long elems = mscnn_deconv_packed_elems(channels_, num_output_, group_, kernel_h_, kernel_w_, stride_h_,
                                                     stride_w_, pad_h_, pad_w_, dilation_h_, dilation_w_, cout_pad);
   CHECK_GE(elems, 0);
-  packed_.update_weights(wb, {PackedParam::DECONV, split, cout_pad, cin_pad, 0, 0, 0}, (size_t)elems * 2,
+  packed_.update_weights(wb, {PackedParam::DECONV, split, cout_pad, cin_pad, 0, 0, 0,
+                              {stride_h_, stride_w_, pad_h_, pad_w_, dilation_h_, dilation_w_}}, (size_t)elems * 2,
                          [&](const float* w, void* hi, void* lo) {
     MSCNN_CHECK(mscnn_pack_deconv_weights(w, hi, lo, channels_, num_output_, group_, kernel_h_, kernel_w_, stride_h_,
                                           stride_w_, pad_h_, pad_w_, dilation_h_, dilation_w_, cout_pad,

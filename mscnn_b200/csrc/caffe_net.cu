@@ -1,6 +1,7 @@
 // caffe::Net for the forward path: graph construction (net.cpp:49-284), split insertion
 // (util/insert_splits.cpp:13-138), execution (net.cpp:544-555), weight loading by layer name
 // (net.cpp:750-803 incl. a protobuf wire-format reader for .caffemodel files).
+#include <algorithm>
 #include <cstdio>
 #include <cstring>
 #include <fstream>
@@ -99,6 +100,10 @@ Net<Dtype>::Net(const string& param_file, Phase phase) : time_layers_(false) {
 template <typename Dtype>
 void Net<Dtype>::Init(const NetParameter& in_param) {
   phase_ = in_param.state().phase();
+  if (cudaGetDevice(&device_) != cudaSuccess) {  // no device: host-only inspection (caffe_api.cu SyncedMemory)
+    cudaGetLastError();
+    device_ = -1;
+  }
   NetParameter upgraded;
   upgraded.CopyFrom(in_param);
   proto_text::UpgradeNetInput(&upgraded);  // UpgradeNetAsNeeded: legacy input fields only
@@ -526,6 +531,50 @@ void Net<Dtype>::CopyTrainedLayersFrom(const NetParameter& param) {
       }
       target_blobs[j]->FromProto(source_layer.blobs((int)j), false);
     }
+  }
+}
+
+// A source layer matches the first layer of this net with its name (the reference's linear search).
+template <typename Dtype>
+string Net<Dtype>::ShareTrainedLayersError(const Net* other) const {
+  std::ostringstream msg;
+  if (other->device_ != device_) {
+    msg << "Cannot share trained layers between nets on different devices (" << other->device_ << " and " << device_
+        << ")";
+    return msg.str();
+  }
+  for (size_t i = 0; i < other->layers().size(); ++i) {
+    const string& name = other->layer_names()[i];
+    const size_t t = std::find(layer_names_.begin(), layer_names_.end(), name) - layer_names_.begin();
+    if (t == layer_names_.size()) continue;
+    const vector<shared_ptr<Blob<Dtype> > >& source_blobs = other->layers()[i]->blobs();
+    const vector<shared_ptr<Blob<Dtype> > >& target_blobs = layers_[t]->blobs();
+    if (target_blobs.size() != source_blobs.size()) {
+      msg << "Incompatible number of blobs for layer " << name << " (" << target_blobs.size() << " vs. "
+          << source_blobs.size() << ")";
+      return msg.str();
+    }
+    for (size_t j = 0; j < target_blobs.size(); ++j)
+      if (target_blobs[j]->shape() != source_blobs[j]->shape()) {
+        msg << "Cannot share param " << j << " weights from layer '" << name
+            << "'; shape mismatch.  Source param shape is " << source_blobs[j]->shape_string()
+            << "; target param shape is " << target_blobs[j]->shape_string();
+        return msg.str();
+      }
+  }
+  return string();
+}
+
+template <typename Dtype>
+void Net<Dtype>::ShareTrainedLayersWith(const Net* other) {
+  const string err = ShareTrainedLayersError(other);
+  if (!err.empty()) LOG(FATAL) << err;
+  for (size_t i = 0; i < other->layers().size(); ++i) {
+    const string& name = other->layer_names()[i];
+    const size_t t = std::find(layer_names_.begin(), layer_names_.end(), name) - layer_names_.begin();
+    if (t == layer_names_.size()) continue;  // "Ignoring source layer"
+    vector<shared_ptr<Blob<Dtype> > >& target_blobs = layers_[t]->blobs();
+    for (size_t j = 0; j < target_blobs.size(); ++j) target_blobs[j]->ShareData(*other->layers()[i]->blobs()[j]);
   }
 }
 

@@ -255,6 +255,20 @@ int mscnn_net_copy_trained(void* h, const char* caffemodel_path) {
   return MSCNN_OK;
 }
 
+int mscnn_net_share_trained_layers(void* h, const void* other) {
+  if (!h || !other) return MSCNN_ERR_INVALID;
+  const Net<float>* src = static_cast<const NetHandle*>(other)->net.get();
+  const std::string err = H(h)->net->ShareTrainedLayersError(src);
+  if (!err.empty()) {
+    fprintf(stderr, "mscnn_net_share_trained_layers: %s\n", err.c_str());
+    return MSCNN_ERR_INVALID;
+  }
+  H(h)->net->ShareTrainedLayersWith(src);
+  return MSCNN_OK;
+}
+
+int mscnn_net_device(void* h) { return H(h)->net->device(); }
+
 int mscnn_net_num_blobs(void* h) { return (int)H(h)->net->blob_names().size(); }
 const char* mscnn_net_blob_name(void* h, int i) { return H(h)->net->blob_names()[i].c_str(); }
 int mscnn_net_num_inputs(void* h) { return H(h)->net->num_inputs(); }

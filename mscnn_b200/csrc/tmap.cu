@@ -73,11 +73,16 @@ int tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t cols, uint64_t row
 }
 
 std::atomic<unsigned long long> g_kernel_launches{0};
+std::atomic<unsigned long long> g_weight_packs{0};
 
 }  // namespace mscnn
 
 extern "C" unsigned long long mscnn_kernel_launch_count(void) {
   return mscnn::g_kernel_launches.load(std::memory_order_relaxed);
+}
+
+extern "C" unsigned long long mscnn_weight_pack_count(void) {
+  return mscnn::g_weight_packs.load(std::memory_order_relaxed);
 }
 
 extern "C" int mscnn_sm_count(void) {

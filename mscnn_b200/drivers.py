@@ -7,9 +7,17 @@ writes the drivers' files.  Every image's detections are those of the drivers' o
 
     res = drivers.run(net, frames, drivers.KITTI_CAR)          # per image: [per class: [k][5] = x y w h prob]
     drivers.write_results("detections", drivers.KITTI_CAR, comp_id, res)   # detections/<comp_id>_car.txt
+
+Several nets (make_nets: one per device entry, the weights loaded once per device and shared by the nets on it) run
+the same frames with one host thread per net, each on its own stream; the result is the one-net result, bit for bit:
+
+    nets = drivers.make_nets(proto, weights, devices=[0, 0, 1, 1])
+    res = drivers.run(nets, frames, drivers.KITTI_CAR)
 """
 from __future__ import annotations
 
+import threading
+from contextlib import contextmanager
 from dataclasses import dataclass, field
 from pathlib import Path
 
@@ -111,16 +119,107 @@ SPECS = {"kitti_car": KITTI_CAR, "kitti_ped_cyc": KITTI_PED_CYC, "caltech": CALT
          "kitti_car_cascade": KITTI_CAR_CASCADE, "citypersons": CITYPERSONS}
 
 
-def run(net, frames, spec: DriverSpec, batch: int = 8, net_hw: tuple[int, int] | None = None, pre=None) -> list:
-    """Final detections of uint8 host frames ([h][w][3], or gray [h][w] / [h][w][1], any sizes) on `net` at the one
+def make_nets(proto: str, weights, devices=(0,)) -> list:
+    """One net.Net of `proto` per entry of `devices` (device ids, repeats allowed), for run / widerface.run over several
+    nets.  The first net on each device loads `weights` (a {layer: [blobs]} dict, as Net.set_params takes, or a
+    .caffemodel path); the others on that device share its weights (Net.share_trained_layers_with), so each device
+    holds one copy.  The calling thread's device is restored."""
+    import torch
+    from . import net as mnet
+    prev = torch.cuda.current_device()
+    owners: dict[int, object] = {}
+    nets = []
+    try:
+        for d in devices:
+            mnet.set_device(int(d))
+            n = mnet.Net(proto)
+            if d in owners:
+                n.share_trained_layers_with(owners[d])
+            else:
+                if isinstance(weights, dict):
+                    n.set_params(weights)
+                else:
+                    n.copy_from(weights)
+                owners[d] = n
+            nets.append(n)
+    finally:
+        mnet.set_device(prev)
+    return nets
+
+
+def serve_batches(nets, batches, serve) -> None:
+    """Hands `batches` out whole, in order, from one queue to one host thread per net: serve(net, take) runs on its net's
+    thread and calls take() for that thread's next batch, None once there are no more.  The first exception in a worker
+    stops the hand-out (take() then returns None everywhere); every thread is joined before it is re-raised here."""
+    if len({id(n) for n in nets}) != len(nets):
+        raise ValueError("each net may appear once: one net runs on one thread")
+    batches = iter(batches)
+    lock = threading.Lock()
+    failed: list[BaseException] = []
+
+    def take():
+        with lock:
+            return None if failed else next(batches, None)
+
+    def work(net):
+        try:
+            serve(net, take)
+        except BaseException as e:          # noqa: BLE001 -- handed to the caller
+            with lock:
+                failed.append(e)
+
+    threads = [threading.Thread(target=work, args=(n,), name=f"mscnn-net-{k}", daemon=True) for k, n in enumerate(nets)]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    if failed:
+        raise failed[0]
+
+
+@contextmanager
+def net_thread(net, precision: str):
+    """The calling (worker) thread set up for `net`: its device, `precision` and a stream of its own for the net and
+    torch.  On exit the stream is drained and the thread's net stream reset."""
+    import torch
+    from . import net as mnet
+    dev = net.device
+    torch.cuda.set_device(dev)
+    mnet.set_device(dev)
+    mnet.set_precision(precision)
+    stream = torch.cuda.Stream(device=dev)
+    mnet.set_stream(stream.cuda_stream)
+    try:
+        with torch.cuda.stream(stream):
+            yield stream
+    finally:
+        stream.synchronize()
+        mnet.set_stream(None)
+
+
+def _plans(pre, n):
+    """pre for run over n nets: None (each worker makes its own), or a list of one plan per net."""
+    if pre is None:
+        return [None] * n
+    if not isinstance(pre, (list, tuple)) or len(pre) != n:
+        raise ValueError("with several nets, pre is None or a list of one pre-processing plan per net")
+    return list(pre)
+
+
+def run(nets, frames, spec: DriverSpec, batch: int = 8, net_hw: tuple[int, int] | None = None, pre=None) -> list:
+    """Final detections of uint8 host frames ([h][w][3], or gray [h][w] / [h][w][1], any sizes) on `nets` at the one
     net size `net_hw` (default spec.net_hw), as the driver `spec` computes them.
 
     Returns, per image in input order, a list over spec.cls_ids of float32 [k][5] = x y w h prob in original-image
     coordinates, the kept rows in the post-process's order.  The frames run in batches of `batch` (the last one short);
     batch k + 1 is pre-processed on the net's copy stream while batch k's forward runs (Net.set_input_images_async), and
     batch k's post-process and readback follow that.  pre: an ops.Preprocess of this net size to reuse (it keeps the
-    resize tables of every original size it has seen)."""
-    import torch
+    resize tables of every original size it has seen).
+
+    nets: one net.Net, run on the calling thread and stream; or a list of nets (make_nets), each served by a host thread
+    of its own on its device, in this thread's precision, on a stream of its own.  The batches are handed out whole
+    in input order (serve_batches); the result is the one-net result, bit for bit.  pre is then None or one plan per
+    net."""
     from . import net as mnet, ops
     if batch < 1:
         raise ValueError(f"batch ({batch}) must be positive")
@@ -130,21 +229,44 @@ def run(net, frames, spec: DriverSpec, batch: int = 8, net_hw: tuple[int, int] |
     out: list = [None] * len(frames)
     if not frames:
         return out
-    net_h, net_w = net_hw or spec.net_hw
+    net_hw = tuple(net_hw or spec.net_hw)
     ops.image_sizes_channels(frames)                          # every frame checked before any work is issued
+    chunks = [list(range(k, min(k + batch, len(frames)))) for k in range(0, len(frames), batch)]
+    if not isinstance(nets, (list, tuple)):
+        todo = iter(chunks)
+        _serve_fixed(nets, lambda: next(todo, None), frames, spec, net_hw, pre, out)
+        return out
+    plans = dict(zip(map(id, nets), _plans(pre, len(nets))))
+    precision = mnet.get_precision()
+
+    def serve(net, take):
+        with net_thread(net, precision):
+            _serve_fixed(net, take, frames, spec, net_hw, plans[id(net)], out)
+
+    serve_batches(nets, chunks, serve)
+    return out
+
+
+def _serve_fixed(net, take, frames, spec: DriverSpec, net_hw, pre, out: list) -> None:
+    """run's loop on one net, in the calling thread: take() gives the next batch of frame indices (None: done), and
+    out[i] receives image i's detections."""
+    import torch
+    from . import net as mnet, ops
+    idx = take()
+    if idx is None:
+        return
     if pre is None:
-        pre = ops.Preprocess(tuple(frames[0].shape[:2]), (net_h, net_w))
-    elif tuple(pre.out_hw) != (net_h, net_w):
-        raise ValueError(f"pre-processing plan for {pre.out_hw}, net size {(net_h, net_w)}")
-    cfg, classes = spec.detect_cfg((net_h, net_w))
+        pre = ops.Preprocess(tuple(frames[0].shape[:2]), net_hw)
+    elif tuple(pre.out_hw) != net_hw:
+        raise ValueError(f"pre-processing plan for {pre.out_hw}, net size {net_hw}")
+    cfg, classes = spec.detect_cfg(net_hw)
     c = len(spec.cls_ids)
     data = net.inputs[0]
     stream = mnet._net_stream()
-    chunks = [list(range(k, min(k + batch, len(frames)))) for k in range(0, len(frames), batch)]
-    net.set_input_images(data, pre, [frames[i] for i in chunks[0]])
-    for k, idx in enumerate(chunks):
+    net.set_input_images(data, pre, [frames[i] for i in idx])
+    while idx is not None:
         net.forward_only()
-        nxt = chunks[k + 1] if k + 1 < len(chunks) else None
+        nxt = take()
         # the same batch shape: pre-process the next batch behind this forward's first layers; a short last batch
         # reshapes the input, which waits until this batch has been post-processed
         if nxt is not None and len(nxt) == len(idx):
@@ -165,7 +287,7 @@ def run(net, frames, spec: DriverSpec, batch: int = 8, net_hw: tuple[int, int] |
             out[i] = [d[j, s, :cnt[j, s]].copy() for s in range(c)]
         if nxt is not None and len(nxt) != len(idx):
             net.set_input_images(data, pre, [frames[i] for i in nxt])
-    return out
+        idx = nxt
 
 
 def write_results(out_dir, spec: DriverSpec, comp_id: str, results, first_index: int = 1,

@@ -13,6 +13,7 @@ No compute happens in Python; a missing native library raises.
 from __future__ import annotations
 
 import ctypes as C
+import threading
 from pathlib import Path
 
 import numpy as np
@@ -38,6 +39,10 @@ def _declare(L):
     L.mscnn_net_param_shape.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_int)]
     L.mscnn_net_set_param.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_void_p, C.c_long]
     L.mscnn_net_copy_trained.argtypes = [C.c_void_p, C.c_char_p]
+    L.mscnn_net_share_trained_layers.argtypes = [C.c_void_p, C.c_void_p]
+    L.mscnn_net_device.argtypes = [C.c_void_p]
+    L.mscnn_weight_pack_count.restype = C.c_ulonglong
+    L.mscnn_weight_pack_count.argtypes = []
     L.mscnn_net_get_param.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_void_p, C.c_long]
     L.mscnn_net_blob_shape.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_int)]
     L.mscnn_net_reshape_blob.argtypes = [C.c_void_p, C.c_char_p] + [C.c_int] * 4
@@ -85,27 +90,37 @@ def _declare(L):
     L._net_declared = True
 
 
+# Precision, stream and device belong to the calling host thread, as the library's Caffe context does
+# (caffe_api.cu Caffe::Get): a thread that never sets them runs on the default stream in the default precision.
 def set_precision(mode: str) -> None:
-    """'fp32' = 3-term split-bf16 (fp32-faithful, default); 'bf16' = single bf16 term."""
+    """'fp32' = 3-term split-bf16 (fp32-faithful, default); 'bf16' = single bf16 term.  For this thread."""
     L = capi.lib()
     _declare(L)
     capi.check(L.mscnn_set_precision(1 if mode.lower() == "bf16" else 0), "set_precision")
 
 
-_net_stream_ptr = None   # the stream the nets of this process run on (mscnn_set_stream); None = the default stream
+def get_precision() -> str:
+    """This thread's precision: 'fp32' or 'bf16'."""
+    L = capi.lib()
+    _declare(L)
+    return "bf16" if L.mscnn_get_precision() else "fp32"
+
+
+_local = threading.local()   # .stream_ptr: the stream this thread's nets run on (mscnn_set_stream); None = default
 
 
 def set_stream(stream_ptr: int | None) -> None:
-    global _net_stream_ptr
+    """The stream the nets run on in this thread."""
     L = capi.lib()
     _declare(L)
     capi.check(L.mscnn_set_stream(stream_ptr), "set_stream")
-    _net_stream_ptr = stream_ptr
+    _local.stream_ptr = stream_ptr
 
 
 def _net_stream():
     import torch
-    return torch.cuda.ExternalStream(_net_stream_ptr) if _net_stream_ptr else torch.cuda.default_stream()
+    ptr = getattr(_local, "stream_ptr", None)
+    return torch.cuda.ExternalStream(ptr) if ptr else torch.cuda.default_stream()
 
 
 def set_device(device: int) -> None:
@@ -177,6 +192,19 @@ class Net:
 
     def copy_from(self, caffemodel: str) -> None:
         capi.check(self._L.mscnn_net_copy_trained(self._h, str(caffemodel).encode()), "copy_trained")
+
+    def share_trained_layers_with(self, other: "Net") -> None:
+        """Net::ShareTrainedLayersWith (pycaffe's share_with): every parameter blob of a layer `other` also has shares
+        `other`'s storage, so a write through either net is seen by both, and both read one packed image of each
+        weight (this net then allocates no weight memory).  Both nets must be on one device; the two may then run
+        forwards at the same time from two host threads, each on its own stream (drivers.run over several nets).
+        Raises MscnnError on a blob count or shape mismatch or different devices, sharing nothing."""
+        capi.check(self._L.mscnn_net_share_trained_layers(self._h, other._h), "share_trained_layers")
+
+    @property
+    def device(self) -> int:
+        """The device that was current when the net was created: where its blobs live (-1: none)."""
+        return int(self._L.mscnn_net_device(self._h))
 
     # ---- blobs ---------------------------------------------------------------------------
     def blob_shape(self, name: str) -> tuple[int, ...]:

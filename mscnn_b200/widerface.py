@@ -5,6 +5,7 @@ as ordinary batches of one shape; the net's input shape changes only between bat
 those of the drivers' one-image-at-a-time loop, bit for bit.
 
     dets = widerface.run(net, frames, names)                 # {name: [k][5] = x y w h prob}, input order
+    dets = widerface.run(drivers.make_nets(proto, weights, [0, 0]), frames, names)     # the same, on two nets
     widerface.write_results("detections/<comp_id>/<event>", dets)
 """
 from __future__ import annotations
@@ -44,46 +45,74 @@ def plan_batches(org_hw, img_hw=(0, 0), max_size: int = MAX_SIZE, max_batch: int
     return batches
 
 
-def run(net, frames, names, cascade: bool = False, max_size: int = MAX_SIZE, max_batch: int = 8,
+def run(nets, frames, names, cascade: bool = False, max_size: int = MAX_SIZE, max_batch: int = 8,
         pixel_budget: int = PIXEL_BUDGET, plans: dict | None = None) -> dict[str, np.ndarray]:
-    """Final face detections of uint8 [h][w][3] host frames (any sizes) on `net`, a models.widerface net (or, with
-    cascade=True, a models.widerface_cascade net read at proposals_3rd / cls_prob_3rd_avg / output_bbox_3rd as
+    """Final face detections of uint8 [h][w][3] host frames (any sizes) on `nets`, models.widerface nets (or, with
+    cascade=True, models.widerface_cascade nets read at proposals_3rd / cls_prob_3rd_avg / output_bbox_3rd as
     run_cascademscnn.m:44-47 does), with the drivers' settings (net.widerface_detect_cfg).
 
     Returns {name: float32 [k][5] = x y w h prob} in input order: the kept rows of each image in the post-process's
     order, in original-image coordinates.  plans: a dict net size -> ops.Preprocess to reuse between calls (the plans
-    keep the resize tables of every original size they have seen); new plans are added to it."""
-    import torch
-    from . import net as mnet, ops
+    keep the resize tables of every original size they have seen); new plans are added to it.
+
+    nets: one net.Net, run on the calling thread and stream; or a list of nets (drivers.make_nets), each served by a
+    host thread of its own (drivers.serve_batches, drivers.net_thread) taking plan_batches' batches, largest first,
+    from one queue.  plans is then None or a list of one dict per net.  The result is the one-net result, bit for bit."""
+    from . import drivers, net as mnet, ops
     names = list(names)
     if len(names) != len(frames) or len(set(names)) != len(names):
         raise ValueError("one distinct name per frame is needed")
     hw = ops.image_sizes(frames)
-    plans = {} if plans is None else plans
-    data = net.inputs[0]
-    stream = mnet._net_stream()
     kept: list[np.ndarray | None] = [None] * len(frames)
-    for (rz_h, rz_w), idx in plan_batches(hw, max_size=max_size, max_batch=max_batch, pixel_budget=pixel_budget):
-        n = len(idx)
-        net.reshape_input(data, n, 3, rz_h, rz_w)
-        pre = plans.get((rz_h, rz_w))
-        if pre is None:
-            pre = plans[(rz_h, rz_w)] = ops.Preprocess(tuple(hw[idx[0]]), (rz_h, rz_w))
-        net.set_input_images(data, pre, [frames[i] for i in idx])
-        net.forward_only()
-        cfg, classes = mnet.widerface_detect_cfg(rz_h, rz_w)    # the original sizes come with the frames
-        with torch.cuda.stream(stream):
-            dets = torch.empty((n, 1, cfg.max_rois_per_image, 5), dtype=torch.float32, device="cuda")
-            counts = torch.empty((n, 1), dtype=torch.int32, device="cuda")
-            if cascade:
-                net.detect_cascade_classes(cfg, classes, dets.data_ptr(), counts.data_ptr(), stage="3rd",
-                                           cls_prob="cls_prob_3rd_avg")
-            else:
-                net.detect_classes(cfg, classes, dets.data_ptr(), counts.data_ptr())
-            d, c = dets.cpu().numpy(), counts.cpu().numpy()
-        for k, i in enumerate(idx):
-            kept[i] = d[k, 0, :c[k, 0]].copy()
+    batches = plan_batches(hw, max_size=max_size, max_batch=max_batch, pixel_budget=pixel_budget)
+    if not isinstance(nets, (list, tuple)):
+        plans = {} if plans is None else plans
+        for b in batches:
+            _run_batch(nets, frames, hw, b, cascade, plans, kept)
+        return dict(zip(names, kept))
+    if plans is None:
+        plans = [{} for _ in nets]
+    elif not isinstance(plans, (list, tuple)) or len(plans) != len(nets):
+        raise ValueError("with several nets, plans is None or a list of one dict per net")
+    per_net = dict(zip(map(id, nets), plans))
+    precision = mnet.get_precision()
+
+    def serve(net, take):
+        with drivers.net_thread(net, precision):
+            b = take()
+            while b is not None:
+                _run_batch(net, frames, hw, b, cascade, per_net[id(net)], kept)
+                b = take()
+
+    drivers.serve_batches(nets, batches, serve)
     return dict(zip(names, kept))
+
+
+def _run_batch(net, frames, hw, batch, cascade: bool, plans: dict, kept: list) -> None:
+    """One plan_batches entry ((net_h, net_w), image indices) on `net` in the calling thread, into kept[i]."""
+    import torch
+    from . import net as mnet, ops
+    (rz_h, rz_w), idx = batch
+    n = len(idx)
+    data = net.inputs[0]
+    net.reshape_input(data, n, 3, rz_h, rz_w)
+    pre = plans.get((rz_h, rz_w))
+    if pre is None:
+        pre = plans[(rz_h, rz_w)] = ops.Preprocess(tuple(hw[idx[0]]), (rz_h, rz_w))
+    net.set_input_images(data, pre, [frames[i] for i in idx])
+    net.forward_only()
+    cfg, classes = mnet.widerface_detect_cfg(rz_h, rz_w)    # the original sizes come with the frames
+    with torch.cuda.stream(mnet._net_stream()):
+        dets = torch.empty((n, 1, cfg.max_rois_per_image, 5), dtype=torch.float32, device="cuda")
+        counts = torch.empty((n, 1), dtype=torch.int32, device="cuda")
+        if cascade:
+            net.detect_cascade_classes(cfg, classes, dets.data_ptr(), counts.data_ptr(), stage="3rd",
+                                       cls_prob="cls_prob_3rd_avg")
+        else:
+            net.detect_classes(cfg, classes, dets.data_ptr(), counts.data_ptr())
+        d, c = dets.cpu().numpy(), counts.cpu().numpy()
+    for k, i in enumerate(idx):
+        kept[i] = d[k, 0, :c[k, 0]].copy()
 
 
 def write_results(event_dir, results) -> None:
