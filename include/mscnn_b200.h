@@ -634,6 +634,27 @@ MSCNN_API int mscnn_net_forward(void* net, int from_layer, int to_layer); /* inc
 MSCNN_API int mscnn_net_resolve_rows(void* net);
 MSCNN_API int mscnn_net_set_graph(void* net, int on);
 MSCNN_API int mscnn_net_graph_replayed(void* net);
+/* Activation reuse (off by default).  With on != 0 the blobs whose lifetimes in a forward do not overlap share one
+ * device arena, planned at the first forward after a change of input shapes, precision or keep set.  Net inputs,
+ * outputs and the n blobs named in `names` stay outside it and readable; after a forward any other blob whose storage
+ * a later blob took is released: its shape stays readable, and mscnn_net_get_blob, mscnn_net_blob_device, the set
+ * entries and mscnn_net_detect* on it return MSCNN_ERR_INVALID (NULL) with a message naming the blob, the layer after
+ * which its storage is reused and how to keep it (mscnn_net_last_error).  mscnn_net_forward(from > 0, ...) is refused
+ * the same way when the range reads a planned blob written before `from`.  A name that is not a blob of the net is
+ * refused (MSCNN_ERR_INVALID, nothing changed).  on == 0 gives every blob its own storage back. */
+MSCNN_API int mscnn_net_set_activation_reuse(void* net, int on, const char* const* names, int n);
+/* Host only (nothing allocated): the arena the plan for the current input shapes and this thread's precision needs,
+ * and what its planned blobs take without reuse.  Both 0 with reuse off. */
+MSCNN_API int mscnn_net_activation_bytes(void* net, size_t* arena, size_t* unplanned);
+/* Host only: the plan, one line per storage (a blob with its Split and in-place tops): "<blob> <bytes> <first>-<last>
+ * @<offset>", first and last being the layers of its first write and last read, or "... input|output|kept" for a
+ * storage outside the arena.  MSCNN_ERR_INVALID when cap is too small. */
+MSCNN_API int mscnn_net_activation_plan_describe(void* net, char* buf, int cap);
+/* Planned blobs an eager forward found without their arena storage, or with device storage of their own the plan did
+ * not give them (a planning bug; each is logged). */
+MSCNN_API unsigned long long mscnn_net_activation_misses(void* net);
+/* The message of the last call this net refused with a message ("" if none). */
+MSCNN_API const char* mscnn_net_last_error(void* net);
 /* Fused groups: the layer that does layer i's work (a Pooling folded into its convolution's epilogue, a sibling
  * ROIPooling pooled by the group's leader), i itself otherwise.  mscnn_net_forward(from, ...) widens `from` back to it. */
 MSCNN_API int mscnn_net_fused_producer(void* net, int layer);

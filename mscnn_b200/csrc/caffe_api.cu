@@ -198,10 +198,18 @@ void* SyncedMemory::mutable_gpu_data() {
 
 // ---------------------------------------------------------------------------- PlaneStore
 PlaneStore::~PlaneStore() {
+  if (!owned) return;
   if (hi) cudaFree(hi);
   if (lo) cudaFree(lo);
 }
 void PlaneStore::reserve(size_t bytes, bool need_lo) {
+  if (!owned) {
+    CHECK(hi && bytes <= capacity && (!need_lo || (lo && bytes <= lo_capacity)))
+        << "activation arena miss: a planned blob needs " << bytes << " bytes per plane" << (need_lo ? " (hi and lo)" : "")
+        << " but its arena slot holds " << capacity << (lo ? " (hi and lo)" : " (hi only)")
+        << "; the activation plan does not describe this forward";
+    return;
+  }
   if (bytes > capacity) {
     if (hi) CUDA_CHECK(cudaFree(hi));
     CUDA_CHECK(cudaMalloc(&hi, bytes));
@@ -307,6 +315,7 @@ void Blob<Dtype>::sync_to_nchw() {
 
 template <typename Dtype>
 const Dtype* Blob<Dtype>::cpu_data() {
+  check_readable();
   CHECK(data_);
   sync_to_nchw();
   return (const Dtype*)data_->cpu_data();
@@ -314,18 +323,21 @@ const Dtype* Blob<Dtype>::cpu_data() {
 template <typename Dtype>
 void Blob<Dtype>::set_cpu_data(Dtype* data) {
   CHECK(data);
+  check_readable();
   data_->set_cpu_data(data);
   layout_head_ = HEAD_NCHW;
   bump_version();
 }
 template <typename Dtype>
 const Dtype* Blob<Dtype>::gpu_data() {
+  check_readable();
   CHECK(data_);
   sync_to_nchw();
   return (const Dtype*)data_->gpu_data();
 }
 template <typename Dtype>
 Dtype* Blob<Dtype>::mutable_cpu_data() {
+  check_readable();
   CHECK(data_);
   sync_to_nchw();
   layout_head_ = HEAD_NCHW;
@@ -334,6 +346,7 @@ Dtype* Blob<Dtype>::mutable_cpu_data() {
 }
 template <typename Dtype>
 Dtype* Blob<Dtype>::mutable_gpu_data() {
+  check_readable();
   CHECK(data_);
   sync_to_nchw();
   layout_head_ = HEAD_NCHW;
@@ -343,6 +356,7 @@ Dtype* Blob<Dtype>::mutable_gpu_data() {
 
 template <typename Dtype>
 typename Blob<Dtype>::Planes Blob<Dtype>::planes(bool split) {
+  check_readable();
   int n, c, h, w;
   planes_dims(&n, &c, &h, &w);
   const int cpad = (c + 63) / 64 * 64;
@@ -369,6 +383,7 @@ typename Blob<Dtype>::Planes Blob<Dtype>::planes(bool split) {
 
 template <typename Dtype>
 typename Blob<Dtype>::Planes Blob<Dtype>::mutable_planes(bool split) {
+  check_readable();
   int n, c, h, w;
   planes_dims(&n, &c, &h, &w);
   const int cpad = (c + 63) / 64 * 64;
@@ -383,6 +398,50 @@ typename Blob<Dtype>::Planes Blob<Dtype>::mutable_planes(bool split) {
   p.lo = split ? planes_->lo : nullptr;
   p.n = n; p.h = h; p.w = w; p.cpad = cpad;
   return p;
+}
+
+template <typename Dtype>
+void Blob<Dtype>::UseArena(void* hi, void* lo, size_t plane_bytes, Dtype* nchw, int nchw_count) {
+  if (hi) {
+    planes_.reset(new PlaneStore());
+    planes_->owned = false;
+    planes_->hi = hi;
+    planes_->lo = lo;
+    planes_->capacity = plane_bytes;
+    planes_->lo_capacity = lo ? plane_bytes : 0;
+  } else {
+    planes_.reset();
+  }
+  if (nchw) {
+    // the slot holds nchw_count values: that is the capacity now, so a Reshape within it keeps the slot
+    capacity_ = nchw_count;
+    data_.reset(new SyncedMemory((size_t)nchw_count * sizeof(Dtype)));
+    data_->set_gpu_data(nchw);
+  } else {
+    data_.reset(new SyncedMemory((size_t)capacity_ * sizeof(Dtype)));
+  }
+  layout_head_ = HEAD_NCHW;
+  planes_split_ = false;
+}
+template <typename Dtype>
+void Blob<Dtype>::LeaveArena() {
+  planes_.reset();
+  data_.reset(new SyncedMemory((size_t)capacity_ * sizeof(Dtype)));
+  layout_head_ = HEAD_NCHW;
+  planes_split_ = false;
+  released_.clear();
+}
+template <typename Dtype>
+bool Blob<Dtype>::OnArena(const void* hi, const void* nchw) const {
+  if (hi && !(planes_ && !planes_->owned && planes_->hi == hi)) return false;
+  if (nchw) return data_ && data_->gpu_ptr() == nchw;
+  return !(data_ && data_->owns_gpu_data());
+}
+template <typename Dtype>
+void Blob<Dtype>::DropDeviceNchw() {
+  if (!data_ || !data_->owns_gpu_data()) return;
+  data_.reset(new SyncedMemory((size_t)capacity_ * sizeof(Dtype)));
+  if (layout_head_ == HEAD_BOTH) layout_head_ = HEAD_PLANES;
 }
 
 template <typename Dtype>

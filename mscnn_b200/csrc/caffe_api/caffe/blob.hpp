@@ -31,12 +31,15 @@ const int kMaxBlobAxes = 32;
 
 namespace caffe {
 
-// Device buffer pair for the planes representation (grow-only, like Blob::Reshape).
+// Device buffer pair for the planes representation (grow-only, like Blob::Reshape).  A store that is not `owned`
+// points into a net's activation arena (Net::set_activation_reuse): it never allocates or frees, and a request
+// beyond its slot is a planning bug, so reserve aborts instead of allocating.
 struct CAFFE_API PlaneStore {
   void* hi = nullptr;
   void* lo = nullptr;
   size_t capacity = 0;     // bytes per plane
   size_t lo_capacity = 0;
+  bool owned = true;
   ~PlaneStore();
   void reserve(size_t bytes, bool need_lo);
 };
@@ -140,6 +143,23 @@ class CAFFE_API Blob {
     return data_->packed_image(key);
   }
 
+  // ---- mscnn_b200 extension: activation arena (Net::set_activation_reuse) ----------------------------------
+  // Storage in a net's arena instead of its own: planes at hi (+ lo) of plane_bytes each (hi NULL: none), NCHW fp32
+  // at nchw for nchw_count values (NULL: none; the NCHW side then allocates lazily as before).  The contents are
+  // undefined until a producer writes them.
+  void UseArena(void* hi, void* lo, size_t plane_bytes, Dtype* nchw, int nchw_count);
+  // back to storage of its own, allocated on first use
+  void LeaveArena();
+  // whether the arena storage set by UseArena(hi, ..., nchw, ...) is still what this blob holds, and (nchw NULL) no
+  // NCHW device buffer of its own has been allocated since
+  bool OnArena(const void* hi, const void* nchw) const;
+  // frees an NCHW device buffer the blob allocated itself (the planes stay)
+  void DropDeviceNchw();
+  // A released blob's storage has been handed to a later blob: every data accessor aborts with `message`; the shape
+  // stays readable.  "" = readable.
+  void set_released(const string& message) { released_ = message; }
+  const string& released() const { return released_; }
+
  protected:
   enum LayoutHead { HEAD_NCHW, HEAD_PLANES, HEAD_BOTH };
   void planes_dims(int* n, int* c, int* h, int* w) const;
@@ -147,6 +167,7 @@ class CAFFE_API Blob {
   void bump_version() {
     if (data_) data_->bump_version();
   }
+  void check_readable() const { CHECK(released_.empty()) << released_; }
   shared_ptr<SyncedMemory> data_;
   shared_ptr<PlaneStore> planes_;
   vector<int> shape_;
@@ -154,6 +175,7 @@ class CAFFE_API Blob {
   int capacity_;
   LayoutHead layout_head_;
   bool planes_split_;
+  string released_;
   DISABLE_COPY_AND_ASSIGN(Blob);
 };
 

@@ -86,6 +86,12 @@ class CAFFE_API ConvolutionLayer : public Layer<Dtype> {
   void set_fused_pool(Blob<Dtype>* pool_top, bool keep_full) { fused_pool_top_ = pool_top; fused_keep_full_ = keep_full; }
   // the route whose epilogue can pool: 64-channel-aligned output, not conv1_1's kernel
   bool can_fuse_pool() const { return num_output_ % 64 == 0 && !is_conv1_1(); }
+  // what a forward reads and writes (Net's activation plan): conv1_1's kernel reads the NCHW fp32 bottom, every
+  // other route planes; the top is planes above 32 outputs, NCHW fp32 for the narrow heads
+  bool reads_nchw() const { return is_conv1_1(); }
+  bool writes_planes() const { return num_output_ > 32; }
+  Blob<Dtype>* fused_pool_top() const { return fused_pool_top_; }
+  bool keep_full() const { return fused_keep_full_; }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   // stride 1, dilation 1, one group: what conv1_1's kernel and the k x 1 head-tap route compute
@@ -162,6 +168,7 @@ class CAFFE_API PoolingLayer : public Layer<Dtype> {
            stride_w_ == 2 && pad_h_ == 0 && pad_w_ == 0;
   }
   void set_fused(bool f) { fused_ = f; }   // folded into the producing convolution: see epilogue_pools
+  bool fused() const { return fused_; }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   int kernel_h_, kernel_w_, stride_h_, stride_w_, pad_h_, pad_w_, mode_, pooled_h_, pooled_w_;
@@ -210,6 +217,7 @@ class CAFFE_API InnerProductLayer : public Layer<Dtype> {
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
   void set_fuse_relu(bool f) { fuse_relu_ = f; }
+  bool writes_planes() const { return N_ > 32; }  // else [M][N] fp32, the Caffe layout
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   int M_, K_, N_;
@@ -265,6 +273,8 @@ class CAFFE_API BoxOutputLayer : public Layer<Dtype> {
   void ResolveRows(const vector<Blob<Dtype>*>& top);
   // after a CUDA-graph replay of this layer's launches (Net::GraphForward): the counts are pending again
   void RearmRows();
+  // the rows Forward sizes its tops for before the count is known
+  int cap_rows(int num) const { return num * cfg_.max_nms_num; }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   mscnn_box_output_cfg cfg_;
@@ -304,6 +314,8 @@ class CAFFE_API ROIPoolingLayer : public Layer<Dtype> {
     channel_offsets_.push_back(follower->channel_offsets_[0]);
     follower->fused_ = true;
   }
+  bool fused() const { return fused_; }
+  Blob<Dtype>* concat_top() const { return concat_top_; }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   int channels_, height_, width_, pooled_height_, pooled_width_;

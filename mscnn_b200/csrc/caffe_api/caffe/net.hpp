@@ -105,6 +105,49 @@ class CAFFE_API Net {
   void set_graph_mode(bool on) { graph_mode_ = on; }
   bool graph_replayed_last_forward() const { return graph_replayed_; }
 
+  // mscnn_b200 extension: activation reuse (off by default; DESIGN.md "Activation memory plan").  With it on, the
+  // storages (a blob with its Split tops and in-place tops) whose lifetimes do not overlap share one device arena, and
+  // after a forward a blob whose bytes a later blob took is released: its shape stays readable, its data accessors
+  // abort with a message naming it.  Net inputs, outputs and the blobs named in `keep` are never in the arena, so they
+  // stay readable.  Every keep name must be a blob of the net.
+  void set_activation_reuse(bool on, const vector<string>& keep = vector<string>());
+  // the message set_activation_reuse(true, keep) would abort with, or ""
+  string ActivationKeepError(const vector<string>& keep) const;
+  bool activation_reuse() const { return reuse_; }
+  struct ActivationStorage {
+    int blob;             // the blob that owns the storage (the others alias it)
+    size_t bytes;         // planes hi (+ lo) and NCHW fp32, each rounded up to 256 B
+    size_t plane_bytes;   // bytes of one plane (0: no planes)
+    bool lo;              // fp32-faithful: a lo plane as well
+    int nchw_count;       // fp32 values of the NCHW side (0: none)
+    int first, last;      // layers (execution order) of its first write and last read
+    long long offset;     // in the arena; -1 = not planned
+    string outside;       // why not: "input", "output" or "kept"
+    vector<int> members;  // every blob on this storage
+    vector<int> touched;  // the layers that read or write it
+  };
+  struct ActivationPlan {
+    vector<ActivationStorage> storages;  // by first write, then blob index
+    size_t arena_bytes = 0;     // the arena the planned storages share
+    size_t planned_bytes = 0;   // what the planned storages take without reuse
+    size_t unplanned_bytes = 0; // the storages outside the arena
+  };
+  // The plan for the current input shapes and this thread's precision (host only: nothing is allocated); empty with
+  // reuse off.
+  const ActivationPlan& activation_plan();
+  // one line per storage: blob, bytes, first and last layer, offset (or why it is outside the arena)
+  string activation_plan_describe();
+  // Planned storages an eager forward found off their arena slot, or holding a device buffer of their own the plan
+  // did not give them (each is also logged).  A plane request beyond its
+  // slot aborts in PlaneStore::reserve instead, before it could allocate.
+  unsigned long long activation_misses() const { return activation_misses_; }
+  // The message a data accessor of blob_name would abort with, or "" (readable, or no such blob).
+  string released_message(const string& blob_name) const;
+  // The message ForwardFromTo(start, end) would abort with, or "".  With reuse on, a range that starts after layer 0
+  // is refused when it reads a planned storage written before it, unless it continues the forward that just ran up to
+  // start - 1 (the C facade splits one forward there to record where the input blob is free).
+  string ForwardRangeError(int start, int end);
+
  protected:
   void AppendTop(const NetParameter& param, const int layer_id, const int top_id,
                  set<string>* available_blobs, map<string, int>* blob_name_to_idx);
@@ -114,6 +157,11 @@ class CAFFE_API Net {
   void FusePooling();
   void MarkDynamicRows();
   bool GraphForward(int start, int end);
+  string ActivationSignature() const;
+  void ComputeActivationPlan(ActivationPlan* plan) const;
+  void BeginActivations(int start, int end);
+  void EndActivations(int start, int end, bool replayed);
+  void DetachActivations();
 
   string name_;
   Phase phase_;
@@ -143,7 +191,18 @@ class CAFFE_API Net {
   bool graph_mode_ = false, graph_replayed_ = false;
   struct GraphState;
   shared_ptr<GraphState> graph_;
-  DISABLE_COPY_AND_ASSIGN(Net);
+  // activation reuse (set_activation_reuse)
+  bool reuse_ = false;
+  vector<string> keep_;
+  ActivationPlan plan_;
+  string plan_signature_;           // what plan_ was made for ("" = nothing)
+  string applied_signature_;        // what the blobs' arena storage was set up for
+  unsigned long long plan_epoch_ = 0;  // changes whenever blob addresses may have changed (part of the graph signature)
+  shared_ptr<void> arena_;          // device memory, grow-only
+  size_t arena_capacity_ = 0;
+  vector<int> on_arena_;            // blobs given arena storage
+  int chain_end_ = -1;              // last layer of the forward in progress (-1: none to continue)
+  unsigned long long activation_misses_ = 0;
 };
 
 }  // namespace caffe

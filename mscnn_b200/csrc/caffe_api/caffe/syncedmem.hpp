@@ -38,6 +38,8 @@ class CAFFE_API SyncedMemory {
   enum SyncedHead { UNINITIALIZED, HEAD_AT_CPU, HEAD_AT_GPU, SYNCED };
   SyncedHead head() { return head_; }
   size_t size() { return size_; }
+  const void* gpu_ptr() const { return gpu_ptr_; }  // the device buffer as it is (NULL: none yet); allocates nothing
+  bool owns_gpu_data() const { return gpu_ptr_ && own_gpu_data_; }  // a device buffer it allocated itself
 
   // mscnn_b200 extension: see the file comment.
   unsigned long version() const { return version_.load(std::memory_order_acquire); }

@@ -425,7 +425,7 @@ bool Net<Dtype>::GraphForward(int start, int end) {
   cudaStream_t stream = Caffe::stream();
   if (!graph_mode_ || time_layers_ || start != 0 || end != (int)layers_.size() - 1 || stream == nullptr) return false;
   std::ostringstream sig;
-  sig << (void*)stream << "|" << (int)Caffe::precision() << "|" << mscnn::config().epoch << "|";
+  sig << (void*)stream << "|" << (int)Caffe::precision() << "|" << mscnn::config().epoch << "|" << plan_epoch_ << "|";
   for (size_t i = 0; i < net_input_blobs_.size(); ++i) sig << net_input_blobs_[i]->shape_string() << ";";
   unsigned long versions = 0;
   for (size_t i = 0; i < layers_.size(); ++i)
@@ -473,7 +473,9 @@ Dtype Net<Dtype>::ForwardFromTo(int start, int end) {
   CHECK_GE(start, 0);
   CHECK_LT(end, (int)layers_.size());
   start = fused_producer(start);  // a range never starts inside a fused group (net.hpp fused_producer)
+  BeginActivations(start, end);
   if (GraphForward(start, end)) {
+    EndActivations(start, end, true);
     if (!lazy_rows_) ResolveRows();
     return Dtype(0);
   }
@@ -495,6 +497,7 @@ Dtype Net<Dtype>::ForwardFromTo(int start, int end) {
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
   }
+  EndActivations(start, end, false);
   if (!lazy_rows_) ResolveRows();
   return Dtype(0);
 }

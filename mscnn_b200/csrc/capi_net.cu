@@ -31,6 +31,7 @@ struct NetHandle {
   // geometry belongs to the forward, so "set batch k + 1, then detect batch k" pairs each batch with its own sizes.
   std::vector<int> next_org_hw;
   std::vector<float> geom;
+  std::string last_error;  // the message of the last call this net refused (mscnn_net_last_error)
   ~NetHandle() {
     if (det_ws) cudaFree(det_ws);
     if (input_ready) cudaEventDestroy(input_ready);
@@ -39,6 +40,17 @@ struct NetHandle {
   }
 };
 NetHandle* H(void* h) { return static_cast<NetHandle*>(h); }
+// A refusal with a message: kept for mscnn_net_last_error and printed, as the other refusals print theirs.
+bool refuse(NetHandle* nh, const char* what, const std::string& msg) {
+  nh->last_error = msg;  // a check that passes clears the last message
+  if (msg.empty()) return false;
+  fprintf(stderr, "%s: %s\n", what, msg.c_str());
+  return true;
+}
+// Whether `name` is a blob whose storage activation reuse handed to a later blob (its data is gone).
+bool released(NetHandle* nh, const char* what, const char* name) {
+  return refuse(nh, what, nh->net->released_message(name));
+}
 // A synchronous input write issued after an asynchronous upload must land after it (the newer write wins).
 int settle_pending(NetHandle* nh) {
   if (!nh->pending_input) return MSCNN_OK;
@@ -122,6 +134,9 @@ int detect_inputs(NetHandle* h, const mscnn_detect_cfg* cfg, const mscnn_detect_
     h->det_ws_bytes = need;
   }
   if (!h->geom.empty() && h->geom.size() != (size_t)4 * N) return MSCNN_ERR_INVALID;
+  if (released(h, "mscnn_net_detect", prop) || released(h, "mscnn_net_detect", cls) ||
+      released(h, "mscnn_net_detect", bbox))
+    return MSCNN_ERR_INVALID;
   in->N = N;
   in->prop = h->net->blob_by_name(prop)->gpu_data();
   in->cls = h->net->blob_by_name(cls)->gpu_data();
@@ -300,7 +315,7 @@ int mscnn_net_set_blob(void* h, const char* name, const float* host, long count)
   H(h)->net->ResolveRowsFor(name);
   if (!H(h)->net->has_blob(name)) return MSCNN_ERR_INVALID;
   Blob<float>* b = H(h)->net->blob_by_name(name).get();
-  if (b->count() != count) return MSCNN_ERR_INVALID;
+  if (b->count() != count || released(H(h), "mscnn_net_set_blob", name)) return MSCNN_ERR_INVALID;
   if (settle_pending(H(h)) != MSCNN_OK) return MSCNN_ERR_CUDA;
   float* dst = b->mutable_gpu_data();
   return cudaMemcpyAsync(dst, host, sizeof(float) * count, cudaMemcpyHostToDevice, Caffe::stream()) == cudaSuccess
@@ -387,7 +402,7 @@ int mscnn_net_set_blob_device(void* h, const char* name, const float* dev, long 
   H(h)->net->ResolveRowsFor(name);
   if (!H(h)->net->has_blob(name)) return MSCNN_ERR_INVALID;
   Blob<float>* b = H(h)->net->blob_by_name(name).get();
-  if (b->count() != count) return MSCNN_ERR_INVALID;
+  if (b->count() != count || released(H(h), "mscnn_net_set_blob_device", name)) return MSCNN_ERR_INVALID;
   if (settle_pending(H(h)) != MSCNN_OK) return MSCNN_ERR_CUDA;
   return cudaMemcpyAsync(b->mutable_gpu_data(), dev, sizeof(float) * count, cudaMemcpyDeviceToDevice,
                          Caffe::stream()) == cudaSuccess
@@ -398,7 +413,7 @@ int mscnn_net_get_blob(void* h, const char* name, float* host, long count) {
   H(h)->net->ResolveRowsFor(name);
   if (!H(h)->net->has_blob(name)) return MSCNN_ERR_INVALID;
   Blob<float>* b = H(h)->net->blob_by_name(name).get();
-  if (b->count() != count) return MSCNN_ERR_INVALID;
+  if (b->count() != count || released(H(h), "mscnn_net_get_blob", name)) return MSCNN_ERR_INVALID;
   const float* src = b->gpu_data();
   if (cudaMemcpyAsync(host, src, sizeof(float) * count, cudaMemcpyDeviceToHost, Caffe::stream()) != cudaSuccess)
     return MSCNN_ERR_CUDA;
@@ -406,7 +421,7 @@ int mscnn_net_get_blob(void* h, const char* name, float* host, long count) {
 }
 const float* mscnn_net_blob_device(void* h, const char* name) {
   H(h)->net->ResolveRowsFor(name);
-  if (!H(h)->net->has_blob(name)) return nullptr;
+  if (!H(h)->net->has_blob(name) || released(H(h), "mscnn_net_blob_device", name)) return nullptr;
   return H(h)->net->blob_by_name(name)->gpu_data();
 }
 
@@ -416,6 +431,7 @@ int mscnn_net_forward(void* h, int from, int to) {
   Net<float>* net = nh->net.get();
   if (to < 0) to = (int)net->layers().size() - 1;
   if (from < 0 || from > to || to >= (int)net->layers().size()) return MSCNN_ERR_INVALID;
+  if (refuse(nh, "mscnn_net_forward", net->ForwardRangeError(net->fused_producer(from), to))) return MSCNN_ERR_INVALID;
   if (from == 0) {
     // a forward from the first layer consumes the sizes recorded for it; the net input's H and W are the net size
     const int n = (int)nh->next_org_hw.size() / 2;
@@ -469,7 +485,7 @@ int mscnn_net_set_blob_async(void* h, const char* name, const float* host, long 
   Net<float>* net = nh->net.get();
   if (!net->has_blob(name)) return MSCNN_ERR_INVALID;
   Blob<float>* b = net->blob_by_name(name).get();
-  if (b->count() != count) return MSCNN_ERR_INVALID;
+  if (b->count() != count || released(nh, "mscnn_net_set_blob_async", name)) return MSCNN_ERR_INVALID;
   int rc = async_begin(nh);
   if (rc) return rc;
   float* dst = b->mutable_gpu_data();
@@ -483,6 +499,33 @@ int mscnn_net_set_graph(void* h, int on) {
   H(h)->net->set_graph_mode(on != 0);
   return MSCNN_OK;
 }
+int mscnn_net_set_activation_reuse(void* h, int on, const char* const* names, int n) {
+  if (!h || n < 0 || (n > 0 && !names)) return MSCNN_ERR_INVALID;
+  std::vector<std::string> keep;
+  for (int k = 0; k < n; ++k) {
+    if (!names[k]) return MSCNN_ERR_INVALID;
+    keep.push_back(names[k]);
+  }
+  if (refuse(H(h), "mscnn_net_set_activation_reuse", H(h)->net->ActivationKeepError(keep))) return MSCNN_ERR_INVALID;
+  H(h)->net->set_activation_reuse(on != 0, keep);
+  return MSCNN_OK;
+}
+int mscnn_net_activation_bytes(void* h, size_t* arena, size_t* unplanned) {
+  if (!h || !arena || !unplanned) return MSCNN_ERR_INVALID;
+  const Net<float>::ActivationPlan& p = H(h)->net->activation_plan();
+  *arena = p.arena_bytes;
+  *unplanned = p.planned_bytes;
+  return MSCNN_OK;
+}
+int mscnn_net_activation_plan_describe(void* h, char* buf, int cap) {
+  if (!h || !buf) return MSCNN_ERR_INVALID;
+  const std::string s = H(h)->net->activation_plan_describe();
+  if ((int)s.size() + 1 > cap) return MSCNN_ERR_INVALID;
+  memcpy(buf, s.c_str(), s.size() + 1);
+  return MSCNN_OK;
+}
+unsigned long long mscnn_net_activation_misses(void* h) { return H(h)->net->activation_misses(); }
+const char* mscnn_net_last_error(void* h) { return H(h)->last_error.c_str(); }
 int mscnn_net_graph_replayed(void* h) { return H(h)->net->graph_replayed_last_forward() ? 1 : 0; }
 // wait for the data-dependent row count of the last forward and trim the blob shapes (every accessor does this)
 int mscnn_net_resolve_rows(void* h) {

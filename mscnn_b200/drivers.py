@@ -119,11 +119,13 @@ SPECS = {"kitti_car": KITTI_CAR, "kitti_ped_cyc": KITTI_PED_CYC, "caltech": CALT
          "kitti_car_cascade": KITTI_CAR_CASCADE, "citypersons": CITYPERSONS}
 
 
-def make_nets(proto: str, weights, devices=(0,)) -> list:
+def make_nets(proto: str, weights, devices=(0,), reuse_activations: bool = False) -> list:
     """One net.Net of `proto` per entry of `devices` (device ids, repeats allowed), for run / widerface.run over several
     nets.  The first net on each device loads `weights` (a {layer: [blobs]} dict, as Net.set_params takes, or a
     .caffemodel path); the others on that device share its weights (Net.share_trained_layers_with), so each device
-    holds one copy.  The calling thread's device is restored."""
+    holds one copy.  reuse_activations: each net shares one arena among the blobs whose lifetimes do not overlap
+    (Net.set_activation_reuse); run and widerface.run keep the blobs their post-process reads.  The calling thread's
+    device is restored."""
     import torch
     from . import net as mnet
     prev = torch.cuda.current_device()
@@ -141,10 +143,21 @@ def make_nets(proto: str, weights, devices=(0,)) -> list:
                 else:
                     n.copy_from(weights)
                 owners[d] = n
+            if reuse_activations:
+                n.set_activation_reuse(True)
             nets.append(n)
     finally:
         mnet.set_device(prev)
     return nets
+
+
+def keep_readable(nets, blobs) -> None:
+    """Adds `blobs` to the keep set of every net of `nets` (one net or a list) that reuses activation memory, so that
+    what the post-process reads after a forward is still there."""
+    for n in nets if isinstance(nets, (list, tuple)) else [nets]:
+        keep = getattr(n, "reuse_keep", None)
+        if keep is not None and not set(blobs) <= set(keep):
+            n.set_activation_reuse(True, tuple(keep) + tuple(b for b in blobs if b not in keep))
 
 
 def serve_batches(nets, batches, serve) -> None:
@@ -231,6 +244,7 @@ def run(nets, frames, spec: DriverSpec, batch: int = 8, net_hw: tuple[int, int] 
         return out
     net_hw = tuple(net_hw or spec.net_hw)
     ops.image_sizes_channels(frames)                          # every frame checked before any work is issued
+    keep_readable(nets, spec.blobs)
     chunks = [list(range(k, min(k + batch, len(frames)))) for k in range(0, len(frames), batch)]
     if not isinstance(nets, (list, tuple)):
         todo = iter(chunks)

@@ -84,6 +84,13 @@ def _declare(L):
     L.mscnn_net_detect_push_classes.restype = C.c_int
     L.mscnn_net_detect_push_classes.argtypes = [C.c_void_p, C.POINTER(capi.DetectCfg), C.POINTER(capi.DetectClasses),
                                                 C.c_void_p]
+    L.mscnn_net_set_activation_reuse.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.c_int]
+    L.mscnn_net_activation_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    L.mscnn_net_activation_plan_describe.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
+    L.mscnn_net_activation_misses.restype = C.c_ulonglong
+    L.mscnn_net_activation_misses.argtypes = [C.c_void_p]
+    L.mscnn_net_last_error.restype = C.c_char_p
+    L.mscnn_net_last_error.argtypes = [C.c_void_p]
     L.mscnn_set_precision.argtypes = [C.c_int]
     L.mscnn_set_stream.argtypes = [C.c_void_p]
     L.mscnn_set_device.argtypes = [C.c_int]
@@ -143,6 +150,13 @@ class Net:
         self.blob_names = [L.mscnn_net_blob_name(h, i).decode() for i in range(L.mscnn_net_num_blobs(h))]
         self.inputs = [L.mscnn_net_input_name(h, i).decode() for i in range(L.mscnn_net_num_inputs(h))]
         self.outputs = [L.mscnn_net_output_name(h, i).decode() for i in range(L.mscnn_net_num_outputs(h))]
+        self.reuse_keep: tuple[str, ...] | None = None   # set_activation_reuse: the keep set, None = reuse off
+
+    def _check(self, rc: int, what: str) -> None:
+        """capi.check, with the message of a refusal that carries one (a released blob, a refused range)."""
+        if rc != capi.OK:
+            msg = self._L.mscnn_net_last_error(self._h).decode()
+            raise capi.MscnnError(f"{what} failed with status {rc}" + (f": {msg}" if msg else ""))
 
     def __del__(self):
         if getattr(self, "_h", None):
@@ -238,14 +252,49 @@ class Net:
     def blob(self, name: str) -> np.ndarray:
         shp = self.blob_shape(name)
         out = np.empty(shp, dtype=np.float32)
-        capi.check(self._L.mscnn_net_get_blob(self._h, name.encode(), out.ctypes.data, out.size), f"get_blob({name})")
+        self._check(self._L.mscnn_net_get_blob(self._h, name.encode(), out.ctypes.data, out.size), f"get_blob({name})")
         return out
 
     def blob_device_ptr(self, name: str) -> int:
         p = self._L.mscnn_net_blob_device(self._h, name.encode())
         if not p:
+            msg = self._L.mscnn_net_last_error(self._h).decode()
+            if msg:                                   # a released blob: say why
+                raise capi.MscnnError(f"blob_device({name}): {msg}")
             raise KeyError(name)
         return p
+
+    # ---- activation memory -------------------------------------------------------------------
+    def set_activation_reuse(self, on: bool = True, keep=()) -> None:
+        """Let blobs whose lifetimes in a forward do not overlap share one device arena (Net::set_activation_reuse).
+        The inputs, the outputs and the blobs named in `keep` stay readable after a forward; reading any other blob
+        whose storage a later blob took raises MscnnError naming it.  on=False gives every blob its own storage back.
+        Raises MscnnError for a keep name that is not a blob, changing nothing."""
+        names = [str(k).encode() for k in keep]
+        arr = (C.c_char_p * max(len(names), 1))(*names)
+        self._check(self._L.mscnn_net_set_activation_reuse(self._h, int(bool(on)), arr, len(names)),
+                    "set_activation_reuse")
+        self.reuse_keep = tuple(str(k) for k in keep) if on else None
+
+    def activation_bytes(self) -> tuple[int, int]:
+        """(arena, without reuse): the bytes of the plan for the current input shapes and this thread's precision,
+        and what its planned blobs take without reuse; (0, 0) with reuse off.  Host only."""
+        arena, unplanned = C.c_size_t(), C.c_size_t()
+        capi.check(self._L.mscnn_net_activation_bytes(self._h, C.byref(arena), C.byref(unplanned)), "activation_bytes")
+        return int(arena.value), int(unplanned.value)
+
+    def activation_plan(self) -> str:
+        """The plan, one line per storage: "<blob> <bytes> <first>-<last> @<offset>" or "... input|output|kept"."""
+        cap = 1 << 16
+        while True:
+            buf = C.create_string_buffer(cap)
+            if self._L.mscnn_net_activation_plan_describe(self._h, buf, cap) == capi.OK:
+                return buf.value.decode()
+            cap *= 4
+
+    def activation_misses(self) -> int:
+        """Planned blobs an eager forward found without their arena storage (0 unless the plan is wrong)."""
+        return int(self._L.mscnn_net_activation_misses(self._h))
 
     # ---- execution -----------------------------------------------------------------------
     def set_input_async(self, name: str, data) -> None:
@@ -327,7 +376,7 @@ class Net:
     def forward_only(self, start: str | None = None, end: str | None = None) -> None:
         i0 = self.layer_names.index(start) if start else 0
         i1 = self.layer_names.index(end) if end else -1
-        capi.check(self._L.mscnn_net_forward(self._h, i0, i1), "forward")
+        self._check(self._L.mscnn_net_forward(self._h, i0, i1), "forward")
 
     def forward(self, **inputs) -> dict[str, np.ndarray]:
         for k, v in inputs.items():
@@ -348,20 +397,20 @@ class Net:
         return {n: float(ms[i]) for i, n in enumerate(self.layer_names)}
 
     def detect(self, cfg: capi.DetectCfg, dets_dev_ptr: int, counts_dev_ptr: int) -> None:
-        capi.check(self._L.mscnn_net_detect(self._h, cfg, dets_dev_ptr, counts_dev_ptr), "net_detect")
+        self._check(self._L.mscnn_net_detect(self._h, cfg, dets_dev_ptr, counts_dev_ptr), "net_detect")
 
     def detect_classes(self, cfg: capi.DetectCfg, classes: capi.DetectClasses, dets_dev_ptr: int,
                        counts_dev_ptr: int) -> None:
         """Final detections of several classes in one post-process (mscnn_net_detect_classes): dets
         [N][C][max_rois_per_image][5], counts [N][C], slot [n][c] = image n, class classes.cls_ids[c]."""
-        capi.check(self._L.mscnn_net_detect_classes(self._h, cfg, classes, dets_dev_ptr, counts_dev_ptr),
+        self._check(self._L.mscnn_net_detect_classes(self._h, cfg, classes, dets_dev_ptr, counts_dev_ptr),
                    "net_detect_classes")
 
     def detect_cascade_classes(self, cfg: capi.DetectCfg, classes: capi.DetectClasses, dets_dev_ptr: int,
                                counts_dev_ptr: int, stage: str = "3rd", cls_prob: str | None = None) -> None:
         """detect_cascade for several classes: dets [N][C][max_rois_per_image][5], counts [N][C]."""
         prop = "proposals" if stage == "1st" else f"proposals_{stage}"
-        capi.check(self._L.mscnn_net_detect_cascade_classes(self._h, cfg, classes, prop.encode(),
+        self._check(self._L.mscnn_net_detect_cascade_classes(self._h, cfg, classes, prop.encode(),
                                                             (cls_prob or f"cls_prob_{stage}").encode(),
                                                             f"output_bbox_{stage}".encode(), dets_dev_ptr,
                                                             counts_dev_ptr), "net_detect_cascade_classes")
@@ -371,7 +420,7 @@ class Net:
         parallel.PeerExchange made for batch * C slots (PeerExchange(batch * C, cap, ...))."""
         from . import parallel
         parallel._declare_xchg(self._L)
-        capi.check(self._L.mscnn_net_detect_push_classes(self._h, cfg, classes, xchg.handle), "net_detect_push_classes")
+        self._check(self._L.mscnn_net_detect_push_classes(self._h, cfg, classes, xchg.handle), "net_detect_push_classes")
 
     def fused_producer(self, layer: str) -> str:
         """The layer that does `layer`'s work (itself unless the fusion pass folded it into another layer)."""
@@ -388,21 +437,21 @@ class Net:
     def detect_gather(self, cfg: capi.DetectCfg, comm, payload_all_ptr: int) -> None:
         """Final detections of this rank packed into its slot of `payload_all` + ONE all-gather on the communicator's
         stream (mscnn_net_detect_gather); `comm` is a parallel.Comm."""
-        capi.check(self._L.mscnn_net_detect_gather(self._h, cfg, comm.handle, payload_all_ptr), "net_detect_gather")
+        self._check(self._L.mscnn_net_detect_gather(self._h, cfg, comm.handle, payload_all_ptr), "net_detect_gather")
 
     def detect_push(self, cfg: capi.DetectCfg, xchg) -> None:
         """Final detections packed and pushed into every rank's gather buffer by the post-process kernel itself
         (mscnn_net_detect_push); `xchg` is a parallel.PeerExchange."""
         from . import parallel
         parallel._declare_xchg(self._L)
-        capi.check(self._L.mscnn_net_detect_push(self._h, cfg, xchg.handle), "net_detect_push")
+        self._check(self._L.mscnn_net_detect_push(self._h, cfg, xchg.handle), "net_detect_push")
 
     def detect_cascade(self, cfg: capi.DetectCfg, dets_dev_ptr: int, counts_dev_ptr: int, stage: str = "3rd",
                        cls_prob: str | None = None) -> None:
         """Final detections of a cascade net from one stage's blobs (run_cascademscnn.m:36-48):
         proposals[_2nd|_3rd], cls_prob_<stage> (or e.g. "cls_prob_3rd_avg"), output_bbox_<stage>."""
         prop = "proposals" if stage == "1st" else f"proposals_{stage}"
-        capi.check(self._L.mscnn_net_detect_cascade(self._h, cfg, prop.encode(),
+        self._check(self._L.mscnn_net_detect_cascade(self._h, cfg, prop.encode(),
                                                     (cls_prob or f"cls_prob_{stage}").encode(),
                                                     f"output_bbox_{stage}".encode(), dets_dev_ptr, counts_dev_ptr),
                    "net_detect_cascade")

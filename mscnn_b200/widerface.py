@@ -65,6 +65,8 @@ def run(nets, frames, names, cascade: bool = False, max_size: int = MAX_SIZE, ma
     hw = ops.image_sizes(frames)
     kept: list[np.ndarray | None] = [None] * len(frames)
     batches = plan_batches(hw, max_size=max_size, max_batch=max_batch, pixel_budget=pixel_budget)
+    drivers.keep_readable(nets, ("proposals_3rd", "cls_prob_3rd_avg", "output_bbox_3rd") if cascade
+                          else ("proposals_score", "cls_pred", "bbox_pred"))
     if not isinstance(nets, (list, tuple)):
         plans = {} if plans is None else plans
         for b in batches:
