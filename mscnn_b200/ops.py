@@ -369,39 +369,43 @@ def box_output_forward(cfg: capi.BoxOutputCfg, maps: list[torch.Tensor]):
     return rois, rois_score, num_out
 
 
-def roi_pool_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled: int, scale: float,
+def roi_pool_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled, scale: float,
                      pad_ratio: float, out: Planes | None = None, channel_offset: int = 0,
                      out_channels: int | None = None) -> Planes:
+    """ROIPooling bins [R, pooled_h, pooled_w, out_channels]; pooled: an int, or (pooled_h, pooled_w)."""
     n, h, w, c = x.hi.shape
+    ph, pw = _pair(pooled)
     ctot = out_channels or c
     if out is None:
-        y_hi = torch.zeros((num_rois, pooled, pooled, ctot), dtype=torch.bfloat16, device=x.hi.device)
+        y_hi = torch.zeros((num_rois, ph, pw, ctot), dtype=torch.bfloat16, device=x.hi.device)
         y_lo = torch.zeros_like(y_hi) if x.lo is not None else None
         out = Planes(y_hi, y_lo, ctot)
     capi.check(capi.lib().mscnn_roi_pool_forward(capi.ptr(x.hi), capi.ptr(x.lo), n, h, w, c, capi.ptr(rois),
-                                                 num_rois, pooled, pooled, scale, pad_ratio, capi.ptr(out.hi),
+                                                 num_rois, ph, pw, scale, pad_ratio, capi.ptr(out.hi),
                                                  capi.ptr(out.lo), ctot, channel_offset, _stream()),
                "roi_pool_forward")
     return out
 
 
-def roi_pool_multi_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled: int, scale: float,
+def roi_pool_multi_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled, scale: float,
                            pad_ratios, channel_offsets, out: Planes | None = None, out_channels: int | None = None,
                            dyn: torch.Tensor | None = None) -> Planes:
     """Up to four pad_ratio variants of one ROI set in one launch; variant i is written at channel offset
-    channel_offsets[i] of a [R, pooled, pooled, out_channels] output.  dyn: device int32 ROI count."""
+    channel_offsets[i] of a [R, pooled_h, pooled_w, out_channels] output.  pooled: an int, or (pooled_h, pooled_w).
+    dyn: device int32 ROI count."""
     import ctypes as C
     n, h, w, c = x.hi.shape
+    ph, pw = _pair(pooled)
     nv = len(pad_ratios)
     assert len(channel_offsets) == nv
     ctot = out_channels or nv * c
     if out is None:
-        y_hi = torch.zeros((num_rois, pooled, pooled, ctot), dtype=torch.bfloat16, device=x.hi.device)
+        y_hi = torch.zeros((num_rois, ph, pw, ctot), dtype=torch.bfloat16, device=x.hi.device)
         y_lo = torch.zeros_like(y_hi) if x.lo is not None else None
         out = Planes(y_hi, y_lo, ctot)
     ratios = (C.c_float * max(nv, 1))(*pad_ratios)
     offs = (C.c_int * max(nv, 1))(*channel_offsets)
-    args = (capi.ptr(x.hi), capi.ptr(x.lo), n, h, w, c, capi.ptr(rois), num_rois, pooled, pooled, scale, nv,
+    args = (capi.ptr(x.hi), capi.ptr(x.lo), n, h, w, c, capi.ptr(rois), num_rois, ph, pw, scale, nv,
             C.cast(ratios, C.c_void_p), C.cast(offs, C.c_void_p), capi.ptr(out.hi), capi.ptr(out.lo), ctot)
     if dyn is None:
         capi.check(capi.lib().mscnn_roi_pool_multi_forward(*args, _stream()), "roi_pool_multi_forward")
@@ -412,18 +416,20 @@ def roi_pool_multi_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled:
     return out
 
 
-def roi_align_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled: int, scale: float,
+def roi_align_forward(x: Planes, rois: torch.Tensor, num_rois: int, pooled, scale: float,
                       pad_ratio: float, out: Planes | None = None, channel_offset: int = 0,
                       out_channels: int | None = None, dyn: torch.Tensor | None = None) -> Planes:
-    """ROIAlign grid [R, pooled+1, pooled+1, C] (roi_align_layer.cpp:49-139), written at channel offset
-    ``channel_offset`` of an ``out_channels``-wide output.  dyn: device int32 ROI count."""
+    """ROIAlign grid [R, pooled_h+1, pooled_w+1, C] (roi_align_layer.cpp:49-139), written at channel offset
+    ``channel_offset`` of an ``out_channels``-wide output.  pooled: an int, or (pooled_h, pooled_w).
+    dyn: device int32 ROI count."""
     n, h, w, c = x.hi.shape
+    ph, pw = _pair(pooled)
     ctot = out_channels or c
     if out is None:
-        y_hi = torch.zeros((num_rois, pooled + 1, pooled + 1, ctot), dtype=torch.bfloat16, device=x.hi.device)
+        y_hi = torch.zeros((num_rois, ph + 1, pw + 1, ctot), dtype=torch.bfloat16, device=x.hi.device)
         y_lo = torch.zeros_like(y_hi) if x.lo is not None else None
         out = Planes(y_hi, y_lo, ctot)
-    args = (capi.ptr(x.hi), capi.ptr(x.lo), n, h, w, c, capi.ptr(rois), num_rois, pooled, pooled, scale, pad_ratio,
+    args = (capi.ptr(x.hi), capi.ptr(x.lo), n, h, w, c, capi.ptr(rois), num_rois, ph, pw, scale, pad_ratio,
             capi.ptr(out.hi), capi.ptr(out.lo), ctot, channel_offset)
     if dyn is None:
         capi.check(capi.lib().mscnn_roi_align_forward(*args, _stream()), "roi_align_forward")

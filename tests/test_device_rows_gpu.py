@@ -40,10 +40,11 @@ def _counts(b, cap):
     return [-5, 0, 1, b - 1, b, b + 1, 2 * b + 7, cap - 1, cap, cap + 17]
 
 
-def _check_counts(cuda, launch, outs, full, b, cap, what):
-    """launch(dyn) writes into `outs` (row dimension first); `full` are the same tensors of a launch without a count."""
+def _check_counts(cuda, launch, outs, full, b, cap, what, counts=None):
+    """launch(dyn) writes into `outs` (row dimension first); `full` are the same tensors of a launch without a count.
+    counts: the device counts to try (default _counts(b, cap))."""
     dyn = torch.zeros(1, dtype=torch.int32, device=cuda)
-    for count in _counts(b, cap):
+    for count in _counts(b, cap) if counts is None else counts:
         for t in outs:
             _fill(t)
         dyn.fill_(count)
