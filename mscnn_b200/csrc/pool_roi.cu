@@ -111,8 +111,10 @@ __global__ void pool_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfl
 // would walk a plane per thread.  Here a CTA owns one image and 8 consecutive 8-channel groups (128 contiguous bytes
 // per pixel and plane); its 256 threads are 32 pixel slices x 8 groups, slice s taking pixels s, s + 32, ... with
 // four loads in flight, and slice 0 then folds the 32 partial results in slice order.  MAX is exact in any order.
-// AVE sums hi + lo in fp32 in that fixed order (deterministic), not the reference's row-major one: the two differ by
-// at most (H W - 1) 2^-24 sum|x| / (H W) in the mean, far inside the planes' own 2^-17 relative rounding.
+// AVE sums hi + lo in fp32 in that fixed order (deterministic), not the reference's row-major one: like the
+// reference's, its mean lies within (H W - 1) 2^-24 mean|x| of the exact mean (plus the division's rounding), so the
+// two differ by at most twice that (tests/test_faithful_planes_gpu.py holds the kernel to this order bit for bit and
+// to the bound).
 constexpr int kGlobalSlices = 32, kGlobalGroups = 8;
 __global__ void __launch_bounds__(kGlobalSlices * kGlobalGroups)
 global_pool_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl,

@@ -1,7 +1,8 @@
-"""Shared by tests/test_deconv_cpu.py, tests/test_deconv_gpu.py and tests/golden/make_deconv_golden.py: the reference's
-deconvolution restated in numpy (the direct scatter of col2im, and its split by output phase into stride-1 convolutions
-that mscnn_deconv_forward runs), the packed-weight layout, and the small net that runs every served Deconvolution
-geometry end to end.
+"""Shared by tests/test_deconv_cpu.py, tests/test_deconv_gpu.py, tests/test_faithful_planes_*.py and
+tests/golden/make_deconv_golden.py: the reference's deconvolution restated in numpy (the direct scatter of col2im, and
+its split by output phase into stride-1 convolutions that mscnn_deconv_forward runs; the depthwise layer in the
+reference's fp32 order), the packed-weight layout, and the small net that runs every served Deconvolution geometry end
+to end.
 
 Reference: DeconvolutionLayer::compute_output_shape / Forward_cpu (deconv_layer.cpp:8-40), col2im_cpu
 (util/im2col.cpp)."""
@@ -47,6 +48,33 @@ def scatter_deconv(x, w, stride, pad, dil=1, group=1, bias=None):
     y = full[:, :, ph:ph + ho, pw:pw + wo]
     if bias is not None:
         y = y + np.asarray(bias, np.float64)[None, :, None, None]
+    return y
+
+
+def depthwise_col2im_f32(x, w, bias=None, stride=1, pad=0, dil=1):
+    """A depthwise deconvolution (group == channels == num_output) in the reference's own fp32 arithmetic and order:
+    each product x w rounded to fp32 (the K = 1 gemm of backward_cpu_gemm), added by col2im into a zeroed image in
+    increasing (ky, kx), then the bias added (forward_cpu_bias).  x [N, C, H, W], w [C, 1, KH, KW], bias [C] or None."""
+    x, w = np.asarray(x, np.float32), np.asarray(w, np.float32)
+    (sh, sw), (ph, pw), (dh, dw) = _pair(stride), _pair(pad), _pair(dil)
+    n, c, h, wd = x.shape
+    kh, kw = w.shape[2:]
+    ho, wo = deconv_out(h, kh, sh, ph, dh), deconv_out(wd, kw, sw, pw, dw)
+    y = np.zeros((n, c, ho, wo), np.float32)
+    iy, ix = np.arange(h), np.arange(wd)
+    for ky in range(kh):
+        oy = iy * sh - ph + ky * dh
+        my = (oy >= 0) & (oy < ho)
+        for kx in range(kw):
+            ox = ix * sw - pw + kx * dw
+            mx = (ox >= 0) & (ox < wo)
+            if not my.any() or not mx.any():
+                continue
+            prod = x[:, :, my][:, :, :, mx] * w[:, 0, ky, kx][None, :, None, None]
+            # one tap reaches each output at most once: a plain fp32 add per output
+            y[:, :, oy[my][:, None], ox[mx][None, :]] += prod
+    if bias is not None:
+        y = y + np.asarray(bias, np.float32)[None, :, None, None]
     return y
 
 
