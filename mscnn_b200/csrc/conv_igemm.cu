@@ -111,6 +111,181 @@ __host__ __device__ inline IgemmLayout igemm_layout(const IgemmParams& p, int bl
   return l;
 }
 
+// Tile `tile` of the static schedule: n tile fastest, so CTAs working on the same pixels share the activation tile
+// through L2; the M tile is the pixel box (tw, th, tn).
+struct TileCoord {
+  int n_tile, tw, th, tn;
+};
+__device__ __forceinline__ TileCoord tile_coord(const IgemmParams& p, int tile) {
+  TileCoord t;
+  t.n_tile = tile % p.n_tiles;
+  int m = tile / p.n_tiles;
+  t.tw = m % p.tiles_w;
+  m /= p.tiles_w;
+  t.th = m % p.tiles_h;
+  t.tn = m / p.tiles_h;
+  return t;
+}
+
+// Producer warp: the TMA loads of every tile of this CTA, k-blocks in the order (term, dy, chunk, dx), each k-block into
+// the next stage of `ring` (A slot s at sA + s a_stride, B stage s at sB + s b_stride).  The whole warp
+// walks the loops (warp-uniform control flow); one elected lane issues.  Row-share fetches the activation rows of one
+// (term, dy, channel chunk) ONCE, with a one-pixel halo on each side ({64, box_w + 2, box_h, 1} from column w0 - pad:
+// TMA zero fill is still the padding), for the taps dx = 0, 1, 2; each stage then carries only the weight tiles.
+// Without row-share each stage carries the tap's shifted activation tile as well.
+template <int BLOCK_N, bool FAT>
+__device__ __forceinline__ void produce_tiles(const IgemmParams& p, const CUtensorMap* tmA_hi, const CUtensorMap* tmA_lo,
+                                              const CUtensorMap* tmB_hi, const CUtensorMap* tmB_lo, uint32_t sA,
+                                              uint32_t a_stride, uint32_t sB, uint32_t b_stride, ptx::Ring& ring,
+                                              ptx::Ring& a_ring, int terms, int total_tiles) {
+  constexpr uint32_t kPlanes = FAT ? 2u : 1u;
+  constexpr uint32_t kBBytes = BLOCK_N * kBlockK * 2;
+  const uint32_t a_tx = kPlanes * static_cast<uint32_t>((p.box_w + (p.rowshare ? 2 : 0)) * p.box_h * p.box_n) * kBlockK * 2;
+  const uint32_t stage_tx = kPlanes * kBBytes + (p.rowshare ? 0u : a_tx);
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const TileCoord t = tile_coord(p, tile);
+    const int w0 = t.tw * p.box_w * p.stride_w - p.pad_w, h0 = t.th * p.box_h * p.stride_h - p.pad_h, n0 = t.tn * p.box_n;
+    const int c_base = t.n_tile * BLOCK_N / p.cout_g * p.cin_g;  // first input channel of the tile's group
+    for (int term = 0; term < terms; ++term) {
+      const CUtensorMap* mapA = (term == 2) ? tmA_lo : tmA_hi;
+      const CUtensorMap* mapB = (term == 1) ? tmB_lo : tmB_hi;
+      for (int dy = 0; dy < p.taps_h; ++dy) {
+        for (int cc = 0; cc < p.cin_chunks; ++cc) {
+          if (p.rowshare) {
+            a_ring.wait_empty();
+            if (ptx::elect_one()) {
+              const uint32_t a0 = sA + a_ring.slot * a_stride;
+              ptx::mbar_expect_tx(a_ring.full_bar(), a_tx);
+              const int c0 = c_base + cc * kBlockK, h = h0 + dy * p.dil_h;
+              ptx::tma_load_4d(a0, mapA, a_ring.full_bar(), c0, w0, h, n0);
+              if (FAT) ptx::tma_load_4d(a0 + p.a_plane, tmA_lo, a_ring.full_bar(), c0, w0, h, n0);
+            }
+            __syncwarp();
+            a_ring.advance();
+          }
+          for (int dx = 0; dx < p.taps_w; ++dx) {
+            const int kcol = ((dy * p.taps_w + dx) * p.cin_chunks + cc) * kBlockK;
+            ring.wait_empty();
+            if (ptx::elect_one()) {
+              const uint32_t a0 = sA + ring.slot * a_stride, b0 = sB + ring.slot * b_stride;
+              ptx::mbar_expect_tx(ring.full_bar(), stage_tx);
+              ptx::tma_load_2d(b0, mapB, ring.full_bar(), kcol, t.n_tile * BLOCK_N);
+              if (FAT) ptx::tma_load_2d(b0 + kBBytes, tmB_lo, ring.full_bar(), kcol, t.n_tile * BLOCK_N);
+              if (!p.rowshare) {
+                const int c0 = c_base + cc * kBlockK, w = w0 + dx * p.dil_w, h = h0 + dy * p.dil_h;
+                ptx::tma_load_4d(a0, mapA, ring.full_bar(), c0, w, h, n0);
+                if (FAT) ptx::tma_load_4d(a0 + p.a_plane, tmA_lo, ring.full_bar(), c0, w, h, n0);
+              }
+            }
+            __syncwarp();
+            ring.advance();
+          }
+        }
+      }
+    }
+  }
+}
+
+// The num_kb k-blocks of one tile on one MMA warpgroup, from the rings in the producer's order; the tile's first K step
+// overwrites `acc`.  The warpgroup's rows start a_row_off bytes into the A tile, and tap dx a further dx a_dx_step bytes.
+// On return every MMA has completed and every stage is handed back (the warpgroup's leader arrives).
+template <int BLOCK_N, bool FAT>
+__device__ __forceinline__ void mma_tile(const IgemmParams& p, uint32_t sA, uint32_t a_stride, uint32_t sB,
+                                         uint32_t b_stride, ptx::Ring& ring, ptx::Ring& a_ring, int num_kb,
+                                         uint32_t a_row_off, uint32_t a_dx_step, bool wg_leader,
+                                         float (&acc)[BLOCK_N / 2]) {
+  constexpr uint32_t kBBytes = BLOCK_N * kBlockK * 2;
+  // the MMAs of a k-block may still read its stage (and A slot) until the next k-block's wgmma_wait<1>
+  auto release_held = [&] {
+    ring.release_held(wg_leader);
+    a_ring.release_held(wg_leader);
+  };
+  int dx = 0;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    // operands first, then the fence: between wgmma.fence and the MMAs nothing but the MMAs is issued
+    const uint32_t a0 = sA + (p.rowshare ? a_ring.slot : ring.slot) * a_stride + a_row_off + dx * a_dx_step;
+    const uint32_t b0 = sB + ring.slot * b_stride;
+    const uint64_t ah = ptx::gmma_desc_sw128(a0), bh = ptx::gmma_desc_sw128(b0);
+    const uint64_t al = ptx::gmma_desc_sw128(a0 + p.a_plane), bl = ptx::gmma_desc_sw128(b0 + kBBytes);
+    const uint32_t accumulate = kb != 0 ? 1u : 0u;  // the tile's first K step overwrites the accumulators
+    if (p.rowshare && dx == 0) a_ring.wait_full();
+    ring.wait_full();
+    ptx::fence_regs(acc);  // keep the accumulators in place across the asynchronous MMAs
+    ptx::wgmma_fence();
+    if constexpr (FAT) {
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k) {
+        ptx::wgmma_bf16<BLOCK_N>(acc, ah + 2u * k, bl + 2u * k, k != 0 ? 1u : accumulate);
+        ptx::wgmma_bf16<BLOCK_N>(acc, al + 2u * k, bh + 2u * k, 1u);
+        ptx::wgmma_bf16<BLOCK_N>(acc, ah + 2u * k, bh + 2u * k, 1u);
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k)
+        // +32 B per K step inside the 128 B swizzle atom -> +2 in the address field
+        ptx::wgmma_bf16<BLOCK_N>(acc, ah + 2u * k, bh + 2u * k, k != 0 ? 1u : accumulate);
+    }
+    ptx::wgmma_commit();
+    ptx::fence_regs(acc);
+    // the previous k-block's MMAs have finished reading their stage: hand it back to the producer
+    ptx::wgmma_wait<1>();
+    release_held();
+    ring.hold_and_advance();
+    // k-blocks run (term, dy, chunk, dx) with dx innermost: after the last dx the A slot is done with
+    if (++dx == p.taps_w) {
+      dx = 0;
+      if (p.rowshare) a_ring.hold_and_advance();
+    }
+  }
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(acc);
+  release_held();
+}
+
+// Fused PoolingLayer (MAX, 2x2, stride 2; pooling_layer.cpp:128-187) of the staged 64-channel chunk at `buf` into the
+// pooled staging tile at `pbuf` ([hi][lo], kPoolBytes apart): exactly what pool_kernel would compute from the stored
+// planes (value = hi + lo).  et: the thread's index among the kEpiThreads epilogue threads; hw_box = box_w box_h.
+__device__ __forceinline__ void pool_staged_chunk(const IgemmParams& p, uint32_t buf, uint32_t pbuf, int et,
+                                                  int hw_box) {
+  const uint32_t lo_plane = kABytes;
+  const int pw_box = p.box_w >> 1, phw_box = pw_box * (p.box_h >> 1);
+  const int prows = phw_box * p.box_n;  // <= 32
+  for (int item = et; item < prows * 8; item += kEpiThreads) {
+    const int pr = item >> 3, j = item & 7;
+    const int dn = pr / phw_box, rem = pr - dn * phw_box;
+    const int ph = rem / pw_box, pwi = rem - ph * pw_box;
+    const int r00 = dn * hw_box + (2 * ph) * p.box_w + 2 * pwi;
+    float best[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) best[e] = -3.402823466e+38f;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const int r = r00 + (c >> 1) * p.box_w + (c & 1);
+      const uint32_t a = buf + r * 128 + static_cast<uint32_t>((j ^ (r & 7)) << 4);
+      uint32_t xh[4], xl[4] = {0u, 0u, 0u, 0u};
+      ptx::ld_shared_v4(a, xh);
+      if (p.has_lo_out) ptx::ld_shared_v4(a + lo_plane, xl);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float v0 = __uint_as_float(xh[q] << 16) + __uint_as_float(xl[q] << 16);
+        const float v1 = __uint_as_float(xh[q] & 0xFFFF0000u) + __uint_as_float(xl[q] & 0xFFFF0000u);
+        best[2 * q] = (v0 > best[2 * q]) ? v0 : best[2 * q];
+        best[2 * q + 1] = (v1 > best[2 * q + 1]) ? v1 : best[2 * q + 1];
+      }
+    }
+    uint32_t oh[4], ol[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      oh[q] = ptx::pack_bf16x2(best[2 * q], best[2 * q + 1]);
+      ol[q] = ptx::pack_bf16x2(best[2 * q] - __uint_as_float(oh[q] << 16),
+                               best[2 * q + 1] - __uint_as_float(oh[q] & 0xFFFF0000u));
+    }
+    const uint32_t pa = pbuf + pr * 128 + static_cast<uint32_t>((j ^ (pr & 7)) << 4);
+    ptx::st_shared_v4(pa, oh);
+    if (p.has_lo_out) ptx::st_shared_v4(pa + kPoolBytes, ol);
+  }
+}
+
 // FAT is a template parameter, not a runtime branch: with both MMA sequences in one body the accumulator registers
 // cross a divergent region and ptxas has to insert extra warpgroup.arrive synchronisation before the MMAs.
 template <int BLOCK_N, bool FAT>
@@ -170,75 +345,19 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
   }
   const int m_tiles = p.tiles_w * p.tiles_h * tiles_n;
   const int total_tiles = m_tiles * p.n_tiles;
-  const int terms = FAT ? 1 : p.num_terms;
+  const int terms = FAT ? 1 : p.num_terms;  // a fat stage carries all three products of its k-block
   const int num_kb = terms * p.taps_h * p.taps_w * p.cin_chunks;
 
-  // M tile -> pixel-box origin
-  auto m_coords = [&](int m, int& tw, int& th, int& tn) {
-    tw = m % p.tiles_w;
-    m /= p.tiles_w;
-    th = m % p.tiles_h;
-    tn = m / p.tiles_h;
-  };
-
   if (warp < 4) {
-    // ------------------------------------------------------------ TMA producer
+    // TMA producer: one warp issues, the others hand their registers to the MMA warpgroups
     ptx::setmaxnreg_dec<40>();
-    if (warp != 0) return;
-    // The whole warp walks the loops (warp-uniform control flow); one elected lane issues.  Row-share fetches the
-    // activation rows of one (term, dy, channel chunk) ONCE, with a one-pixel halo on each side ({64, box_w + 2, box_h,
-    // 1} from column w0 - pad: TMA zero fill is still the padding), for the taps dx = 0, 1, 2; each stage then carries
-    // only the weight tiles.  Without row-share each stage carries the tap's shifted activation tile as well.
-    const uint32_t a_tx = kPlanes * static_cast<uint32_t>((p.box_w + (p.rowshare ? 2 : 0)) * p.box_h * p.box_n) * kBlockK * 2;
-    const uint32_t stage_tx = kPlanes * kBBytes + (p.rowshare ? 0u : a_tx);
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int n_tile = tile % p.n_tiles;
-      int tw, th, tn;
-      m_coords(tile / p.n_tiles, tw, th, tn);
-      const int w0 = tw * p.box_w * p.stride_w - p.pad_w, h0 = th * p.box_h * p.stride_h - p.pad_h, n0 = tn * p.box_n;
-      const int c_base = n_tile * BLOCK_N / p.cout_g * p.cin_g;  // first input channel of the tile's group
-      for (int term = 0; term < terms; ++term) {
-        const CUtensorMap* mapA = (term == 2) ? &tmA_lo : &tmA_hi;
-        const CUtensorMap* mapB = (term == 1) ? &tmB_lo : &tmB_hi;
-        for (int dy = 0; dy < p.taps_h; ++dy) {
-          for (int cc = 0; cc < p.cin_chunks; ++cc) {
-            if (p.rowshare) {
-              a_ring.wait_empty();
-              if (ptx::elect_one()) {
-                const uint32_t a0 = sA + a_ring.slot * a_stride;
-                ptx::mbar_expect_tx(a_ring.full_bar(), a_tx);
-                const int c0 = c_base + cc * kBlockK, h = h0 + dy * p.dil_h;
-                ptx::tma_load_4d(a0, mapA, a_ring.full_bar(), c0, w0, h, n0);
-                if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, a_ring.full_bar(), c0, w0, h, n0);
-              }
-              __syncwarp();
-              a_ring.advance();
-            }
-            for (int dx = 0; dx < p.taps_w; ++dx) {
-              const int kcol = ((dy * p.taps_w + dx) * p.cin_chunks + cc) * kBlockK;
-              ring.wait_empty();
-              if (ptx::elect_one()) {
-                const uint32_t a0 = sA + ring.slot * a_stride, b0 = sB + ring.slot * b_stride;
-                ptx::mbar_expect_tx(ring.full_bar(), stage_tx);
-                ptx::tma_load_2d(b0, mapB, ring.full_bar(), kcol, n_tile * BLOCK_N);
-                if (FAT) ptx::tma_load_2d(b0 + kBBytes, &tmB_lo, ring.full_bar(), kcol, n_tile * BLOCK_N);
-                if (!p.rowshare) {
-                  const int c0 = c_base + cc * kBlockK, w = w0 + dx * p.dil_w, h = h0 + dy * p.dil_h;
-                  ptx::tma_load_4d(a0, mapA, ring.full_bar(), c0, w, h, n0);
-                  if (FAT) ptx::tma_load_4d(a0 + p.a_plane, &tmA_lo, ring.full_bar(), c0, w, h, n0);
-                }
-              }
-              __syncwarp();
-              ring.advance();
-            }
-          }
-        }
-      }
-    }
+    if (warp == 0)
+      produce_tiles<BLOCK_N, FAT>(p, &tmA_hi, &tmA_lo, &tmB_hi, &tmB_lo, sA, a_stride, sB, b_stride, ring, a_ring, terms,
+                                  total_tiles);
     return;
   }
 
-  // ------------------------------------------------------------------ MMA warpgroups + epilogue
+  // MMA warpgroups + epilogue
   ptx::setmaxnreg_inc<232>();
   const int et = threadIdx.x - 128;          // 0..255
   const int wg = et >> 7;                    // rows [64 wg, 64 wg + 64) of the M tile
@@ -254,58 +373,13 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
   const int box_rows = hw_box * p.box_n;
   int ebuf = 0;
   float acc[kAcc];
-  // the MMAs of a k-block may still read its stage (and A slot) until the next k-block's wgmma_wait<1>
-  auto release_held = [&] {
-    ring.release_held(wg_leader);
-    a_ring.release_held(wg_leader);
-  };
 
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int n_tile = tile % p.n_tiles;
-    const int n_base = n_tile * BLOCK_N;
-    int dx = 0;
-    for (int kb = 0; kb < num_kb; ++kb) {
-      // operands first, then the fence: between wgmma.fence and the MMAs nothing but the MMAs is issued
-      const uint32_t a0 = sA + (p.rowshare ? a_ring.slot : ring.slot) * a_stride + a_row_off + dx * a_dx_step;
-      const uint32_t b0 = sB + ring.slot * b_stride;
-      const uint64_t ah = ptx::gmma_desc_sw128(a0), bh = ptx::gmma_desc_sw128(b0);
-      const uint64_t al = ptx::gmma_desc_sw128(a0 + p.a_plane), bl = ptx::gmma_desc_sw128(b0 + kBBytes);
-      const uint32_t accumulate = kb != 0 ? 1u : 0u;  // the tile's first K step overwrites the accumulators
-      if (p.rowshare && dx == 0) a_ring.wait_full();
-      ring.wait_full();
-      ptx::fence_regs(acc);  // keep the accumulators in place across the asynchronous MMAs
-      ptx::wgmma_fence();
-      if constexpr (FAT) {
-#pragma unroll
-        for (int k = 0; k < kBlockK / 16; ++k) {
-          ptx::wgmma_bf16<BLOCK_N>(acc, ah + 2u * k, bl + 2u * k, k != 0 ? 1u : accumulate);
-          ptx::wgmma_bf16<BLOCK_N>(acc, al + 2u * k, bh + 2u * k, 1u);
-          ptx::wgmma_bf16<BLOCK_N>(acc, ah + 2u * k, bh + 2u * k, 1u);
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < kBlockK / 16; ++k)
-          // +32 B per K step inside the 128 B swizzle atom -> +2 in the address field
-          ptx::wgmma_bf16<BLOCK_N>(acc, ah + 2u * k, bh + 2u * k, k != 0 ? 1u : accumulate);
-      }
-      ptx::wgmma_commit();
-      ptx::fence_regs(acc);
-      // the previous k-block's MMAs have finished reading their stage: hand it back to the producer
-      ptx::wgmma_wait<1>();
-      release_held();
-      ring.hold_and_advance();
-      // k-blocks run (term, dy, chunk, dx) with dx innermost: after the last dx the A slot is done with
-      if (++dx == p.taps_w) {
-        dx = 0;
-        if (p.rowshare) a_ring.hold_and_advance();
-      }
-    }
-    ptx::wgmma_wait<0>();
-    ptx::fence_regs(acc);
-    release_held();
-
-    int tw, th, tn;
-    m_coords(tile / p.n_tiles, tw, th, tn);
+    // The first output channel before the k-block loop, the pixel box after it: the instruction schedule depends on
+    // where these divisions are issued.
+    const int n_base = tile % p.n_tiles * BLOCK_N;
+    mma_tile<BLOCK_N, FAT>(p, sA, a_stride, sB, b_stride, ring, a_ring, num_kb, a_row_off, a_dx_step, wg_leader, acc);
+    const TileCoord t = tile_coord(p, tile);
     if (p.out_mode == MSCNN_OUT_NHWC_BF16) {
       if constexpr (BLOCK_N >= 64) {
         const uint32_t lo_plane = kABytes;
@@ -329,51 +403,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
           }
           const uint32_t pbuf = buf + kABytes * (p.has_lo_out ? 2 : 1);  // pooled staging [hi][lo]
           if (p.pool) {
-            // Fused PoolingLayer (MAX, 2x2, stride 2; pooling_layer.cpp:128-187) on the staged tile:
-            // exactly what pool_kernel would compute from the stored planes (value = hi + lo).
             ptx::named_bar_sync(kEpiBarId, kEpiThreads);
-            const int pw_box = p.box_w >> 1, phw_box = pw_box * (p.box_h >> 1);
-            const int prows = phw_box * p.box_n;  // <= 32
-            for (int item = et; item < prows * 8; item += kEpiThreads) {
-              const int pr = item >> 3, j = item & 7;
-              const int dn = pr / phw_box, rem = pr - dn * phw_box;
-              const int ph = rem / pw_box, pwi = rem - ph * pw_box;
-              const int r00 = dn * hw_box + (2 * ph) * p.box_w + 2 * pwi;
-              float best[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) best[e] = -3.402823466e+38f;
-#pragma unroll
-              for (int c = 0; c < 4; ++c) {
-                const int r = r00 + (c >> 1) * p.box_w + (c & 1);
-                const uint32_t a = buf + r * 128 + static_cast<uint32_t>((j ^ (r & 7)) << 4);
-                uint32_t xh[4], xl[4] = {0u, 0u, 0u, 0u};
-                asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                             : "=r"(xh[0]), "=r"(xh[1]), "=r"(xh[2]), "=r"(xh[3]) : "r"(a));
-                if (p.has_lo_out)
-                  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                               : "=r"(xl[0]), "=r"(xl[1]), "=r"(xl[2]), "=r"(xl[3]) : "r"(a + lo_plane));
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float v0 = __uint_as_float(xh[q] << 16) + __uint_as_float(xl[q] << 16);
-                  const float v1 = __uint_as_float(xh[q] & 0xFFFF0000u) + __uint_as_float(xl[q] & 0xFFFF0000u);
-                  best[2 * q] = (v0 > best[2 * q]) ? v0 : best[2 * q];
-                  best[2 * q + 1] = (v1 > best[2 * q + 1]) ? v1 : best[2 * q + 1];
-                }
-              }
-              uint32_t oh[4], ol[4];
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                oh[q] = ptx::pack_bf16x2(best[2 * q], best[2 * q + 1]);
-                ol[q] = ptx::pack_bf16x2(best[2 * q] - __uint_as_float(oh[q] << 16),
-                                         best[2 * q + 1] - __uint_as_float(oh[q] & 0xFFFF0000u));
-              }
-              const uint32_t pa = pbuf + pr * 128 + static_cast<uint32_t>((j ^ (pr & 7)) << 4);
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(pa), "r"(oh[0]), "r"(oh[1]),
-                           "r"(oh[2]), "r"(oh[3]) : "memory");
-              if (p.has_lo_out)
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(pa + kPoolBytes), "r"(ol[0]),
-                             "r"(ol[1]), "r"(ol[2]), "r"(ol[3]) : "memory");
-            }
+            pool_staged_chunk(p, buf, pbuf, et, hw_box);
           }
           ptx::fence_proxy_async_smem();
           ptx::named_bar_sync(kEpiBarId, kEpiThreads);
@@ -381,11 +412,11 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
             // one bulk group per staging buffer, pooled tile included
             const int c0 = n_base + chunk * 64;
             if (!p.pool || p.store_full)
-              ptx::tma_store_hi_lo(&tmO_hi, &tmO_lo, buf, p.has_lo_out, lo_plane, c0, tw * p.box_w, th * p.box_h,
-                                   tn * p.box_n);
+              ptx::tma_store_hi_lo(&tmO_hi, &tmO_lo, buf, p.has_lo_out, lo_plane, c0, t.tw * p.box_w,
+                                   t.th * p.box_h, t.tn * p.box_n);
             if (p.pool)
-              ptx::tma_store_hi_lo(&tmP_hi, &tmP_lo, pbuf, p.has_lo_out, kPoolBytes, c0, tw * (p.box_w >> 1),
-                                   th * (p.box_h >> 1), tn * p.box_n);
+              ptx::tma_store_hi_lo(&tmP_hi, &tmP_lo, pbuf, p.has_lo_out, kPoolBytes, c0, t.tw * (p.box_w >> 1),
+                                   t.th * (p.box_h >> 1), t.tn * p.box_n);
             ptx::tma_store_commit();
           }
           if (++ebuf == p.epi_bufs) ebuf = 0;
@@ -399,7 +430,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA_hi,
         const int row = r0 + 8 * h;
         const int dn = row / hw_box, rem = row - dn * hw_box;
         const int dh = rem / p.box_w, dw = rem - dh * p.box_w;
-        const int n = tn * p.box_n + dn, y = th * p.box_h + dh, x = tw * p.box_w + dw;
+        const int n = t.tn * p.box_n + dn, y = t.th * p.box_h + dh, x = t.tw * p.box_w + dw;
         const bool ok = row < box_rows && n < p.out_n && y < p.out_h && x < p.out_w;
         if (!ok) continue;
         // NCHW: lanes of one quad are consecutive channels of one pixel
@@ -466,33 +497,15 @@ static void pick_box(int N, int Ho, int Wo, bool even, int stride_h, int stride_
 constexpr int kSmemBudget = 227 * 1024;
 constexpr int kMaxDevices = 64;
 
-// cudaFuncAttributeMaxDynamicSharedMemorySize is per device and function: raised once to the whole budget.
-template <typename K>
-static cudaError_t raise_smem_once(K kern, bool (&done)[kMaxDevices], int device) {
-  if (device >= 0 && device < kMaxDevices && done[device]) return cudaSuccess;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
-  if (e == cudaSuccess && device >= 0 && device < kMaxDevices) done[device] = true;
-  return e;
-}
-
-template <int BLOCK_N, bool FAT>
-static cudaError_t launch_igemm(const CUtensorMap maps[8], const IgemmParams& p, int grid,
-                                size_t smem, int device, cudaStream_t stream) {
-  auto kern = conv_igemm_kernel<BLOCK_N, FAT>;
-  static bool done[kMaxDevices];
-  cudaError_t e = raise_smem_once(kern, done, device);
-  if (e != cudaSuccess) return e;
-  mscnn::note_launch();
-  kern<<<grid, kThreads, smem, stream>>>(maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], maps[6], maps[7], p);
-  return cudaGetLastError();
-}
+// The kernel's tensor-map arguments, in order (P: the fused pooling output).
+enum MapSlot { kMapAHi, kMapALo, kMapBHi, kMapBLo, kMapOHi, kMapOLo, kMapPHi, kMapPLo, kNumMaps };
 
 // A launch plan: everything mscnn_conv_forward derives from a descriptor (tile shapes, ring sizes, the eight tensor
 // maps).  Plans are cached per (descriptor, device, config epoch): a steady-state forward does one hash lookup per
 // convolution instead of a few getenv() and up to 8 cuTensorMapEncodeTiled calls (27 convolutions per step).
 struct ConvPlan {
   IgemmParams p;
-  CUtensorMap maps[8];
+  CUtensorMap maps[kNumMaps];
   int grid;
   int BN;
   size_t smem;
@@ -504,90 +517,6 @@ struct ConvPlan {
 struct OutView {
   int ho, wo, step_h, step_w, r_h, r_w, full_h, full_w;
 };
-
-struct PlanKey {
-  const void* ptr[11];
-  int v[28];
-  bool operator==(const PlanKey& o) const { return memcmp(this, &o, sizeof(PlanKey)) == 0; }
-};
-struct PlanKeyHash {
-  size_t operator()(const PlanKey& k) const {
-    const unsigned char* b = reinterpret_cast<const unsigned char*>(&k);
-    uint64_t h = 1469598103934665603ull;  // FNV-1a
-    for (size_t i = 0; i < sizeof(PlanKey); ++i) h = (h ^ b[i]) * 1099511628211ull;
-    return static_cast<size_t>(h);
-  }
-};
-static std::mutex g_plan_mu;
-static std::unordered_map<PlanKey, ConvPlan, PlanKeyHash> g_plans;
-
-void conv_plan_cache_clear() {
-  std::lock_guard<std::mutex> lk(g_plan_mu);
-  g_plans.clear();
-}
-
-static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps = true,
-                      const OutView* view = nullptr);
-
-// The cached launch plan of (d, view), built and cached on a miss.
-static int resolve_plan(const mscnn_conv_desc* d, const OutView* view, int device, ConvPlan* plan) {
-  PlanKey key;
-  memset(&key, 0, sizeof(key));
-  const void* ptrs[11] = {d->x_hi, d->x_lo, d->w_hi, d->w_lo, d->bias, d->y_hi, d->y_lo, d->y_f32, d->pool_hi, d->pool_lo, d->dyn_n};
-  memcpy(key.ptr, ptrs, sizeof(ptrs));
-  const OutView dense = {0, 0, 0, 0, 0, 0, 0, 0};
-  const OutView& v = view ? *view : dense;
-  const int vals[28] = {d->N, d->H, d->W, d->C, d->Cout, d->Cout_pad, d->KH, d->KW, d->pad_h, d->pad_w, d->relu,
-                        d->out_mode, device, static_cast<int>(config().epoch), 0,
-                        d->stride_h, d->stride_w, d->dil_h, d->dil_w, d->group,
-                        v.ho, v.wo, v.step_h, v.step_w, v.r_h, v.r_w, v.full_h, v.full_w};
-  memcpy(key.v, vals, sizeof(vals));
-  {
-    std::lock_guard<std::mutex> lk(g_plan_mu);
-    auto it = g_plans.find(key);
-    if (it != g_plans.end()) {
-      *plan = it->second;
-      return MSCNN_OK;
-    }
-  }
-  const int rc = build_plan(d, plan, true, view);
-  if (rc != MSCNN_OK) return rc;
-  std::lock_guard<std::mutex> lk(g_plan_mu);
-  if (g_plans.size() >= 4096) g_plans.clear();  // blobs that keep moving (re-allocation): bound the table
-  g_plans.emplace(key, *plan);
-  return MSCNN_OK;
-}
-
-static int launch_plan(const ConvPlan& plan, int device, cudaStream_t stream, const char* who) {
-  // [BLOCK_N = 32 << i][fat]; fat stages only below BLOCK_N = 256 (build_plan): no <256, true> instantiation
-  static const decltype(&launch_igemm<32, false>) launch[4][2] = {
-      {launch_igemm<32, false>, launch_igemm<32, true>}, {launch_igemm<64, false>, launch_igemm<64, true>},
-      {launch_igemm<128, false>, launch_igemm<128, true>}, {launch_igemm<256, false>, nullptr}};
-  const cudaError_t e =
-      launch[__builtin_ctz(plan.BN) - 5][plan.p.fat](plan.maps, plan.p, plan.grid, plan.smem, device, stream);
-  if (e != cudaSuccess) {
-    fprintf(stderr, "%s: launch failed: %s\n", who, cudaGetErrorString(e));
-    return MSCNN_ERR_CUDA;
-  }
-  return MSCNN_OK;
-}
-
-}  // namespace mscnn
-
-using namespace mscnn;
-
-extern "C" int mscnn_conv_forward(const mscnn_conv_desc* d, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!d) return MSCNN_ERR_INVALID;
-  int device = 0;
-  if (cudaGetDevice(&device) != cudaSuccess) return MSCNN_ERR_CUDA;
-  ConvPlan plan;
-  const int rc = resolve_plan(d, nullptr, device, &plan);
-  if (rc != MSCNN_OK) return rc;
-  return launch_plan(plan, device, stream, "mscnn_conv_forward");
-}
-
-namespace mscnn {
 
 // The deepest B ring, up to kMaxStages, whose layout fits the shared-memory budget (0 if none does).
 static int deepest_ring(IgemmParams p, int block_n) {
@@ -625,10 +554,19 @@ static int unsupported(const mscnn_conv_desc* d, const char* rule) {
   return MSCNN_ERR_INVALID;
 }
 
-// view != NULL (a deconvolution phase): the output extents are the view's, the pad may be negative (the extents are
-// not derived from it), and only NHWC_BF16 planes without pooling or dyn_n are written.
-static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps, const OutView* view) {
-  const Config& cfg = config();
+// What a served descriptor implies before any plan choice: strides, dilations and group (0 read as 1), the output
+// extents, the channels of one group, the instantiation's BLOCK_N, and which operands and outputs the launch has.
+struct ConvShape {
+  int sh, sw, dh, dw, g, Ho, Wo, cin_g, cout_g, BN;
+  bool split;   // fp32-faithful operands (x_lo, w_lo)
+  bool pool;    // fused 2x2 pooling output
+  bool staged;  // NHWC bf16 planes, written through shared-memory staging
+};
+
+// Plan step 1: check the descriptor and derive its shape.  view != NULL (a deconvolution phase): the output extents are
+// the view's, the pad may be negative (the extents are not derived from it), and only NHWC_BF16 planes without pooling
+// or dyn_n are written.
+static int conv_shape(const mscnn_conv_desc* d, const OutView* view, ConvShape* s) {
   if (!d->x_hi || !d->w_hi || !d->bias) return MSCNN_ERR_INVALID;
   if (d->C % 64 != 0) return MSCNN_ERR_INVALID;
   const bool split = (d->x_lo != nullptr);
@@ -651,58 +589,70 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
   const int cin_g = d->C / g, cout_g = d->Cout_pad / g;
   const int BN = pick_block_n(cout_g);
   if (d->Cout_pad % BN != 0 || d->Cout > d->Cout_pad) return MSCNN_ERR_INVALID;
-  const bool pool = (d->out_mode == MSCNN_OUT_NHWC_BF16 && d->pool_hi != nullptr);
-  if (d->out_mode == MSCNN_OUT_NHWC_BF16 && (BN < 64 || (!d->y_hi && !pool))) return MSCNN_ERR_INVALID;
+  const bool staged = d->out_mode == MSCNN_OUT_NHWC_BF16;
+  const bool pool = (staged && d->pool_hi != nullptr);
+  if (staged && (BN < 64 || (!d->y_hi && !pool))) return MSCNN_ERR_INVALID;
   if (pool && ((Ho & 1) || (Wo & 1))) return MSCNN_ERR_INVALID;  // fused pooling: even output extents only
   if ((d->out_mode == MSCNN_OUT_NCHW_F32 || d->out_mode == MSCNN_OUT_NHWC_F32) && !d->y_f32) return MSCNN_ERR_INVALID;
+  // a lo plane is written for every staged output or none
+  const bool lo_out = staged && (d->y_lo != nullptr || (pool && d->pool_lo != nullptr));
+  if (pool && d->y_hi && lo_out && !d->y_lo) return MSCNN_ERR_INVALID;
+  if (pool && lo_out && !d->pool_lo) return MSCNN_ERR_INVALID;
+  *s = {sh, sw, dh, dw, g, Ho, Wo, cin_g, cout_g, BN, split, pool, staged};
+  return MSCNN_OK;
+}
 
-  IgemmParams& p = plan->p;
+// Plan step 2: the kernel parameters of the geometry, tiles and outputs; staging is left to stage_operands.
+static IgemmParams igemm_params(const mscnn_conv_desc* d, const ConvShape& s) {
+  IgemmParams p;
   memset(&p, 0, sizeof(p));
-  p.num_terms = split ? 3 : 1;
+  p.num_terms = s.split ? 3 : 1;
   p.taps_h = d->KH;
   p.taps_w = d->KW;
   p.pad_h = d->pad_h;
   p.pad_w = d->pad_w;
-  p.stride_h = sh;
-  p.stride_w = sw;
-  p.dil_h = dh;
-  p.dil_w = dw;
-  p.cin_g = cin_g;
-  p.cout_g = cout_g;
-  p.cin_chunks = cin_g / 64;
-  pick_box(d->N, Ho, Wo, pool, sh, sw, &p.box_w, &p.box_h, &p.box_n);
-  p.tiles_w = (Wo + p.box_w - 1) / p.box_w;
-  p.tiles_h = (Ho + p.box_h - 1) / p.box_h;
+  p.stride_h = s.sh;
+  p.stride_w = s.sw;
+  p.dil_h = s.dh;
+  p.dil_w = s.dw;
+  p.cin_g = s.cin_g;
+  p.cout_g = s.cout_g;
+  p.cin_chunks = s.cin_g / 64;
+  pick_box(d->N, s.Ho, s.Wo, s.pool, s.sh, s.sw, &p.box_w, &p.box_h, &p.box_n);
+  p.tiles_w = (s.Wo + p.box_w - 1) / p.box_w;
+  p.tiles_h = (s.Ho + p.box_h - 1) / p.box_h;
   p.tiles_n = (d->N + p.box_n - 1) / p.box_n;
-  p.n_tiles = d->Cout_pad / BN;
+  p.n_tiles = d->Cout_pad / s.BN;
   p.relu = d->relu;
   p.out_mode = d->out_mode;
-  p.has_lo_out = (d->out_mode == MSCNN_OUT_NHWC_BF16 && (d->y_lo != nullptr || (pool && d->pool_lo != nullptr))) ? 1 : 0;
-  p.pool = pool ? 1 : 0;
+  p.has_lo_out = (s.staged && (d->y_lo != nullptr || (s.pool && d->pool_lo != nullptr))) ? 1 : 0;
+  p.pool = s.pool ? 1 : 0;
   p.store_full = (d->y_hi != nullptr) ? 1 : 0;
-  if (pool && p.store_full && p.has_lo_out && !d->y_lo) return MSCNN_ERR_INVALID;
-  if (pool && p.has_lo_out && !d->pool_lo) return MSCNN_ERR_INVALID;
   p.bias = d->bias;
   p.dyn_n = d->dyn_n;
   p.out_f32 = d->y_f32;
   p.out_n = d->N;
   p.out_c = d->Cout;
-  p.out_h = Ho;
-  p.out_w = Wo;
+  p.out_h = s.Ho;
+  p.out_w = s.Wo;
   p.out_ld = d->Cout_pad;
+  return p;
+}
 
+// Plan step 3: operand staging and ring depths.
+static int stage_operands(const mscnn_conv_desc* d, const ConvShape& s, IgemmParams& p) {
+  const Config& cfg = config();
   // Fat stages (A_hi, A_lo, B_hi, B_lo of a k-block in one stage, three MMAs per K step) for the narrow-N layers of
   // the fp32-faithful path: A_hi / B_hi are fetched once instead of twice and a barrier round trip covers 3x the MMAs.
   // BLOCK_N = 256 keeps single tiles: a fat stage would be 96 KB.  The choice depends on the layer alone (not on
   // pooling), so that fused and unfused launches of a layer sum in the same order.
-  const int planes = (split && BN <= 128 && !cfg.no_fat) ? 2 : 1;
-  const bool staged = d->out_mode == MSCNN_OUT_NHWC_BF16;  // fp32 outputs carve no staging region
+  const int planes = (s.split && s.BN <= 128 && !cfg.no_fat) ? 2 : 1;
   p.fat = planes == 2;
   p.a_slot = kABytes * planes;
   p.a_plane = kABytes;
   p.a_wg_row = 64;
-  p.epi_bufs = staged ? 2 : 0;
-  fit_rings(p, BN);
+  p.epi_bufs = s.staged ? 2 : 0;  // fp32 outputs carve no staging region
+  fit_rings(p, s.BN);
   if (p.stages < 2) return MSCNN_ERR_INVALID;
 
   // Row-share (3 horizontal taps, one image row per MMA warpgroup: 64x2 and 128x1 boxes, BLOCK_N <= 128).  The three
@@ -712,7 +662,7 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
   // has to be at least as deep (in taps) as the per-tap ring it replaces, else the per-tap plan stays.  The haloed
   // row serves neighbouring taps only when they are neighbouring columns: stride and dilation 1 in W.
   const bool rs_box = p.box_n == 1 && ((p.box_w == 64 && p.box_h == 2) || (p.box_w == 128 && p.box_h == 1));
-  if (!cfg.no_rowshare && d->KW == 3 && sw == 1 && dw == 1 && BN <= 128 && rs_box) {
+  if (!cfg.no_rowshare && d->KW == 3 && s.sw == 1 && s.dw == 1 && s.BN <= 128 && rs_box) {
     IgemmParams rs = p;
     rs.rowshare = 1;
     rs.a_stages = 2;
@@ -720,75 +670,91 @@ static int build_plan(const mscnn_conv_desc* d, ConvPlan* plan, bool encode_maps
     rs.a_slot = rs.a_plane * planes;
     rs.a_wg_row = 64 / p.box_w * (p.box_w + 2) + 64 % p.box_w;  // halo-tile row of output pixel 64
     // a second epilogue buffer only overlaps the two 64-channel chunks of a BLOCK_N = 128 tile
-    rs.epi_bufs = staged ? (BN > 64 ? 2 : 1) : 0;
-    fit_rings(rs, BN);
+    rs.epi_bufs = s.staged ? (s.BN > 64 ? 2 : 1) : 0;
+    fit_rings(rs, s.BN);
     if (rs.stages >= p.stages) p = rs;
   }
-  const size_t smem = igemm_layout(p, BN).total;
-  const int total_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_tiles;
-  if (cfg.verbose_conv)
-    fprintf(stderr, "conv plan: N=%d H=%d W=%d C=%d Cout_pad=%d k=%dx%d BN=%d box=%dx%dx%d fat=%d terms=%d rowshare=%d a_stages=%d stages=%d epi_bufs=%d smem=%zu tiles=%d\n",
-            d->N, d->H, d->W, d->C, d->Cout_pad, d->KH, d->KW, BN, p.box_w, p.box_h, p.box_n, p.fat, p.num_terms,
-            p.rowshare, p.a_stages, p.stages, p.epi_bufs, smem, total_tiles);
+  return MSCNN_OK;
+}
 
-  plan->BN = BN;
-  plan->smem = smem;
-  CUtensorMap* maps = plan->maps;
-  memset(maps, 0, sizeof(plan->maps));
-  if (!encode_maps) {  // mscnn_conv_plan_describe: the shape decisions only, no driver call
-    plan->grid = 0;
-    return MSCNN_OK;
-  }
-  // The kernel's maps A_hi, A_lo, B_hi, B_lo, O_hi, O_lo, P_hi, P_lo (P: fused pooling output).  One the launch does
-  // not use is a copy of its primary (a lo plane of its hi plane, a hi plane of A_hi), so every argument is valid.
-  const bool lo_out = staged && p.has_lo_out;
-  // a view starts at pixel (r_h, r_w) of the full planes and steps (step_h, step_w) pixels: every byte stride is a
-  // multiple of Cout_pad * 2 = 128 B
+// Plan step 4: the eight tensor maps.  A map the launch does not use is a copy of its primary (a lo plane of its hi
+// plane, a hi plane of A_hi), so every kernel argument is a valid map.
+static int encode_maps(const mscnn_conv_desc* d, const OutView* view, const ConvShape& s, const IgemmParams& p,
+                       CUtensorMap (&maps)[kNumMaps]) {
+  const uint64_t N = (uint64_t)d->N, Ho = (uint64_t)s.Ho, Wo = (uint64_t)s.Wo, cout_pad = (uint64_t)d->Cout_pad;
+  // activation: with element strides TMA loads ceil(box / stride) = box_w (+ the row-share halo) x box_h pixels of a
+  // box given in image pixels
+  const uint64_t act_dims[4] = {(uint64_t)d->C, (uint64_t)d->W, (uint64_t)d->H, N};
+  const uint32_t act_box[4] = {64u, (uint32_t)((p.box_w + (p.rowshare ? 2 : 0)) * s.sw), (uint32_t)(p.box_h * s.sh),
+                               (uint32_t)p.box_n};
+  const uint32_t act_strides[4] = {1u, (uint32_t)s.sw, (uint32_t)s.sh, 1u};
+  auto activation = [&](CUtensorMap* m, const void* x) { return tmap_nhwc_bf16(m, x, act_dims, act_box, act_strides); };
+  // weights: K-major [Cout_pad][taps x channels of one group]
+  auto weights = [&](CUtensorMap* m, const void* w) {
+    return tmap_2d_bf16(m, w, (uint64_t)d->KH * d->KW * s.cin_g, cout_pad, 64u, (uint32_t)s.BN);
+  };
+  // output: a view starts at pixel (r_h, r_w) of the full planes and steps (step_h, step_w) pixels: every byte stride
+  // is a multiple of Cout_pad * 2 = 128 B
   const size_t pix = (size_t)d->Cout_pad * 2;
   const size_t view_off = view ? ((size_t)view->r_h * view->full_w + view->r_w) * pix : 0;
   const uint64_t view_strides[3] = {view ? view->step_w * pix : 0, view ? (size_t)view->step_h * view->full_w * pix : 0,
                                     view ? (size_t)view->full_h * view->full_w * pix : 0};
-  void* y_hi = d->y_hi ? static_cast<uint8_t*>(d->y_hi) + view_off : nullptr;
-  void* y_lo = d->y_lo ? static_cast<uint8_t*>(d->y_lo) + view_off : nullptr;
-  const void* src[8] = {d->x_hi, split ? d->x_lo : nullptr, d->w_hi, split ? d->w_lo : nullptr,
-                        staged ? y_hi : nullptr, lo_out ? y_lo : nullptr,
-                        p.pool ? d->pool_hi : nullptr, p.pool && lo_out ? d->pool_lo : nullptr};
-  const uint64_t dims[4][4] = {{(uint64_t)d->C, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->N},
-                               {},
-                               {(uint64_t)d->Cout_pad, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)d->N},
-                               {(uint64_t)d->Cout_pad, (uint64_t)(Wo / 2), (uint64_t)(Ho / 2), (uint64_t)d->N}};
-  // the activation box in image pixels: with element strides TMA loads ceil(box / stride) = box_w x box_h of them
-  const uint32_t boxes[4][4] = {{64u, (uint32_t)((p.box_w + (p.rowshare ? 2 : 0)) * sw), (uint32_t)(p.box_h * sh), (uint32_t)p.box_n},
-                                {},
-                                {64u, (uint32_t)p.box_w, (uint32_t)p.box_h, (uint32_t)p.box_n},
-                                {64u, (uint32_t)(p.box_w / 2), (uint32_t)(p.box_h / 2), (uint32_t)p.box_n}};
-  const uint32_t a_strides[4] = {1u, (uint32_t)sw, (uint32_t)sh, 1u};
-  for (int i = 0; i < 8; ++i) {
-    if (!src[i]) {
-      maps[i] = maps[(i & 1) ? i - 1 : 0];
-      continue;
-    }
-    const int rc = (i >> 1) == 1
-                       ? tmap_2d_bf16(&maps[i], src[i], (uint64_t)d->KH * d->KW * cin_g, (uint64_t)d->Cout_pad, 64u, (uint32_t)BN)
-                       : tmap_nhwc_bf16(&maps[i], src[i], dims[i >> 1], boxes[i >> 1], (i >> 1) == 0 ? a_strides : nullptr,
-                                        (i >> 1) == 2 && view ? view_strides : nullptr);
-    if (rc) return rc;
-  }
+  const uint64_t out_dims[4] = {cout_pad, Wo, Ho, N};
+  const uint32_t out_box[4] = {64u, (uint32_t)p.box_w, (uint32_t)p.box_h, (uint32_t)p.box_n};
+  auto output = [&](CUtensorMap* m, const void* y) {
+    return tmap_nhwc_bf16(m, static_cast<const uint8_t*>(y) + view_off, out_dims, out_box, nullptr,
+                          view ? view_strides : nullptr);
+  };
+  const uint64_t pool_dims[4] = {cout_pad, Wo / 2, Ho / 2, N};
+  const uint32_t pool_box[4] = {64u, (uint32_t)(p.box_w / 2), (uint32_t)(p.box_h / 2), (uint32_t)p.box_n};
+  auto pooled = [&](CUtensorMap* m, const void* y) { return tmap_nhwc_bf16(m, y, pool_dims, pool_box); };
 
-  int grid = mscnn_sm_count();
-  if (grid > total_tiles) grid = total_tiles;
-  plan->grid = grid;
+  // slot i encoded from `base`, or a copy of slot `primary` where the launch has no such operand (base NULL)
+  auto put = [&](MapSlot i, const void* base, MapSlot primary, auto encode) -> int {
+    if (!base) {
+      maps[i] = maps[primary];
+      return MSCNN_OK;
+    }
+    return encode(&maps[i], base);
+  };
+  const bool lo = p.has_lo_out;
+  int rc = put(kMapAHi, d->x_hi, kMapAHi, activation);
+  if (!rc) rc = put(kMapALo, s.split ? d->x_lo : nullptr, kMapAHi, activation);
+  if (!rc) rc = put(kMapBHi, d->w_hi, kMapAHi, weights);
+  if (!rc) rc = put(kMapBLo, s.split ? d->w_lo : nullptr, kMapBHi, weights);
+  if (!rc) rc = put(kMapOHi, s.staged ? d->y_hi : nullptr, kMapAHi, output);
+  if (!rc) rc = put(kMapOLo, lo ? d->y_lo : nullptr, kMapOHi, output);
+  if (!rc) rc = put(kMapPHi, p.pool ? d->pool_hi : nullptr, kMapAHi, pooled);
+  if (!rc) rc = put(kMapPLo, p.pool && lo ? d->pool_lo : nullptr, kMapPHi, pooled);
+  return rc;
+}
+
+// The launch plan of (d, view).  encode = false (mscnn_*_plan_describe): the shape decisions only, no driver call.
+static int build_plan(const mscnn_conv_desc* d, const OutView* view, bool encode, ConvPlan* plan) {
+  ConvShape s;
+  int rc = conv_shape(d, view, &s);
+  if (rc != MSCNN_OK) return rc;
+  IgemmParams& p = plan->p;
+  p = igemm_params(d, s);
+  if ((rc = stage_operands(d, s, p)) != MSCNN_OK) return rc;
+  plan->BN = s.BN;
+  plan->smem = igemm_layout(p, s.BN).total;
+  const int total_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_tiles;
+  if (config().verbose_conv)
+    fprintf(stderr, "conv plan: N=%d H=%d W=%d C=%d Cout_pad=%d k=%dx%d BN=%d box=%dx%dx%d fat=%d terms=%d rowshare=%d a_stages=%d stages=%d epi_bufs=%d smem=%zu tiles=%d\n",
+            d->N, d->H, d->W, d->C, d->Cout_pad, d->KH, d->KW, s.BN, p.box_w, p.box_h, p.box_n, p.fat, p.num_terms,
+            p.rowshare, p.a_stages, p.stages, p.epi_bufs, plan->smem, total_tiles);
+  memset(plan->maps, 0, sizeof(plan->maps));
+  plan->grid = 0;
+  if (!encode) return MSCNN_OK;
+  if ((rc = encode_maps(d, view, s, p, plan->maps)) != MSCNN_OK) return rc;
+  plan->grid = mscnn_sm_count();
+  if (plan->grid > total_tiles) plan->grid = total_tiles;
   return MSCNN_OK;
 }
 
-}  // namespace mscnn
-
-// The launch plan mscnn_conv_forward would use for `d`, as text, WITHOUT touching the device (no tensor map is encoded,
-// the pointers in `d` only have to be non-NULL where the call would require them): which instantiation, pixel box,
-// operand staging and pipeline depth (`stages` = depth of the ring carrying the weights; with rowshare=1 the
-// activation tiles have their own ring of a_stages slots).  Host-side tests pin the variant every full-size layer takes.
-namespace mscnn {
-
+// The plan as text: which instantiation, pixel box, operand staging and pipeline depth (`stages` = depth of the ring
+// carrying the weights; with rowshare=1 the activation tiles have their own ring of a_stages slots).
 static int format_plan(const ConvPlan& plan, const mscnn_conv_desc* d, char* buf, int cap) {
   const IgemmParams& p = plan.p;
   int n = snprintf(buf, (size_t)cap,
@@ -806,22 +772,130 @@ static int format_plan(const ConvPlan& plan, const mscnn_conv_desc* d, char* buf
   return (n > 0 && n < cap) ? MSCNN_OK : MSCNN_ERR_INVALID;
 }
 
+// ------------------------------------------------------------------ plan cache
+
+struct PlanKey {
+  const void* ptr[11];
+  int v[28];
+  bool operator==(const PlanKey& o) const { return memcmp(this, &o, sizeof(PlanKey)) == 0; }
+};
+struct PlanKeyHash {
+  size_t operator()(const PlanKey& k) const {
+    const unsigned char* b = reinterpret_cast<const unsigned char*>(&k);
+    uint64_t h = 1469598103934665603ull;  // FNV-1a
+    for (size_t i = 0; i < sizeof(PlanKey); ++i) h = (h ^ b[i]) * 1099511628211ull;
+    return static_cast<size_t>(h);
+  }
+};
+static std::mutex g_plan_mu;
+static std::unordered_map<PlanKey, ConvPlan, PlanKeyHash> g_plans;
+
+void conv_plan_cache_clear() {
+  std::lock_guard<std::mutex> lk(g_plan_mu);
+  g_plans.clear();
+}
+
+// The cached launch plan of (d, view), built and cached on a miss.
+static int resolve_plan(const mscnn_conv_desc* d, const OutView* view, int device, ConvPlan* plan) {
+  PlanKey key;
+  memset(&key, 0, sizeof(key));
+  const void* ptrs[11] = {d->x_hi, d->x_lo, d->w_hi, d->w_lo, d->bias, d->y_hi, d->y_lo, d->y_f32, d->pool_hi, d->pool_lo, d->dyn_n};
+  memcpy(key.ptr, ptrs, sizeof(ptrs));
+  const OutView dense = {0, 0, 0, 0, 0, 0, 0, 0};
+  const OutView& v = view ? *view : dense;
+  const int vals[28] = {d->N, d->H, d->W, d->C, d->Cout, d->Cout_pad, d->KH, d->KW, d->pad_h, d->pad_w, d->relu,
+                        d->out_mode, device, static_cast<int>(config().epoch), 0,
+                        d->stride_h, d->stride_w, d->dil_h, d->dil_w, d->group,
+                        v.ho, v.wo, v.step_h, v.step_w, v.r_h, v.r_w, v.full_h, v.full_w};
+  memcpy(key.v, vals, sizeof(vals));
+  {
+    std::lock_guard<std::mutex> lk(g_plan_mu);
+    auto it = g_plans.find(key);
+    if (it != g_plans.end()) {
+      *plan = it->second;
+      return MSCNN_OK;
+    }
+  }
+  const int rc = build_plan(d, view, true, plan);
+  if (rc != MSCNN_OK) return rc;
+  std::lock_guard<std::mutex> lk(g_plan_mu);
+  if (g_plans.size() >= 4096) g_plans.clear();  // blobs that keep moving (re-allocation): bound the table
+  g_plans.emplace(key, *plan);
+  return MSCNN_OK;
+}
+
+// ------------------------------------------------------------------ launch
+
+// cudaFuncAttributeMaxDynamicSharedMemorySize is per device and function: raised once to the whole budget.
+template <typename K>
+static cudaError_t raise_smem_once(K kern, bool (&done)[kMaxDevices], int device) {
+  if (device >= 0 && device < kMaxDevices && done[device]) return cudaSuccess;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
+  if (e == cudaSuccess && device >= 0 && device < kMaxDevices) done[device] = true;
+  return e;
+}
+
+template <int BLOCK_N, bool FAT>
+static cudaError_t launch_igemm(const CUtensorMap (&maps)[kNumMaps], const IgemmParams& p, int grid, size_t smem,
+                                int device, cudaStream_t stream) {
+  auto kern = conv_igemm_kernel<BLOCK_N, FAT>;
+  static bool done[kMaxDevices];
+  cudaError_t e = raise_smem_once(kern, done, device);
+  if (e != cudaSuccess) return e;
+  mscnn::note_launch();
+  kern<<<grid, kThreads, smem, stream>>>(maps[kMapAHi], maps[kMapALo], maps[kMapBHi], maps[kMapBLo], maps[kMapOHi],
+                                         maps[kMapOLo], maps[kMapPHi], maps[kMapPLo], p);
+  return cudaGetLastError();
+}
+
+static int launch_plan(const ConvPlan& plan, int device, cudaStream_t stream, const char* who) {
+  // [BLOCK_N = 32 << i][fat]; fat stages only below BLOCK_N = 256 (stage_operands): no <256, true> instantiation
+  static const decltype(&launch_igemm<32, false>) launch[4][2] = {
+      {launch_igemm<32, false>, launch_igemm<32, true>}, {launch_igemm<64, false>, launch_igemm<64, true>},
+      {launch_igemm<128, false>, launch_igemm<128, true>}, {launch_igemm<256, false>, nullptr}};
+  const cudaError_t e =
+      launch[__builtin_ctz(plan.BN) - 5][plan.p.fat](plan.maps, plan.p, plan.grid, plan.smem, device, stream);
+  if (e != cudaSuccess) {
+    fprintf(stderr, "%s: launch failed: %s\n", who, cudaGetErrorString(e));
+    return MSCNN_ERR_CUDA;
+  }
+  return MSCNN_OK;
+}
+
 }  // namespace mscnn
 
+using namespace mscnn;
+
+// ------------------------------------------------------------------ C entries
+
+extern "C" int mscnn_conv_forward(const mscnn_conv_desc* d, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (!d) return MSCNN_ERR_INVALID;
+  int device = 0;
+  if (cudaGetDevice(&device) != cudaSuccess) return MSCNN_ERR_CUDA;
+  ConvPlan plan;
+  const int rc = resolve_plan(d, nullptr, device, &plan);
+  if (rc != MSCNN_OK) return rc;
+  return launch_plan(plan, device, stream, "mscnn_conv_forward");
+}
+
+// The launch plan mscnn_conv_forward would use for `d`, as text, WITHOUT touching the device (no tensor map is encoded,
+// the pointers in `d` only have to be non-NULL where the call would require them).  Host-side tests pin the variant
+// every full-size layer takes.
 extern "C" int mscnn_conv_plan_describe(const mscnn_conv_desc* d, char* buf, int cap) {
   if (!d || !buf || cap <= 0) return MSCNN_ERR_INVALID;
-  mscnn::ConvPlan plan;
-  const int rc = mscnn::build_plan(d, &plan, false);
+  ConvPlan plan;
+  const int rc = build_plan(d, nullptr, false, &plan);
   if (rc != MSCNN_OK) return rc;
-  return mscnn::format_plan(plan, d, buf, cap);
+  return format_plan(plan, d, buf, cap);
 }
 
 // Entries in the launch-plan cache.  A net adds one per convolution for every new combination of input shape and blob
 // addresses it runs with; the table is emptied when it reaches 4096 entries, so it stays bounded however many input
 // sizes a process goes through.
 extern "C" int mscnn_conv_plan_count(void) {
-  std::lock_guard<std::mutex> lk(mscnn::g_plan_mu);
-  return (int)mscnn::g_plans.size();
+  std::lock_guard<std::mutex> lk(g_plan_mu);
+  return (int)g_plans.size();
 }
 
 // ------------------------------------------------------------------ deconvolution by output phase
@@ -983,7 +1057,7 @@ extern "C" int mscnn_deconv_plan_describe(const mscnn_conv_desc* d, char* buf, i
     n += m;
     if (ph.launches()) {
       ConvPlan plan;
-      if ((rc = build_plan(&ph.sub, &plan, false, &ph.view)) != MSCNN_OK) return rc;
+      if ((rc = build_plan(&ph.sub, &ph.view, false, &plan)) != MSCNN_OK) return rc;
       if ((rc = format_plan(plan, &ph.sub, buf + n, cap - n)) != MSCNN_OK) return rc;
       m = (int)strlen(buf + n);
     } else {

@@ -149,6 +149,14 @@ __device__ __forceinline__ void stage_pair(uint32_t buf, int r, int j, int c, fl
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(h) : "memory");
   if (lo) asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + lo_plane), "r"(l) : "memory");
 }
+// 16 B of a staged tile as four 32-bit words (the fused pooling of conv_igemm.cu reads and writes its tiles this way)
+__device__ __forceinline__ void ld_shared_v4(uint32_t addr, uint32_t (&v)[4]) {
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr));
+}
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint32_t (&v)[4]) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
+               : "memory");
+}
 // TMA store of a staged (hi, lo) tile pair at NHWC coordinates (c0, c1, c2, c3); the caller commits the bulk group.
 __device__ __forceinline__ void tma_store_hi_lo(const CUtensorMap* hi, const CUtensorMap* lo, uint32_t src, bool has_lo,
                                                 uint32_t lo_plane, int c0, int c1, int c2, int c3) {
