@@ -29,6 +29,11 @@ struct DynRows {
   bool pending;
 };
 
+// mscnn_b200 extension: how a forward touches a blob (Net's activation plan).  PLANES: bf16 hi (+ lo in fp32-faithful
+// precision) planes; NCHW: fp32 in the Caffe layout; TOUCH: in place, on whichever representation is current.
+enum Access { TOUCH, PLANES, NCHW };
+template <typename Dtype> using BlobAccesses = vector<pair<const Blob<Dtype>*, Access> >;
+
 template <typename Dtype>
 class CAFFE_API Layer {
  public:
@@ -76,6 +81,15 @@ class CAFFE_API Layer {
   // mscnn_b200 extension (set by Net for the layers behind a BoxOutput layer): see DynRows
   void set_dyn_rows(const DynRows* d) { dyn_rows_ = d; }
   const int* dyn_rows_device() const { return (dyn_rows_ && dyn_rows_->pending) ? dyn_rows_->device_rows : nullptr; }
+  // mscnn_b200 extension: appends each blob a forward on blobs of these shapes reads or writes, with its representation;
+  // work a fused layer does for another is stated where it runs.  false: no statement (the net cannot be planned).
+  virtual bool Accesses(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top,
+                        BlobAccesses<Dtype>* out) const { return false; }
+  // mscnn_b200 extension: a forward leaves every top on bottom[0]'s bytes (ShareData): one storage for the net
+  virtual bool TopsShareBottom(const vector<Blob<Dtype>*>& bottom) const { return false; }
+  // mscnn_b200 extension: shapes top as a forward on bottom writes it, before the host learns any data-dependent row
+  // count (Net's activation plan): Reshape's shapes, unless Forward_gpu sizes its tops itself
+  virtual void ReshapeAsForward(const vector<Blob<Dtype>*>& b, const vector<Blob<Dtype>*>& t) { Reshape(b, t); }
   virtual inline const char* type() const { return ""; }
   virtual inline int ExactNumBottomBlobs() const { return -1; }
   virtual inline int MinBottomBlobs() const { return -1; }

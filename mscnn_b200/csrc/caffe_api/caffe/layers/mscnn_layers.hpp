@@ -4,6 +4,7 @@
 // (/root/reference/include/caffe/layers/*.hpp); the per-layer headers next to this file
 // (conv_layer.hpp, ...) only include this one so that existing #include lines keep working.
 #pragma once
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -52,6 +53,7 @@ class CAFFE_API InputLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {}
   virtual inline const char* type() const { return "Input"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int ExactNumBottomBlobs() const { return 0; }
   virtual inline int MinTopBlobs() const { return 1; }
  protected:
@@ -75,25 +77,23 @@ class CAFFE_API ConvolutionLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "Convolution"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
   // mscnn_b200 extension: fold the in-place ReLU that follows into the epilogue (set by Net).
   void set_fuse_relu(bool f) { fuse_relu_ = f; }
   bool fuse_relu() const { return fuse_relu_; }
   // mscnn_b200 extension (set by Net): the folded 2x2/2 MAX Pooling that follows is computed in this layer's epilogue
-  // and written to `pool_top` whenever epilogue_pools(top); then, with keep_full == false, nothing else reads this
-  // layer's own top, which is not written (its blob holds no data).
-  void set_fused_pool(Blob<Dtype>* pool_top, bool keep_full) { fused_pool_top_ = pool_top; fused_keep_full_ = keep_full; }
+  // and written to `pool_top` whenever epilogue_pools(top); then, unless store_full, nothing else reads this layer's
+  // own top, which is not written (its blob holds no data).
+  void set_fused_pool(Blob<Dtype>* pool_top, bool store_full) { fused_pool_top_ = pool_top; store_full_ = store_full; }
   // the route whose epilogue can pool: 64-channel-aligned output, not conv1_1's kernel
   bool can_fuse_pool() const { return num_output_ % 64 == 0 && !is_conv1_1(); }
-  // what a forward reads and writes (Net's activation plan): conv1_1's kernel reads the NCHW fp32 bottom, every
-  // other route planes; the top is planes above 32 outputs, NCHW fp32 for the narrow heads
-  bool reads_nchw() const { return is_conv1_1(); }
-  bool writes_planes() const { return num_output_ > 32; }
-  Blob<Dtype>* fused_pool_top() const { return fused_pool_top_; }
-  bool keep_full() const { return fused_keep_full_; }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
+  // the top is planes above 32 outputs, NCHW fp32 for the narrow heads
+  bool planes_top() const { return num_output_ > 32; }
+  bool pools_here(const Blob<Dtype>& top) const { return fused_pool_top_ && epilogue_pools(top); }
   // stride 1, dilation 1, one group: what conv1_1's kernel and the k x 1 head-tap route compute
   bool plain_geometry() const {
     return stride_h_ == 1 && stride_w_ == 1 && dilation_h_ == 1 && dilation_w_ == 1 && group_ == 1;
@@ -103,7 +103,7 @@ class CAFFE_API ConvolutionLayer : public Layer<Dtype> {
            plain_geometry();
   }
   Blob<Dtype>* fused_pool_top_ = nullptr;
-  bool fused_keep_full_ = true;
+  bool store_full_ = true;
   int num_output_, channels_, kernel_h_, kernel_w_, pad_h_, pad_w_;
   int stride_h_, stride_w_, dilation_h_, dilation_w_, group_;
   bool bias_term_, fuse_relu_;
@@ -121,6 +121,7 @@ class CAFFE_API DeconvolutionLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "Deconvolution"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
  protected:
@@ -142,6 +143,7 @@ class CAFFE_API ReLULayer : public Layer<Dtype> {
     top[0]->ReshapeLike(*bottom[0]);
   }
   virtual inline const char* type() const { return "ReLU"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
   void set_fused(bool f) { fused_ = f; }   // producer already applied it
@@ -159,6 +161,7 @@ class CAFFE_API PoolingLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "Pooling"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int MinTopBlobs() const { return 1; }
   virtual inline int MaxTopBlobs() const { return 1; }
@@ -171,6 +174,7 @@ class CAFFE_API PoolingLayer : public Layer<Dtype> {
   bool fused() const { return fused_; }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
+  bool pooled_by_conv(const Blob<Dtype>& bottom) const { return fused_ && epilogue_pools(bottom); }
   int kernel_h_, kernel_w_, stride_h_, stride_w_, pad_h_, pad_w_, mode_, pooled_h_, pooled_w_;
   bool global_pooling_, fused_;
 };
@@ -182,6 +186,8 @@ class CAFFE_API SplitLayer : public Layer<Dtype> {
   explicit SplitLayer(const LayerParameter& param) : Layer<Dtype>(param) {}
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "Split"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
+  virtual bool TopsShareBottom(const vector<Blob<Dtype>*>& bottom) const { return true; }
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int MinTopBlobs() const { return 1; }
  protected:
@@ -196,12 +202,17 @@ class CAFFE_API ConcatLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "Concat"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
+  virtual bool TopsShareBottom(const vector<Blob<Dtype>*>& bottom) const { return bottom.size() == 1; }
   virtual inline int MinBottomBlobs() const { return 1; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
   void set_fused(bool f) { fused_ = f; }   // the producers write straight into top[0]
   bool fused() const { return fused_; }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
+  static bool aligned(const vector<Blob<Dtype>*>& bottom) {  // every bottom 64-channel aligned: planes, else NCHW fp32
+    return std::all_of(bottom.begin(), bottom.end(), [](const Blob<Dtype>* b) { return b->channels() % 64 == 0; });
+  }
   bool fused_;
 };
 
@@ -214,12 +225,13 @@ class CAFFE_API InnerProductLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "InnerProduct"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
   void set_fuse_relu(bool f) { fuse_relu_ = f; }
-  bool writes_planes() const { return N_ > 32; }  // else [M][N] fp32, the Caffe layout
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
+  bool planes_top() const { return N_ > 32; }  // else [M][N] fp32, the Caffe layout
   int M_, K_, N_;
   bool bias_term_, fuse_relu_;
   PackedParam packed_;
@@ -234,6 +246,8 @@ class CAFFE_API DropoutLayer : public Layer<Dtype> {
     if (top[0] != bottom[0]) top[0]->ReshapeLike(*bottom[0]);
   }
   virtual inline const char* type() const { return "Dropout"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
+  virtual bool TopsShareBottom(const vector<Blob<Dtype>*>& bottom) const { return true; }
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
  protected:
@@ -253,6 +267,7 @@ class CAFFE_API BoxOutputLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "BoxOutput"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int MinBottomBlobs() const { return 1; }
   virtual inline int MinTopBlobs() const { return 1; }
   virtual inline int MaxTopBlobs() const { return 2; }
@@ -273,8 +288,12 @@ class CAFFE_API BoxOutputLayer : public Layer<Dtype> {
   void ResolveRows(const vector<Blob<Dtype>*>& top);
   // after a CUDA-graph replay of this layer's launches (Net::GraphForward): the counts are pending again
   void RearmRows();
-  // the rows Forward sizes its tops for before the count is known
-  int cap_rows(int num) const { return num * cfg_.max_nms_num; }
+  // the tops at cap rows (N x max_nms_num), as Forward sizes them before the count is known
+  virtual void ReshapeAsForward(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
+    const int cap = bottom[0]->num() * cfg_.max_nms_num;
+    top[0]->Reshape(cap, 5, 1, 1);
+    if (output_proposal_with_score_) top[1]->Reshape(cap, 6, 1, 1);
+  }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   mscnn_box_output_cfg cfg_;
@@ -284,7 +303,6 @@ class CAFFE_API BoxOutputLayer : public Layer<Dtype> {
   int* num_out_dev_;
   int* num_out_host_;
   int num_out_cap_;
-  Blob<Dtype> scratch_score_;
   bool defer_rows_ = false;
   DynRows dyn_ = {nullptr, false};
   cudaEvent_t rows_event_ = nullptr;
@@ -299,6 +317,7 @@ class CAFFE_API ROIPoolingLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "ROIPooling"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int MinBottomBlobs() const { return 2; }
   virtual inline int MaxBottomBlobs() const { return 2; }
   virtual inline int MinTopBlobs() const { return 1; }
@@ -315,9 +334,9 @@ class CAFFE_API ROIPoolingLayer : public Layer<Dtype> {
     follower->fused_ = true;
   }
   bool fused() const { return fused_; }
-  Blob<Dtype>* concat_top() const { return concat_top_; }
  protected:
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
+  Blob<Dtype>* output(const vector<Blob<Dtype>*>& top) const { return concat_top_ ? concat_top_ : top[0]; }
   int channels_, height_, width_, pooled_height_, pooled_width_;
   float spatial_scale_;
   vector<float> pad_ratios_;     // one variant per entry, pooled in one launch: this layer's own, then its followers'
@@ -335,6 +354,7 @@ class CAFFE_API ROIAlignLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "ROIAlign"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int MinBottomBlobs() const { return 2; }
   virtual inline int MaxBottomBlobs() const { return 2; }
   virtual inline int MinTopBlobs() const { return 1; }
@@ -354,6 +374,7 @@ class CAFFE_API DecodeBBoxLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "DecodeBBox"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int MinBottomBlobs() const { return 2; }
   virtual inline int MaxBottomBlobs() const { return 3; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
@@ -369,6 +390,7 @@ class CAFFE_API SoftmaxLayer : public Layer<Dtype> {
   explicit SoftmaxLayer(const LayerParameter& param) : Layer<Dtype>(param) {}
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "Softmax"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int ExactNumBottomBlobs() const { return 1; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
  protected:
@@ -384,6 +406,7 @@ class CAFFE_API EltwiseLayer : public Layer<Dtype> {
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
   virtual inline const char* type() const { return "Eltwise"; }
+  virtual bool Accesses(const vector<Blob<Dtype>*>&, const vector<Blob<Dtype>*>&, BlobAccesses<Dtype>*) const;
   virtual inline int MinBottomBlobs() const { return 2; }
   virtual inline int ExactNumTopBlobs() const { return 1; }
  protected:

@@ -89,7 +89,7 @@ class CAFFE_API Net {
   // blob its producer never wrote; fused_group_end(i) = the last layer whose work layer i does.
   int fused_producer(int layer) const { return fused_producer_.empty() ? layer : fused_producer_[layer]; }
   int fused_group_end(int layer) const;
-  // mscnn_b200 extension: the last layer that reads blob_name's storage, directly or through a Split top (-1: none)
+  // mscnn_b200 extension: the last layer that reads blob_name's storage, directly or through a top on it (-1: none)
   int last_reader(const string& blob_name) const;
   // mscnn_b200 extension: data-dependent rows (layer.hpp DynRows).  No layer waits for the device in the middle of a
   // forward: the blobs behind BoxOutput keep cap rows while the kernels read the true count on the device.
@@ -106,7 +106,7 @@ class CAFFE_API Net {
   bool graph_replayed_last_forward() const { return graph_replayed_; }
 
   // mscnn_b200 extension: activation reuse (off by default; DESIGN.md "Activation memory plan").  With it on, the
-  // storages (a blob with its Split tops and in-place tops) whose lifetimes do not overlap share one device arena, and
+  // storages (storage_blob_) whose lifetimes do not overlap share one device arena, and
   // after a forward a blob whose bytes a later blob took is released: its shape stays readable, its data accessors
   // abort with a message naming it.  Net inputs, outputs and the blobs named in `keep` are never in the arena, so they
   // stay readable.  Every keep name must be a blob of the net.
@@ -181,7 +181,8 @@ class CAFFE_API Net {
   vector<Blob<Dtype>*> net_output_blobs_;
   bool time_layers_;
   vector<float> layer_ms_;
-  vector<int> storage_blob_;    // per blob: the blob whose storage it shares (itself unless a Split top)
+  vector<int> storage_blob_;    // per blob: the blob whose bytes it is on (itself unless Layer::TopsShareBottom)
+  vector<vector<int> > writers_, readers_;  // per blob: the layers with it among their tops / bottoms, in order
   vector<int> fused_producer_;  // per layer: who does its work (itself unless fused away)
   int dyn_box_ = -1;            // index of the BoxOutput layer whose rows are deferred (-1: none / several)
   vector<int> dyn_layers_;      // layers whose row count derives from it, in execution order

@@ -71,6 +71,19 @@ static mscnn_conv_desc conv_desc(const Blob<float>::Planes& x, const PackedParam
   return d;
 }
 
+// Defines T::Accesses (Layer::Accesses), whose parameters are bottom, top and out.
+#define LAYER_ACCESSES(T)                                                                                              \
+  template <typename Dtype>                                                                                           \
+  bool T<Dtype>::Accesses(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top,                       \
+                          BlobAccesses<Dtype>* out) const
+
+// every blob of `blobs` in representation a
+template <typename Dtype>
+static bool access_all(BlobAccesses<Dtype>* out, const vector<Blob<Dtype>*>& blobs, Access a) {
+  for (size_t k = 0; k < blobs.size(); ++k) out->push_back(make_pair(blobs[k], a));
+  return true;
+}
+
 void FillBlob(const FillerParameter& filler, Blob<float>* blob) {
   const std::string& type = filler.type();
   float* data = blob->mutable_cpu_data();
@@ -110,6 +123,7 @@ void InputLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vec
     for (int i = 0; i < num_top; ++i) top[i]->Reshape(param.shape(num_shape == 1 ? 0 : i));
   }
 }
+LAYER_ACCESSES(InputLayer) { return access_all(out, top, NCHW); }
 
 // Kernel, pad, stride and dilation of a 2-D ConvolutionParameter (base_conv_layer.cpp:27-108), shared by Convolution
 // and Deconvolution.
@@ -257,11 +271,11 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
   d.stride_h = stride_h_; d.stride_w = stride_w_;
   d.dil_h = dilation_h_; d.dil_w = dilation_w_;
   d.group = group_;
-  if (cout_pad % 64 == 0) {
+  if (planes_top()) {
     d.out_mode = MSCNN_OUT_NHWC_BF16;
     const int ho = top[0]->height(), wo = top[0]->width();
-    const bool pool_here = fused_pool_top_ && epilogue_pools(*top[0]);
-    if (!pool_here || fused_keep_full_) {
+    const bool pool_here = pools_here(*top[0]);
+    if (!pool_here || store_full_) {
       typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
       d.y_hi = y.hi;
       d.y_lo = y.lo;
@@ -277,6 +291,13 @@ void ConvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, co
     d.y_f32 = top[0]->mutable_gpu_data();
   }
   MSCNN_CHECK(mscnn_conv_forward(&d, Caffe::stream()));
+}
+LAYER_ACCESSES(ConvolutionLayer) {
+  out->push_back(make_pair(bottom[0], is_conv1_1() ? NCHW : PLANES));
+  if (!pools_here(*top[0])) return access_all(out, top, planes_top() ? PLANES : NCHW);
+  if (store_full_) out->push_back(make_pair(top[0], PLANES));  // else the un-pooled top is not written
+  out->push_back(make_pair(fused_pool_top_, PLANES));
+  return true;
 }
 
 // -------------------------------------------------------------------------- Deconvolution
@@ -370,6 +391,7 @@ void DeconvolutionLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, 
   d.y_lo = y.lo;
   MSCNN_CHECK(mscnn_deconv_forward(&d, Caffe::stream()));
 }
+LAYER_ACCESSES(DeconvolutionLayer) { return access_all(out, bottom, PLANES) && access_all(out, top, PLANES); }
 
 // ----------------------------------------------------------------------------------- ReLU
 template <typename Dtype>
@@ -387,6 +409,11 @@ void ReLULayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vec
   } else {
     MSCNN_CHECK(mscnn_relu_f32(top[0]->mutable_gpu_data(), top[0]->count(), Caffe::stream()));
   }
+}
+LAYER_ACCESSES(ReLULayer) {
+  if (fused_) return true;
+  if (top[0] == bottom[0]) return access_all(out, top, TOUCH);
+  return access_all(out, bottom, NCHW) && access_all(out, top, NCHW);
 }
 
 // -------------------------------------------------------------------------------- Pooling
@@ -448,12 +475,16 @@ void PoolingLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const vect
 }
 template <typename Dtype>
 void PoolingLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
-  if (fused_ && epilogue_pools(*bottom[0])) return;  // computed in the producing convolution's epilogue
+  if (pooled_by_conv(*bottom[0])) return;  // computed in the producing convolution's epilogue
   const bool split = Caffe::split();
   typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
   typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
   MSCNN_CHECK(mscnn_pool2d_forward_dyn(x.hi, x.lo, y.hi, y.lo, x.n, x.h, x.w, x.cpad, kernel_h_, kernel_w_, stride_h_,
                                        stride_w_, pad_h_, pad_w_, mode_, this->dyn_rows_device(), Caffe::stream()));
+}
+LAYER_ACCESSES(PoolingLayer) {
+  if (pooled_by_conv(*bottom[0])) return true;  // the convolution writes the top
+  return access_all(out, bottom, PLANES) && access_all(out, top, PLANES);
 }
 
 // ---------------------------------------------------------------------------------- Split
@@ -468,6 +499,7 @@ template <typename Dtype>
 void SplitLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   for (size_t i = 0; i < top.size(); ++i) top[i]->ShareData(*bottom[0]);
 }
+LAYER_ACCESSES(SplitLayer) { return true; }  // the tops are on the bottom's storage (TopsShareBottom)
 
 // --------------------------------------------------------------------------------- Concat
 template <typename Dtype>
@@ -491,11 +523,9 @@ void ConcatLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const vecto
 template <typename Dtype>
 void ConcatLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   if (fused_) return;  // ROIPooling producers already wrote their channel ranges of top[0]
-  if (bottom.size() == 1) { top[0]->ShareData(*bottom[0]); return; }
+  if (TopsShareBottom(bottom)) { top[0]->ShareData(*bottom[0]); return; }
   const bool split = Caffe::split();
-  bool aligned = true;
-  for (size_t i = 0; i < bottom.size(); ++i) aligned = aligned && (bottom[i]->channels() % 64 == 0);
-  if (aligned) {
+  if (aligned(bottom)) {
     typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
     int off = 0;
     for (size_t i = 0; i < bottom.size(); ++i) {
@@ -518,6 +548,11 @@ void ConcatLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const v
       off += row;
     }
   }
+}
+LAYER_ACCESSES(ConcatLayer) {
+  if (fused_ || TopsShareBottom(bottom)) return true;  // fused: the ROIPooling producers write the top
+  const Access a = aligned(bottom) ? PLANES : NCHW;
+  return access_all(out, bottom, a) && access_all(out, top, a);
 }
 
 // --------------------------------------------------------------------------- InnerProduct
@@ -569,7 +604,7 @@ void InnerProductLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, c
   // the NHWC flattening of the bottom is the channel vector of a 1 x 1 "image"
   mscnn_conv_desc d = conv_desc(x, packed_, M_, 1, 1, H * W * x.cpad, N_, 1, 1, 0, 0, this->dyn_rows_device());
   d.relu = fuse_relu_ ? 1 : 0;
-  if (nout_pad % 64 == 0) {
+  if (planes_top()) {
     typename Blob<Dtype>::Planes y = top[0]->mutable_planes(split);
     d.out_mode = MSCNN_OUT_NHWC_BF16;
     d.y_hi = y.hi;
@@ -580,6 +615,9 @@ void InnerProductLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, c
   }
   MSCNN_CHECK(mscnn_conv_forward(&d, Caffe::stream()));
 }
+LAYER_ACCESSES(InnerProductLayer) {
+  return access_all(out, bottom, PLANES) && access_all(out, top, planes_top() ? PLANES : NCHW);
+}
 
 // -------------------------------------------------------------------------------- Dropout
 template <typename Dtype>
@@ -587,6 +625,7 @@ void DropoutLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const 
   CHECK(this->phase_ == TEST) << "mscnn_b200 is forward-only: Dropout runs in the TEST phase";
   if (top[0] != bottom[0]) top[0]->ShareData(*bottom[0]);  // dropout_layer.cpp:43-45 copies; sharing is equivalent
 }
+LAYER_ACCESSES(DropoutLayer) { return true; }  // the top is on the bottom's storage (TopsShareBottom)
 
 // ------------------------------------------------------------------------------ BoxOutput
 template <typename Dtype>
@@ -683,12 +722,9 @@ void BoxOutputLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, cons
   dyn_.pending = false;  // a new Forward supersedes counts nobody asked for
   // Size the tops for the cap, let the kernels write in place, then shrink to the true row
   // count (Blob::Reshape never reallocates when shrinking, blob.cpp:40-44).
-  const int cap = N * cfg_.max_nms_num;
-  top[0]->Reshape(cap, 5, 1, 1);
-  Blob<Dtype>* score_blob = output_proposal_with_score_ ? top[1] : &scratch_score_;
-  score_blob->Reshape(cap, 6, 1, 1);
+  ReshapeAsForward(bottom, top);
   Dtype* rois = top[0]->mutable_gpu_data();
-  Dtype* rois_score = output_proposal_with_score_ ? score_blob->mutable_gpu_data() : nullptr;
+  Dtype* rois_score = output_proposal_with_score_ ? top[1]->mutable_gpu_data() : nullptr;
   MSCNN_CHECK(mscnn_box_output_forward(&cfg_, N, maps, workspace_, workspace_bytes_, rois, rois_score,
                                        num_out_dev_, Caffe::stream()));
   CUDA_CHECK(cudaMemcpyAsync(num_out_host_, num_out_dev_, sizeof(int) * (2 + N), cudaMemcpyDeviceToHost,
@@ -700,6 +736,7 @@ void BoxOutputLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, cons
   dyn_.pending = true;  // tops have `cap` rows; the true count is in num_out_dev_[0] (and soon in num_out_host_[0])
   if (!defer_rows_) ResolveRows(top);
 }
+LAYER_ACCESSES(BoxOutputLayer) { return access_all(out, bottom, NCHW) && access_all(out, top, NCHW); }
 
 // ----------------------------------------------------------------------------- ROIPooling
 template <typename Dtype>
@@ -727,16 +764,20 @@ void ROIPoolingLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, con
   typename Blob<Dtype>::Planes x = bottom[0]->planes(split);
   const int R = bottom[1]->num();
   const Dtype* rois = bottom[1]->gpu_data();
-  Blob<Dtype>* out = top[0];
-  if (concat_top_) {  // fused ConcatLayer: its top is [R, total, ph, pw]
-    concat_top_->Reshape(R, concat_channels_, pooled_height_, pooled_width_);
-    out = concat_top_;
-  }
+  Blob<Dtype>* out = output(top);
+  if (concat_top_) out->Reshape(R, concat_channels_, pooled_height_, pooled_width_);  // the fused Concat's top
   typename Blob<Dtype>::Planes y = out->mutable_planes(split);
   MSCNN_CHECK(mscnn_roi_pool_multi_forward_dyn(x.hi, x.lo, x.n, x.h, x.w, x.cpad, rois, R, pooled_height_, pooled_width_,
                                                spatial_scale_, (int)pad_ratios_.size(), pad_ratios_.data(),
                                                channel_offsets_.data(), y.hi, y.lo, y.cpad, this->dyn_rows_device(),
                                                Caffe::stream()));
+}
+LAYER_ACCESSES(ROIPoolingLayer) {
+  if (fused_) return true;  // pooled in its leader's launch
+  out->push_back(make_pair(bottom[0], PLANES));
+  out->push_back(make_pair(bottom[1], NCHW));
+  out->push_back(make_pair(output(top), PLANES));
+  return true;
 }
 
 // ------------------------------------------------------------------------------- ROIAlign
@@ -767,6 +808,11 @@ void ROIAlignLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const
   MSCNN_CHECK(mscnn_roi_align_forward_dyn(x.hi, x.lo, x.n, x.h, x.w, x.cpad, bottom[1]->gpu_data(), bottom[1]->num(),
                                           pooled_height_, pooled_width_, spatial_scale_, pad_ratio_, y.hi, y.lo,
                                           y.cpad, 0, this->dyn_rows_device(), Caffe::stream()));
+}
+LAYER_ACCESSES(ROIAlignLayer) {
+  out->push_back(make_pair(bottom[0], PLANES));
+  out->push_back(make_pair(bottom[1], NCHW));
+  return access_all(out, top, PLANES);
 }
 
 // ----------------------------------------------------------------------------- DecodeBBox
@@ -802,6 +848,7 @@ void DecodeBBoxLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, con
   MSCNN_CHECK(mscnn_decode_bbox_forward(bottom[0]->gpu_data(), bottom[1]->gpu_data(), num, bottom[0]->channels(),
                                         bbox_mean_, bbox_std_, top[0]->mutable_gpu_data(), Caffe::stream()));
 }
+LAYER_ACCESSES(DecodeBBoxLayer) { return access_all(out, bottom, NCHW) && access_all(out, top, NCHW); }
 
 // -------------------------------------------------------------------------------- Softmax
 template <typename Dtype>
@@ -816,6 +863,7 @@ void SoftmaxLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const 
   MSCNN_CHECK(mscnn_softmax_forward(bottom[0]->gpu_data(), outer_num_, bottom[0]->shape(softmax_axis_), inner_num_,
                                     top[0]->mutable_gpu_data(), Caffe::stream()));
 }
+LAYER_ACCESSES(SoftmaxLayer) { return access_all(out, bottom, NCHW) && access_all(out, top, NCHW); }
 
 // -------------------------------------------------------------------------------- Eltwise
 template <typename Dtype>
@@ -844,6 +892,7 @@ void EltwiseLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const 
   MSCNN_CHECK(mscnn_eltwise_forward(in, (int)bottom.size(), op_, coeffs_.data(), (size_t)top[0]->count(),
                                     top[0]->mutable_gpu_data(), Caffe::stream()));
 }
+LAYER_ACCESSES(EltwiseLayer) { return access_all(out, bottom, NCHW) && access_all(out, top, NCHW); }
 
 INSTANTIATE_CLASS(InputLayer);
 INSTANTIATE_CLASS(ConvolutionLayer);

@@ -164,11 +164,17 @@ void Net<Dtype>::Init(const NetParameter& in_param) {
   for (size_t i = 0; i < layer_names_.size(); ++i) layer_names_index_[layer_names_[i]] = (int)i;
   layer_ms_.assign(layers_.size(), 0.f);
   storage_blob_.resize(blobs_.size());
+  writers_.resize(blobs_.size());
+  readers_.resize(blobs_.size());
   for (size_t b = 0; b < blobs_.size(); ++b) storage_blob_[b] = (int)b;
-  for (size_t i = 0; i < layers_.size(); ++i)  // a Split's tops share its bottom's storage (SplitLayer::Forward_gpu)
-    if (dynamic_cast<SplitLayer<Dtype>*>(layers_[i].get()))
-      for (size_t t = 0; t < top_id_vecs_[i].size(); ++t)
-        storage_blob_[top_id_vecs_[i][t]] = storage_blob_[bottom_id_vecs_[i][0]];
+  for (int i = 0; i < L; ++i) {
+    for (size_t k = 0; k < bottom_id_vecs_[i].size(); ++k) readers_[bottom_id_vecs_[i][k]].push_back(i);
+    for (size_t k = 0; k < top_id_vecs_[i].size(); ++k) {
+      writers_[top_id_vecs_[i][k]].push_back(i);
+      if (layers_[i]->TopsShareBottom(bottom_vecs_[i]))
+        storage_blob_[top_id_vecs_[i][k]] = storage_blob_[bottom_id_vecs_[i][0]];
+    }
+  }
   fused_producer_.resize(layers_.size());
   for (size_t i = 0; i < layers_.size(); ++i) fused_producer_[i] = (int)i;
   if (!std::getenv("MSCNN_NO_FUSION")) {
@@ -267,15 +273,10 @@ void Net<Dtype>::FuseLayers() {
     ReLULayer<Dtype>* relu = dynamic_cast<ReLULayer<Dtype>*>(layers_[i].get());
     if (!relu || bottom_vecs_[i].size() != 1 || top_vecs_[i][0] != bottom_vecs_[i][0]) continue;
     const int blob_id = bottom_id_vecs_[i][0];
-    int writer = -1;
-    bool clean = true;
-    for (int k = i - 1; k >= 0 && writer < 0; --k) {
-      for (size_t t = 0; t < top_id_vecs_[k].size(); ++t)
-        if (top_id_vecs_[k][t] == blob_id) writer = k;
-      if (writer < 0)
-        for (size_t b = 0; b < bottom_id_vecs_[k].size(); ++b)
-          if (bottom_id_vecs_[k][b] == blob_id) clean = false;  // someone reads the pre-ReLU value
-    }
+    int writer = -1;  // the last layer before the ReLU that writes the blob
+    for (int k : writers_[blob_id]) writer = k < i ? k : writer;
+    bool clean = true;  // nobody reads the pre-ReLU value
+    for (int k : readers_[blob_id]) clean = clean && !(k > writer && k < i);
     if (writer < 0 || !clean) continue;
     if (ConvolutionLayer<Dtype>* conv = dynamic_cast<ConvolutionLayer<Dtype>*>(layers_[writer].get())) {
       conv->set_fuse_relu(true);
@@ -292,16 +293,9 @@ void Net<Dtype>::FuseLayers() {
     bool ok = true;
     int total = 0;
     for (size_t b = 0; b < bottom_id_vecs_[i].size() && ok; ++b) {
-      const int blob_id = bottom_id_vecs_[i][b];
-      int writer = -1, readers = 0;
-      for (int k = 0; k < L; ++k) {
-        for (size_t t = 0; t < top_id_vecs_[k].size(); ++t)
-          if (top_id_vecs_[k][t] == blob_id) writer = k;
-        for (size_t bb = 0; bb < bottom_id_vecs_[k].size(); ++bb)
-          if (bottom_id_vecs_[k][bb] == blob_id) ++readers;
-      }
+      const int blob_id = bottom_id_vecs_[i][b], writer = writers_[blob_id].back();  // every blob has a writer
       const int c = bottom_vecs_[i][b]->channels();
-      if (writer < 0 || !dynamic_cast<ROIPoolingLayer<Dtype>*>(layers_[writer].get()) || readers != 1 || c % 64 != 0)
+      if (!dynamic_cast<ROIPoolingLayer<Dtype>*>(layers_[writer].get()) || readers_[blob_id].size() != 1 || c % 64 != 0)
         ok = false;
       else
         offset[writer] = total;
@@ -346,12 +340,12 @@ void Net<Dtype>::FusePooling() {
     if (!pool || !pool->is_max_2x2_s2()) continue;
     const int blob_id = bottom_id_vecs_[i][0];
     // walk back over the writers of the blob: [conv] or [conv, fused in-place relu]
+    const vector<int>& w = writers_[blob_id];
     int conv_idx = -1;
     bool ok = true;
-    for (int k = i - 1; k >= 0 && conv_idx < 0 && ok; --k) {
-      bool writes = false;
-      for (size_t t = 0; t < top_id_vecs_[k].size(); ++t) writes = writes || (top_id_vecs_[k][t] == blob_id);
-      if (!writes) continue;
+    for (int j = (int)w.size() - 1; j >= 0 && conv_idx < 0 && ok; --j) {
+      const int k = w[j];
+      if (k >= i) continue;
       if (ReLULayer<Dtype>* r = dynamic_cast<ReLULayer<Dtype>*>(layers_[k].get())) {
         if (!r->fused()) ok = false;
         continue;
@@ -362,16 +356,9 @@ void Net<Dtype>::FusePooling() {
     if (!ok || conv_idx < 0) continue;
     ConvolutionLayer<Dtype>* conv = static_cast<ConvolutionLayer<Dtype>*>(layers_[conv_idx].get());
     if (!conv->can_fuse_pool()) continue;
-    // other readers of the un-pooled blob (in-place layers excluded)?
+    // other readers of the un-pooled blob (in-place layers, which write it too, excluded)?
     int readers = 0;
-    for (int k = 0; k < L; ++k) {
-      if (k == i) continue;
-      for (size_t b = 0; b < bottom_id_vecs_[k].size(); ++b) {
-        if (bottom_id_vecs_[k][b] != blob_id) continue;
-        const bool in_place = b < top_id_vecs_[k].size() && top_id_vecs_[k][b] == blob_id;
-        if (!in_place) ++readers;
-      }
-    }
+    for (int k : readers_[blob_id]) readers += k != i && std::find(w.begin(), w.end(), k) == w.end();
     bool is_net_output = false;
     for (size_t o = 0; o < net_output_blob_indices_.size(); ++o)
       is_net_output = is_net_output || (net_output_blob_indices_[o] == blob_id);
@@ -385,9 +372,8 @@ template <typename Dtype>
 int Net<Dtype>::last_reader(const string& blob_name) const {
   const int storage = storage_blob_[blob_names_index_.at(blob_name)];
   int last = -1;
-  for (size_t i = 0; i < layers_.size(); ++i)
-    for (size_t b = 0; b < bottom_id_vecs_[i].size(); ++b)
-      if (storage_blob_[bottom_id_vecs_[i][b]] == storage) last = (int)i;
+  for (size_t b = 0; b < blobs_.size(); ++b)
+    if (storage_blob_[b] == storage && !readers_[b].empty()) last = std::max(last, readers_[b].back());
   return last;
 }
 

@@ -1,24 +1,21 @@
 // Activation reuse for caffe::Net (net.hpp set_activation_reuse; DESIGN.md "Activation memory plan").
 //
-// The unit is a storage: a blob together with its Split tops and the tops a layer shares with its bottom (in-place
-// tops, Dropout, a one-bottom Concat).  The plan is made on the host from the net's static structure and the shapes
-// of the forward it is for: every layer's Reshape runs, in order, on shadow blobs (BoxOutput's tops at their cap
-// rows, as its Forward sizes them), and each layer type says which representation of which blob it reads and writes
-// at which layer.  A storage is live from its first access to its last; storages whose intervals do not intersect may
-// share bytes of the arena.
+// The unit is a storage: a blob together with the tops on its bytes (Net::storage_blob_).  The plan is made on the host
+// from the net's static structure and the shapes of the forward it is for: every layer's Reshape runs, in order, on
+// shadow blobs (Layer::ReshapeAsForward: BoxOutput's tops at their cap rows), and each layer states which
+// representation of which blob its forward reads and writes (Layer::Accesses).  A storage is live from its first
+// access to its last; storages whose intervals do not intersect may share bytes of the arena.
 #include <algorithm>
 #include <climits>
 #include <map>
 #include <set>
 #include <sstream>
 
-#include "caffe/layers/mscnn_layers.hpp"
 #include "caffe/net.hpp"
 
 namespace caffe {
 
 namespace {
-enum Access { TOUCH, PLANES, NCHW };  // TOUCH: in-place work on whatever representation is current
 inline size_t round256(size_t b) { return (b + 255) / 256 * 256; }
 }  // namespace
 
@@ -94,111 +91,39 @@ void Net<Dtype>::ComputeActivationPlan(ActivationPlan* plan) const {
   for (int i = 0; i < L; ++i) {
     for (size_t k = 0; k < bottom_id_vecs_[i].size(); ++k) sb[i].push_back(shadow[bottom_id_vecs_[i][k]].get());
     for (size_t k = 0; k < top_id_vecs_[i].size(); ++k) st[i].push_back(shadow[top_id_vecs_[i][k]].get());
-    layers_[i]->Reshape(sb[i], st[i]);
-    if (BoxOutputLayer<Dtype>* box = dynamic_cast<BoxOutputLayer<Dtype>*>(layers_[i].get())) {
-      const int cap = box->cap_rows(sb[i][0]->num());
-      st[i][0]->Reshape(cap, 5, 1, 1);
-      if (st[i].size() > 1) st[i][1]->Reshape(cap, 6, 1, 1);
-    }
+    layers_[i]->ReshapeAsForward(sb[i], st[i]);
   }
-  // 2. storages
-  vector<int> root(storage_blob_);
-  for (int i = 0; i < L; ++i) {
-    Layer<Dtype>* l = layers_[i].get();
-    if ((dynamic_cast<DropoutLayer<Dtype>*>(l) ||
-         (dynamic_cast<ConcatLayer<Dtype>*>(l) && bottom_id_vecs_[i].size() == 1)) &&
-        top_id_vecs_[i][0] != bottom_id_vecs_[i][0])
-      root[top_id_vecs_[i][0]] = bottom_id_vecs_[i][0];
-  }
-  auto find = [&](int b) {
-    while (root[b] != b) b = root[b];
-    return b;
-  };
+  // 2. who reads and writes what, where, as each layer states it; a fused target (a pooled or Concat top) is named
+  // by its real blob, every other blob by its shadow
   std::map<const Blob<Dtype>*, int> id_of;
-  for (int b = 0; b < B; ++b) id_of[blobs_[b].get()] = b;
+  for (int b = 0; b < B; ++b) id_of[blobs_[b].get()] = id_of[shadow[b].get()] = b;
   struct Use {
     int first = INT_MAX, last = -1;
     bool planes = false, nchw = false;
     vector<int> at;
   };
   vector<Use> use(B);
-  // 3. who reads and writes what, where (the layer that runs it: fused work happens at its producer)
   for (int i = 0; i < L; ++i) {
-    auto touch = [&](int blob, Access a) {
-      Use& u = use[find(blob)];
+    BlobAccesses<Dtype> acc;
+    if (!layers_[i]->Accesses(sb[i], st[i], &acc))
+      LOG(FATAL) << "activation reuse has no plan for layer type " << layers_[i]->type() << " (layer "
+                 << layer_names_[i] << ")";
+    for (size_t k = 0; k < acc.size(); ++k) {
+      Use& u = use[storage_blob_[id_of.at(acc[k].first)]];
       u.first = std::min(u.first, i);
       u.last = std::max(u.last, i);
-      u.planes = u.planes || a == PLANES;
-      u.nchw = u.nchw || a == NCHW;
+      u.planes = u.planes || acc[k].second == PLANES;
+      u.nchw = u.nchw || acc[k].second == NCHW;
       if (u.at.empty() || u.at.back() != i) u.at.push_back(i);
-    };
-    auto all = [&](const vector<int>& ids, Access a) {
-      for (size_t k = 0; k < ids.size(); ++k) touch(ids[k], a);
-    };
-    Layer<Dtype>* l = layers_[i].get();
-    const vector<int>& bt = bottom_id_vecs_[i];
-    const vector<int>& tp = top_id_vecs_[i];
-    if (dynamic_cast<InputLayer<Dtype>*>(l)) {
-      all(tp, NCHW);
-    } else if (ConvolutionLayer<Dtype>* c = dynamic_cast<ConvolutionLayer<Dtype>*>(l)) {
-      touch(bt[0], c->reads_nchw() ? NCHW : PLANES);
-      if (c->fused_pool_top() && epilogue_pools(*st[i][0])) {
-        if (c->keep_full()) touch(tp[0], PLANES);  // else the un-pooled top takes no bytes
-        touch(id_of.at(c->fused_pool_top()), PLANES);
-      } else {
-        touch(tp[0], c->writes_planes() ? PLANES : NCHW);
-      }
-    } else if (dynamic_cast<DeconvolutionLayer<Dtype>*>(l)) {
-      all(bt, PLANES);
-      all(tp, PLANES);
-    } else if (ReLULayer<Dtype>* r = dynamic_cast<ReLULayer<Dtype>*>(l)) {
-      if (r->fused()) continue;
-      if (tp[0] == bt[0]) {
-        touch(bt[0], TOUCH);
-      } else {
-        all(bt, NCHW);
-        all(tp, NCHW);
-      }
-    } else if (PoolingLayer<Dtype>* p = dynamic_cast<PoolingLayer<Dtype>*>(l)) {
-      if (p->fused() && epilogue_pools(*sb[i][0])) continue;  // written by the convolution
-      all(bt, PLANES);
-      all(tp, PLANES);
-    } else if (dynamic_cast<SplitLayer<Dtype>*>(l) || dynamic_cast<DropoutLayer<Dtype>*>(l)) {
-      continue;
-    } else if (ConcatLayer<Dtype>* cat = dynamic_cast<ConcatLayer<Dtype>*>(l)) {
-      if (cat->fused() || bt.size() == 1) continue;  // the ROIPooling producers write the top / a shared storage
-      bool aligned = true;
-      for (size_t k = 0; k < bt.size(); ++k) aligned = aligned && sb[i][k]->channels() % 64 == 0;
-      all(bt, aligned ? PLANES : NCHW);
-      all(tp, aligned ? PLANES : NCHW);
-    } else if (InnerProductLayer<Dtype>* ip = dynamic_cast<InnerProductLayer<Dtype>*>(l)) {
-      all(bt, PLANES);
-      all(tp, ip->writes_planes() ? PLANES : NCHW);
-    } else if (ROIPoolingLayer<Dtype>* rp = dynamic_cast<ROIPoolingLayer<Dtype>*>(l)) {
-      if (rp->fused()) continue;  // pooled in its leader's launch
-      touch(bt[0], PLANES);
-      touch(bt[1], NCHW);
-      touch(rp->concat_top() ? id_of.at(rp->concat_top()) : tp[0], PLANES);
-    } else if (dynamic_cast<ROIAlignLayer<Dtype>*>(l)) {
-      touch(bt[0], PLANES);
-      touch(bt[1], NCHW);
-      all(tp, PLANES);
-    } else if (dynamic_cast<BoxOutputLayer<Dtype>*>(l) || dynamic_cast<DecodeBBoxLayer<Dtype>*>(l) ||
-               dynamic_cast<SoftmaxLayer<Dtype>*>(l) || dynamic_cast<EltwiseLayer<Dtype>*>(l)) {
-      all(bt, NCHW);
-      all(tp, NCHW);
-    } else {
-      LOG(FATAL) << "activation reuse has no plan for layer type " << l->type() << " (layer " << layer_names_[i]
-                 << ")";
     }
   }
-  // 4. bytes, and what stays outside the arena
+  // 3. bytes, and what stays outside the arena
   std::set<int> inputs(net_input_blob_indices_.begin(), net_input_blob_indices_.end());
   std::set<int> outputs(net_output_blob_indices_.begin(), net_output_blob_indices_.end());
   std::set<int> kept;
   for (size_t k = 0; k < keep_.size(); ++k) kept.insert(blob_names_index_.at(keep_[k]));
   std::map<int, vector<int> > members;
-  for (int b = 0; b < B; ++b) members[find(b)].push_back(b);
+  for (int b = 0; b < B; ++b) members[storage_blob_[b]].push_back(b);
   for (std::map<int, vector<int> >::iterator it = members.begin(); it != members.end(); ++it) {
     const Use& u = use[it->first];
     if (u.last < 0 || !(u.planes || u.nchw)) continue;
@@ -231,7 +156,7 @@ void Net<Dtype>::ComputeActivationPlan(ActivationPlan* plan) const {
   std::sort(plan->storages.begin(), plan->storages.end(), [](const ActivationStorage& a, const ActivationStorage& b) {
     return a.first != b.first ? a.first < b.first : a.blob < b.blob;
   });
-  // 5. offsets: largest first, each into the smallest gap left by the placed storages it is live with
+  // 4. offsets: largest first, each into the smallest gap left by the placed storages it is live with
   vector<int> order;
   for (size_t k = 0; k < plan->storages.size(); ++k) {
     if (plan->storages[k].outside.empty()) {
