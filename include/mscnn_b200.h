@@ -378,6 +378,19 @@ MSCNN_API int mscnn_detect_postprocess_sized(const mscnn_detect_cfg* cfg, int N,
                                              void* workspace, size_t workspace_bytes, float* dets, int* det_counts,
                                              const float* geom, void* stream);
 
+/* The drivers' proposal list (examples/kitti_car/run_mscnn_detection.m:75-91, the same lines in kitti_ped_cyc, caltech
+ * :83-96, widerface :96-109), on the device: for image n, the rows of BoxOutput's proposals_score [R][6] (num_rois:
+ * its DEVICE row counts, read as the post-process reads them, so a lazy row count needs no host wait) with
+ * w = x2 - x1, h = y2 - y1 in single, kept iff score >= cfg->proposal_thr && w != 0 && h != 0 (single compares; a NaN
+ * score is dropped), in row order, written as float64 props[n][k] = [x y w h score] with x and w divided by
+ * (double)net_w / org_w and y and h by (double)net_h / org_h in double, without clipping.  counts[n] = rows kept.
+ * cap = cfg->max_rois_per_image; props is [N][cap][5].  org_hw: HOST int [N][2] = h, w per image, or NULL for
+ * cfg->org_h / org_w.  Reads cfg->proposal_thr, max_rois_per_image and (org_hw NULL) org_h, org_w only.  An image
+ * with more kept rows than cap gets counts[n] = -1 (mscnn_net_proposals refuses such a cap before any launch). */
+MSCNN_API int mscnn_proposals_postprocess(const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
+                                          const int* num_rois, int net_h, int net_w, const int* org_hw, double* props,
+                                          int* counts, void* stream);
+
 /* Packed output of the same post-process, for the multi-GPU exchange below: `payload` (device,
  * mscnn_detect_payload_floats(N, max_rois_per_image) floats) = int32 header [N, total, counts[0..N)] padded to a
  * multiple of 4 words, then the kept rows of all N images back to back, [total][5] = [x y w h prob] in image order. */
@@ -679,6 +692,11 @@ MSCNN_API int mscnn_net_detect_cascade_classes(void* net, const mscnn_detect_cfg
                                                float* dets_dev, int* det_counts_dev);
 MSCNN_API int mscnn_net_detect_push_classes(void* net, const mscnn_detect_cfg* cfg, const mscnn_detect_classes* classes,
                                             void* xchg);
+/* mscnn_proposals_postprocess on the last forward's proposals_score, with its per-image original sizes (or cfg's
+ * org_h / org_w when it had none) and the net input size, on the net's stream: props_dev [N][max_rois_per_image][5]
+ * float64, counts_dev [N].  Refused like mscnn_net_detect* (MSCNN_ERR_INVALID, nothing launched): a cap below what
+ * BoxOutput can emit per image, or proposals_score released under activation reuse (mscnn_net_last_error). */
+MSCNN_API int mscnn_net_proposals(void* net, const mscnn_detect_cfg* cfg, double* props_dev, int* counts_dev);
 
 
 /* ------------------------------------------------------------------------------------

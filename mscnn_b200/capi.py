@@ -224,6 +224,11 @@ def _declare(L: C.CDLL) -> None:
     L.mscnn_detect_postprocess_classes_packed.restype = c_int
     L.mscnn_detect_postprocess_classes_packed.argtypes = [C.POINTER(DetectCfg), C.POINTER(DetectClasses), c_int] + \
         [c_void_p] * 5 + [C.c_size_t] + [c_void_p] * 3
+    L.mscnn_proposals_postprocess.restype = c_int
+    L.mscnn_proposals_postprocess.argtypes = [C.POINTER(DetectCfg), c_int, c_void_p, c_void_p, c_int, c_int] + \
+        [c_void_p] * 4
+    L.mscnn_net_proposals.restype = c_int
+    L.mscnn_net_proposals.argtypes = [c_void_p, C.POINTER(DetectCfg), c_void_p, c_void_p]
 
 
     L.mscnn_preprocess_create.restype = c_int

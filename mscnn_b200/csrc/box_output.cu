@@ -1024,3 +1024,95 @@ extern "C" int mscnn_detect_postprocess_classes_packed(const mscnn_detect_cfg* c
   return detect_postprocess(false, cfg, classes, N, proposals_score, cls_pred, bbox_pred, num_rois, workspace,
                             workspace_bytes, geom, DetectOut::packed(payload), stream);
 }
+
+// ------------------------------------------------------------------------------------------------- proposal list
+// The drivers' proposal list (examples/kitti_car/run_mscnn_detection.m:78-91, the same lines in kitti_ped_cyc, caltech
+// :83-96, widerface :96-109): w = x2 - x1 and h = y2 - y1 of every proposals_score row in single (:78), the row kept iff
+// score >= proposal_thr && w ~= 0 && h ~= 0 in single (:82, `find` keeps row order), then widened to double and divided
+// by the double ratios net / original (:86-90), without clipping.  The detection path divides by the fp32 ratio_*
+// instead, because there MATLAB divides singles; here the operands are doubles, and a single quotient rounded from the
+// fp32 ratio can differ from the double one in the last place of the double.
+namespace mscnn {
+constexpr int kPropThreads = 256;
+constexpr int kPropPerLaunch = 64;
+struct ProposalRatios {
+  int n0;
+  double2 r[kPropPerLaunch];  // (ratio_h, ratio_w) of images n0, n0 + 1, ... (one CTA each)
+};
+}  // namespace mscnn
+
+// One CTA per image: chunks of kPropThreads rows, each compacted in row order by a warp ballot and a prefix over the
+// warps' counts, so the output order is the input order and does not depend on scheduling.
+__global__ void __launch_bounds__(kPropThreads)
+proposals_kernel(const ProposalRatios ratios, const float* __restrict__ prop, const int* __restrict__ num_rois,
+                 float thr, int cap, double* __restrict__ out, int* __restrict__ counts) {
+  __shared__ int s_warp[kPropThreads / 32];
+  const int n = ratios.n0 + blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const double rh = ratios.r[blockIdx.x].x, rw = ratios.r[blockIdx.x].y;
+  int start = 0;
+  for (int m = 0; m < n; ++m) start += num_rois[2 + m];
+  const int cnt = num_rois[2 + n];
+  double* o = out + (size_t)n * cap * 5;
+  int base = 0;  // rows kept before this chunk
+  for (int c0 = 0; c0 < cnt; c0 += kPropThreads) {
+    const int i = c0 + tid;
+    float x = 0.f, y = 0.f, w = 0.f, h = 0.f, sc = 0.f;
+    bool keep = false;
+    if (i < cnt) {
+      const float* q = prop + (size_t)(start + i) * 6;
+      x = q[1]; y = q[2]; w = q[3] - q[1]; h = q[4] - q[2]; sc = q[5];
+      keep = sc >= thr && w != 0.f && h != 0.f;  // a NaN score fails the compare, as in MATLAB
+    }
+    const unsigned ballot = __ballot_sync(0xFFFFFFFFu, keep);
+    if (lane == 0) s_warp[warp] = __popc(ballot);
+    __syncthreads();
+    int rank = base, total = base;
+    for (int k = 0; k < kPropThreads / 32; ++k) {
+      if (k < warp) rank += s_warp[k];
+      total += s_warp[k];
+    }
+    rank += __popc(ballot & ((1u << lane) - 1u));
+    if (keep && rank < cap) {
+      double* r = o + (size_t)rank * 5;
+      r[0] = (double)x / rw; r[1] = (double)y / rh; r[2] = (double)w / rw; r[3] = (double)h / rh; r[4] = (double)sc;
+    }
+    base = total;
+    __syncthreads();  // s_warp is rewritten by the next chunk
+  }
+  if (tid == 0) counts[n] = base <= cap ? base : -1;
+}
+
+extern "C" int mscnn_proposals_postprocess(const mscnn_detect_cfg* cfg, int N, const float* proposals_score,
+                                           const int* num_rois, int net_h, int net_w, const int* org_hw, double* props,
+                                           int* counts, void* stream_v) {
+  if (!cfg || N <= 0 || !proposals_score || !num_rois || !props || !counts || net_h < 1 || net_w < 1)
+    return MSCNN_ERR_INVALID;
+  if (cfg->max_rois_per_image <= 0) return MSCNN_ERR_INVALID;
+  if (org_hw) {
+    for (int n = 0; n < N; ++n)
+      if (org_hw[2 * n] < 1 || org_hw[2 * n + 1] < 1) return MSCNN_ERR_INVALID;
+  } else if (!(cfg->org_h > 0.f && cfg->org_w > 0.f) || cfg->org_h == INFINITY || cfg->org_w == INFINITY) {
+    return MSCNN_ERR_INVALID;
+  }
+  cudaStream_t stream = (cudaStream_t)stream_v;
+  for (int n0 = 0; n0 < N; n0 += kPropPerLaunch) {
+    const int blocks = N - n0 < kPropPerLaunch ? N - n0 : kPropPerLaunch;
+    ProposalRatios r;
+    r.n0 = n0;
+    for (int i = 0; i < blocks; ++i) {
+      // ratios = [imgH imgW] ./ [orgH orgW] (run_mscnn_detection.m:65), in double as MATLAB keeps it
+      const double oh = org_hw ? (double)org_hw[2 * (n0 + i)] : (double)cfg->org_h;
+      const double ow = org_hw ? (double)org_hw[2 * (n0 + i) + 1] : (double)cfg->org_w;
+      r.r[i] = make_double2((double)net_h / oh, (double)net_w / ow);
+    }
+    mscnn::note_launch();
+    proposals_kernel<<<blocks, kPropThreads, 0, stream>>>(r, proposals_score, num_rois, cfg->proposal_thr,
+                                                          cfg->max_rois_per_image, props, counts);
+  }
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    fprintf(stderr, "mscnn_proposals_postprocess: %s\n", cudaGetErrorString(e));
+    return MSCNN_ERR_CUDA;
+  }
+  return MSCNN_OK;
+}

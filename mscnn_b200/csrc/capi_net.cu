@@ -646,4 +646,31 @@ int mscnn_net_detect_push_classes(void* hv, const mscnn_detect_cfg* cfg, const m
   return mscnn::xchg_detect_push(cfg, classes, in.N, in.prop, in.cls, in.bbox, h->box->num_out_device(), h->det_ws,
                                  h->det_ws_bytes, xchg, in.geom, Caffe::stream());
 }
+// The proposal list of the last forward.  The original sizes come back from its geometry: org_* there is the
+// (float) of the int size, exact for any image size.
+int mscnn_net_proposals(void* hv, const mscnn_detect_cfg* cfg, double* props_dev, int* counts_dev) {
+  NetHandle* h = H(hv);
+  if (!h || !h->box || !cfg || !props_dev || !counts_dev || !h->net->has_blob("proposals_score"))
+    return MSCNN_ERR_INVALID;
+  // the drivers keep every proposal of an image: a cap below what BoxOutput can emit is refused, as in detect_inputs
+  if (cfg->max_rois_per_image < h->box->max_rows_per_image()) {
+    refuse(h, "mscnn_net_proposals",
+           "max_rois_per_image = " + std::to_string(cfg->max_rois_per_image) + " < " +
+               std::to_string(h->box->max_rows_per_image()) +
+               " proposals an image can carry (BoxOutput max_nms_num / max_post_nms_num)");
+    return MSCNN_ERR_INVALID;
+  }
+  if (released(h, "mscnn_net_proposals", "proposals_score")) return MSCNN_ERR_INVALID;
+  const Blob<float>* in = h->net->input_blobs()[0];
+  const int N = in->num();
+  if (!h->geom.empty() && h->geom.size() != (size_t)4 * N) return MSCNN_ERR_INVALID;
+  std::vector<int> org_hw;
+  for (int n = 0; n < (int)h->geom.size() / 4; ++n) {
+    org_hw.push_back((int)h->geom[4 * n + 2]);
+    org_hw.push_back((int)h->geom[4 * n + 3]);
+  }
+  return mscnn_proposals_postprocess(cfg, N, h->net->blob_by_name("proposals_score")->gpu_data(),
+                                     h->box->num_out_device(), in->height(), in->width(),
+                                     org_hw.empty() ? nullptr : org_hw.data(), props_dev, counts_dev, Caffe::stream());
+}
 }

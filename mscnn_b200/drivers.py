@@ -7,6 +7,8 @@ writes the drivers' files.  Every image's detections are those of the drivers' o
 
     res = drivers.run(net, frames, drivers.KITTI_CAR)          # per image: [per class: [k][5] = x y w h prob]
     drivers.write_results("detections", drivers.KITTI_CAR, comp_id, res)   # detections/<comp_id>_car.txt
+    res, props = drivers.run(net, frames, drivers.KITTI_CAR, proposals=True)  # + per image: float64 [k][5] proposals
+    drivers.write_proposals("proposals", drivers.KITTI_CAR, comp_id, props)   # proposals/<comp_id>.txt
 
 Several nets (make_nets: one per device entry, the weights loaded once per device and shared by the nets on it) run
 the same frames with one host thread per net, each on its own stream; the result is the one-net result, bit for bit:
@@ -44,6 +46,7 @@ class DriverSpec:
     det_thr: float                        # <= 0: off
     result_files: tuple[str, ...]         # one per class, "{comp_id}" filled in
     index_across_groups: bool             # the image index runs across groups of frames (CityPersons' idcount)
+    proposals_file: str | None = None     # the proposal list's file under proposals/, "{comp_id}" filled in; None: none
     source: dict = field(default_factory=dict, compare=False)
 
     def detect_cfg(self, net_hw: tuple[int, int] | None = None) -> tuple[capi.DetectCfg, capi.DetectClasses]:
@@ -69,29 +72,35 @@ KITTI_CAR = DriverSpec(
     script="examples/kitti_car/run_mscnn_detection.m",
     net_hw=(768, 2560), num_cls=5, cls_ids=(2,), obj_names=("bg", "car", "van", "truck", "tram"), cascade=False,
     blobs=PLAIN_BLOBS, bbox_stds=(0.1, 0.1, 0.2, 0.2), proposal_thr=-10.0, nms_overlap=0.5, det_thr=-1.0,
-    result_files=("{comp_id}_car.txt",), index_across_groups=False,
+    result_files=("{comp_id}_car.txt",), index_across_groups=False, proposals_file="{comp_id}.txt",
     source={"net_hw": ":36", "bbox_stds": ":42-43", "nms_overlap": ":46", "cls_ids": ":48", "obj_names": ":49",
             "proposal_thr": ":51", "blobs": ":75-77", "det_thr": "none (no threshold before bbNms, :117-119)",
             "result_files": ":156-160", "index": ":150-153 (k = position in image_list)",
+            "proposals": ":75-91 (keep_id :82, double then ./ ratios :86-90)",
+            "proposals_file": ":162 (commented dlmwrite, index :154, cell2mat :161)",
             "num_cls": "mscnn-8s-768-trainval/mscnn_deploy.prototxt cls_pred num_output 5"})
 
 KITTI_PED_CYC = DriverSpec(
     script="examples/kitti_ped_cyc/run_mscnn_detection.m",
     net_hw=(768, 2560), num_cls=3, cls_ids=(2, 3), obj_names=("bg", "ped", "cyc"), cascade=False,
     blobs=PLAIN_BLOBS, bbox_stds=(0.1, 0.1, 0.2, 0.2), proposal_thr=-10.0, nms_overlap=0.5, det_thr=-1.0,
-    result_files=("{comp_id}_ped.txt", "{comp_id}_cyc.txt"), index_across_groups=False,
+    result_files=("{comp_id}_ped.txt", "{comp_id}_cyc.txt"), index_across_groups=False, proposals_file="{comp_id}.txt",
     source={"net_hw": ":36", "bbox_stds": ":42-43", "nms_overlap": ":46", "cls_ids": ":48", "obj_names": ":49",
             "proposal_thr": ":51", "blobs": ":75-77", "det_thr": "none (:117-119)", "result_files": ":156-160",
+            "proposals": ":75-91 (keep_id :82, double then ./ ratios :86-90)",
+            "proposals_file": ":162 (commented dlmwrite, index :154, cell2mat :161)",
             "index": ":150-153", "num_cls": "mscnn-8s-768-trainval/mscnn_deploy.prototxt cls_pred num_output 3"})
 
 CALTECH = DriverSpec(
     script="examples/caltech/run_mscnn_detection.m",
     net_hw=(720, 960), num_cls=2, cls_ids=(2,), obj_names=("bg", "ped"), cascade=False,
     blobs=PLAIN_BLOBS, bbox_stds=None, proposal_thr=-10.0, nms_overlap=0.5, det_thr=-1.0,
-    result_files=("{comp_id}_ped.txt",), index_across_groups=False,
+    result_files=("{comp_id}_ped.txt",), index_across_groups=False, proposals_file="{comp_id}.txt",
     source={"net_hw": ":35", "bbox_stds": ":41-48 (do_bb_norm = 0: bbox_means = [], bbox_stds = [])",
             "nms_overlap": ":51", "cls_ids": ":53", "obj_names": ":54", "proposal_thr": ":56", "blobs": ":80-82",
             "det_thr": "none (:124-126)", "result_files": ":163-167", "index": ":157-160",
+            "proposals": ":80-96 (keep_id :87, double then ./ ratios :91-95)",
+            "proposals_file": ":169 (commented dlmwrite, index :161, cell2mat :168)",
             "num_cls": "mscnn-7s-720/mscnn_deploy.prototxt cls_pred num_output 2"})
 
 KITTI_CAR_CASCADE = DriverSpec(
@@ -115,8 +124,27 @@ CITYPERSONS = DriverSpec(
             "bbox_stds": "none: the net decodes the boxes (DecodeBBox)",
             "num_cls": "cascade-mscnn-8s-1344-2x/mscnn_deploy.prototxt cls_prob_3rd_avg: 2 classes"})
 
+# The CityPersons script's default net, mscnn-8s-1344-2x-pretrained (:11): no "cascade" in its path, so CASCADE = 0
+# and the script post-processes the single stage's decoded boxes.
+CITYPERSONS_BASELINE = DriverSpec(
+    script="examples/citypersons/run_cascademscnn.m",
+    net_hw=(1344, 2688), num_cls=2, cls_ids=(2,), obj_names=None, cascade=True,
+    blobs=("proposals", "cls_prob_1st", "output_bbox_1st"), bbox_stds=None, proposal_thr=None,
+    nms_overlap=0.5, det_thr=-1.0, result_files=("{comp_id}_1st_results.txt",), index_across_groups=True,
+    source={"script": ":11 (root_dir mscnn-8s-1344-2x-pretrained), :34-35 (CASCADE = 0)", "cls_ids": ":31 (obj_ids)",
+            "obj_names": "none (the script has no obj_names)", "cascade": ":97-131 (the decoded-box post-process)",
+            "blobs": ":36-41 (~CASCADE: proposals, cls_prob_1st, output_bbox_1st)", "det_thr": ":56",
+            "nms_overlap": ":57", "net_hw": ":63, :85 (multiples of 32)", "gray": ":82",
+            "result_files": ":155-165 (output_names {'1st'} :41)",
+            "index_across_groups": ":74, :131, :150 (idcount runs across the city directories :75-151)",
+            "index": ":74, :131, :150", "proposal_thr": "none: only w, h ~= 0 are filtered (:119)",
+            "bbox_stds": "none: the net decodes the boxes (DecodeBBox output_bbox_1st)",
+            "proposals_file": "none: the script computes no proposal list",
+            "num_cls": "mscnn-8s-1344-2x/mscnn_deploy.prototxt cls_prob_1st: 2 classes"})
+
 SPECS = {"kitti_car": KITTI_CAR, "kitti_ped_cyc": KITTI_PED_CYC, "caltech": CALTECH,
-         "kitti_car_cascade": KITTI_CAR_CASCADE, "citypersons": CITYPERSONS}
+         "kitti_car_cascade": KITTI_CAR_CASCADE, "citypersons": CITYPERSONS,
+         "citypersons_baseline": CITYPERSONS_BASELINE}
 
 
 def make_nets(proto: str, weights, devices=(0,), reuse_activations: bool = False) -> list:
@@ -219,7 +247,16 @@ def _plans(pre, n):
     return list(pre)
 
 
-def run(nets, frames, spec: DriverSpec, batch: int = 8, net_hw: tuple[int, int] | None = None, pre=None) -> list:
+def _cascade_stage(spec: DriverSpec) -> str:
+    """The stage whose blobs a cascade spec reads: "1st" (proposals, output_bbox_1st) or "3rd"."""
+    for stage, prop in (("1st", "proposals"), ("3rd", "proposals_3rd")):
+        if spec.blobs[0] == prop and spec.blobs[2] == f"output_bbox_{stage}":
+            return stage
+    raise ValueError(f"unsupported cascade blobs {spec.blobs}")
+
+
+def run(nets, frames, spec: DriverSpec, batch: int = 8, net_hw: tuple[int, int] | None = None, pre=None,
+        proposals: bool = False):
     """Final detections of uint8 host frames ([h][w][3], or gray [h][w] / [h][w][1], any sizes) on `nets` at the one
     net size `net_hw` (default spec.net_hw), as the driver `spec` computes them.
 
@@ -232,38 +269,46 @@ def run(nets, frames, spec: DriverSpec, batch: int = 8, net_hw: tuple[int, int] 
     nets: one net.Net, run on the calling thread and stream; or a list of nets (make_nets), each served by a host thread
     of its own on its device, in this thread's precision, on a stream of its own.  The batches are handed out whole
     in input order (serve_batches); the result is the one-net result, bit for bit.  pre is then None or one plan per
-    net."""
+    net.
+
+    proposals=True: returns (dets, props), props[i] being image i's proposal list, float64 [k][5] = x y w h score in
+    original-image coordinates (run_mscnn_detection.m:75-91, Net.proposals), issued after the detections of the same
+    batch on the same stream.  Only the plain specs have one: a cascade spec raises ValueError."""
     from . import net as mnet, ops
     if batch < 1:
         raise ValueError(f"batch ({batch}) must be positive")
-    if spec.cascade and (spec.blobs[0] != "proposals_3rd" or spec.blobs[2] != "output_bbox_3rd"):
-        raise ValueError(f"unsupported cascade blobs {spec.blobs}")
+    if spec.cascade:
+        _cascade_stage(spec)
+        if proposals:
+            raise ValueError(f"{spec.script} computes no proposal list")
     frames = list(frames)
     out: list = [None] * len(frames)
+    props: list | None = [None] * len(frames) if proposals else None
     if not frames:
-        return out
+        return (out, props) if proposals else out
     net_hw = tuple(net_hw or spec.net_hw)
     ops.image_sizes_channels(frames)                          # every frame checked before any work is issued
     keep_readable(nets, spec.blobs)
     chunks = [list(range(k, min(k + batch, len(frames)))) for k in range(0, len(frames), batch)]
+    extra = (props,) if proposals else ()     # the proposal list's output, only when one is asked for
     if not isinstance(nets, (list, tuple)):
         todo = iter(chunks)
-        _serve_fixed(nets, lambda: next(todo, None), frames, spec, net_hw, pre, out)
-        return out
+        _serve_fixed(nets, lambda: next(todo, None), frames, spec, net_hw, pre, out, *extra)
+        return (out, props) if proposals else out
     plans = dict(zip(map(id, nets), _plans(pre, len(nets))))
     precision = mnet.get_precision()
 
     def serve(net, take):
         with net_thread(net, precision):
-            _serve_fixed(net, take, frames, spec, net_hw, plans[id(net)], out)
+            _serve_fixed(net, take, frames, spec, net_hw, plans[id(net)], out, *extra)
 
     serve_batches(nets, chunks, serve)
-    return out
+    return (out, props) if proposals else out
 
 
-def _serve_fixed(net, take, frames, spec: DriverSpec, net_hw, pre, out: list) -> None:
+def _serve_fixed(net, take, frames, spec: DriverSpec, net_hw, pre, out: list, props: list | None = None) -> None:
     """run's loop on one net, in the calling thread: take() gives the next batch of frame indices (None: done), and
-    out[i] receives image i's detections."""
+    out[i] receives image i's detections, props[i] (props not None) its proposal list."""
     import torch
     from . import net as mnet, ops
     idx = take()
@@ -290,18 +335,53 @@ def _serve_fixed(net, take, frames, spec: DriverSpec, net_hw, pre, out: list) ->
             dets = torch.empty((n, c, cfg.max_rois_per_image, 5), dtype=torch.float32, device="cuda")
             counts = torch.empty((n, c), dtype=torch.int32, device="cuda")
             if spec.cascade:
-                net.detect_cascade_classes(cfg, classes, dets.data_ptr(), counts.data_ptr(), stage="3rd",
+                net.detect_cascade_classes(cfg, classes, dets.data_ptr(), counts.data_ptr(), stage=_cascade_stage(spec),
                                            cls_prob=spec.blobs[1])
             else:
                 net.detect_classes(cfg, classes, dets.data_ptr(), counts.data_ptr())
+            if props is not None:
+                pp = read_proposals(net, cfg, n)
             cnt = counts.cpu().numpy()
             kmax = int(cnt.max()) if cnt.size else 0
             d = dets[:, :, :kmax].cpu().numpy()
         for j, i in enumerate(idx):
             out[i] = [d[j, s, :cnt[j, s]].copy() for s in range(c)]
+            if props is not None:
+                props[i] = pp[j]
         if nxt is not None and len(nxt) != len(idx):
             net.set_input_images(data, pre, [frames[i] for i in nxt])
         idx = nxt
+
+
+def read_proposals(net, cfg, n: int) -> list[np.ndarray]:
+    """Net.proposals of the last forward of `n` images, issued on the current torch stream and read back: per image
+    float64 [k][5].  Only the rows up to the largest count are copied."""
+    import torch
+    props = torch.empty((n, cfg.max_rois_per_image, 5), dtype=torch.float64, device="cuda")
+    counts = torch.empty(n, dtype=torch.int32, device="cuda")
+    net.proposals(cfg, props.data_ptr(), counts.data_ptr())
+    cnt = counts.cpu().numpy()
+    kmax = int(cnt.max()) if cnt.size else 0
+    p = props[:, :kmax].cpu().numpy()
+    return [p[j, :cnt[j]].copy() for j in range(n)]
+
+
+def write_proposals(out_dir, spec: DriverSpec, comp_id: str, props, first_index: int = 1) -> Path:
+    """The proposal file the plain drivers leave commented out (run_mscnn_detection.m:154, :161-162;
+    caltech :161, :168-169): dlmwrite(['proposals/' comp_id '.txt'], [index x y w h score]) of every image in order,
+    ',' and %.5g of the float64 values (the float32 writer would round them first).  props: per image, a float64
+    [k][5] list (what run(..., proposals=True) returns); image i has index first_index + i.  out_dir (created with
+    its parents) plays the script's proposals/.  Returns the path written."""
+    if spec.proposals_file is None:
+        raise ValueError(f"{spec.script} writes no proposal list")
+    path = Path(out_dir) / spec.proposals_file.format(comp_id=comp_id)
+    Path(out_dir).mkdir(parents=True, exist_ok=True)
+    lines = []
+    for i, p in enumerate(props):
+        for row in np.asarray(p, dtype=np.float64).reshape(-1, 5):
+            lines.append(",".join("%.5g" % v for v in (float(first_index + i), *row.tolist())) + "\n")
+    path.write_text("".join(lines))
+    return path
 
 
 def write_results(out_dir, spec: DriverSpec, comp_id: str, results, first_index: int = 1,

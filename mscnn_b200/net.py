@@ -422,6 +422,11 @@ class Net:
         parallel._declare_xchg(self._L)
         self._check(self._L.mscnn_net_detect_push_classes(self._h, cfg, classes, xchg.handle), "net_detect_push_classes")
 
+    def proposals(self, cfg: capi.DetectCfg, props_dev_ptr: int, counts_dev_ptr: int) -> None:
+        """The drivers' proposal list of the last forward (mscnn_net_proposals): props float64
+        [N][cfg.max_rois_per_image][5] = x y w h score in original-image coordinates, counts int32 [N]."""
+        self._check(self._L.mscnn_net_proposals(self._h, cfg, props_dev_ptr, counts_dev_ptr), "net_proposals")
+
     def fused_producer(self, layer: str) -> str:
         """The layer that does `layer`'s work (itself unless the fusion pass folded it into another layer)."""
         i = self._L.mscnn_net_fused_producer(self._h, self.layer_names.index(layer))

@@ -549,6 +549,23 @@ def detect_postprocess_classes_packed(cfg: capi.DetectCfg, classes: capi.DetectC
                            (proposals_score, cls_pred, bbox_pred), num_out, geometry, packed=True)
 
 
+def proposals_postprocess(cfg: capi.DetectCfg, n: int, proposals_score, num_out, net_hw, org_hw=None):
+    """The drivers' proposal list (mscnn_proposals_postprocess): props float64 [n, cap, 5] = x y w h score in
+    original-image coordinates, counts int32 [n] (-1: more kept rows than cap = cfg.max_rois_per_image).  org_hw:
+    None (cfg.org_h / org_w) or per-image [n][2] = h, w."""
+    dev = proposals_score.device
+    props = torch.zeros((n, cfg.max_rois_per_image, 5), dtype=torch.float64, device=dev)
+    counts = torch.zeros(n, dtype=torch.int32, device=dev)
+    hw = None
+    if org_hw is not None:
+        hw = np.ascontiguousarray(org_hw, dtype=np.int32)
+        assert hw.shape == (n, 2), (hw.shape, n)
+    capi.check(capi.lib().mscnn_proposals_postprocess(cfg, n, capi.ptr(proposals_score), capi.ptr(num_out),
+                                                      int(net_hw[0]), int(net_hw[1]), capi.ptr(hw), capi.ptr(props),
+                                                      capi.ptr(counts), _stream()), "proposals_postprocess")
+    return props, counts
+
+
 def conv1_tc_forward(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None, relu: bool, split: bool) -> Planes:
     """conv1_1 (3 -> 64, 3x3, pad 1) as the single tensor-core kernel: x [N,3,H,W] fp32 NCHW -> planes."""
     n, c, h, wd = x.shape

@@ -46,7 +46,7 @@ def plan_batches(org_hw, img_hw=(0, 0), max_size: int = MAX_SIZE, max_batch: int
 
 
 def run(nets, frames, names, cascade: bool = False, max_size: int = MAX_SIZE, max_batch: int = 8,
-        pixel_budget: int = PIXEL_BUDGET, plans: dict | None = None) -> dict[str, np.ndarray]:
+        pixel_budget: int = PIXEL_BUDGET, plans: dict | None = None, proposals: bool = False):
     """Final face detections of uint8 [h][w][3] host frames (any sizes) on `nets`, models.widerface nets (or, with
     cascade=True, models.widerface_cascade nets read at proposals_3rd / cls_prob_3rd_avg / output_bbox_3rd as
     run_cascademscnn.m:44-47 does), with the drivers' settings (net.widerface_detect_cfg).
@@ -57,21 +57,32 @@ def run(nets, frames, names, cascade: bool = False, max_size: int = MAX_SIZE, ma
 
     nets: one net.Net, run on the calling thread and stream; or a list of nets (drivers.make_nets), each served by a
     host thread of its own (drivers.serve_batches, drivers.net_thread) taking plan_batches' batches, largest first,
-    from one queue.  plans is then None or a list of one dict per net.  The result is the one-net result, bit for bit."""
+    from one queue.  plans is then None or a list of one dict per net.  The result is the one-net result, bit for bit.
+
+    proposals=True (plain nets only): returns (dets, props), props = {name: float64 [k][5] = x y w h score}, each
+    image's proposal list at its own net size with proposal_thr -5 (run_mscnn_detection.m:55, :95-109)."""
     from . import drivers, net as mnet, ops
     names = list(names)
     if len(names) != len(frames) or len(set(names)) != len(names):
         raise ValueError("one distinct name per frame is needed")
+    if cascade and proposals:
+        raise ValueError("run_cascademscnn.m computes no proposal list")
     hw = ops.image_sizes(frames)
     kept: list[np.ndarray | None] = [None] * len(frames)
+    props: list | None = [None] * len(frames) if proposals else None
+
+    def result():
+        dets = dict(zip(names, kept))
+        return (dets, dict(zip(names, props))) if proposals else dets
+
     batches = plan_batches(hw, max_size=max_size, max_batch=max_batch, pixel_budget=pixel_budget)
     drivers.keep_readable(nets, ("proposals_3rd", "cls_prob_3rd_avg", "output_bbox_3rd") if cascade
                           else ("proposals_score", "cls_pred", "bbox_pred"))
     if not isinstance(nets, (list, tuple)):
         plans = {} if plans is None else plans
         for b in batches:
-            _run_batch(nets, frames, hw, b, cascade, plans, kept)
-        return dict(zip(names, kept))
+            _run_batch(nets, frames, hw, b, cascade, plans, kept, props)
+        return result()
     if plans is None:
         plans = [{} for _ in nets]
     elif not isinstance(plans, (list, tuple)) or len(plans) != len(nets):
@@ -83,17 +94,18 @@ def run(nets, frames, names, cascade: bool = False, max_size: int = MAX_SIZE, ma
         with drivers.net_thread(net, precision):
             b = take()
             while b is not None:
-                _run_batch(net, frames, hw, b, cascade, per_net[id(net)], kept)
+                _run_batch(net, frames, hw, b, cascade, per_net[id(net)], kept, props)
                 b = take()
 
     drivers.serve_batches(nets, batches, serve)
-    return dict(zip(names, kept))
+    return result()
 
 
-def _run_batch(net, frames, hw, batch, cascade: bool, plans: dict, kept: list) -> None:
-    """One plan_batches entry ((net_h, net_w), image indices) on `net` in the calling thread, into kept[i]."""
+def _run_batch(net, frames, hw, batch, cascade: bool, plans: dict, kept: list, props: list | None = None) -> None:
+    """One plan_batches entry ((net_h, net_w), image indices) on `net` in the calling thread, into kept[i] (and
+    props[i], props not None)."""
     import torch
-    from . import net as mnet, ops
+    from . import drivers, net as mnet, ops
     (rz_h, rz_w), idx = batch
     n = len(idx)
     data = net.inputs[0]
@@ -112,9 +124,13 @@ def _run_batch(net, frames, hw, batch, cascade: bool, plans: dict, kept: list) -
                                        cls_prob="cls_prob_3rd_avg")
         else:
             net.detect_classes(cfg, classes, dets.data_ptr(), counts.data_ptr())
+        if props is not None:
+            pp = drivers.read_proposals(net, cfg, n)
         d, c = dets.cpu().numpy(), counts.cpu().numpy()
     for k, i in enumerate(idx):
         kept[i] = d[k, 0, :c[k, 0]].copy()
+        if props is not None:
+            props[i] = pp[k]
 
 
 def write_results(event_dir, results) -> None:
