@@ -596,6 +596,22 @@ MSCNN_API int mscnn_net_set_blob_device(void* net, const char* blob, const float
 MSCNN_API int mscnn_net_set_blob_async(void* net, const char* blob, const float* host, long count);
 MSCNN_API int mscnn_net_get_blob(void* net, const char* blob, float* host, long count);             /* D2H + sync */
 MSCNN_API const float* mscnn_net_blob_device(void* net, const char* blob);
+/* pycaffe's Blob.data (_caffe.cpp binds it to mutable_cpu_data): the host side of a blob, or of parameter blob i of
+ * `layer`, NCHW fp32 in the blob's shape, after the net's stream has drained (no queued copy reads or writes it).  The
+ * memory is valid until that blob's next reshape.  As with every mutable_* accessor the storage's version changes, so
+ * what is written there is uploaded by the next forward that reads the blob, and a weight written there is packed
+ * again before the next forward.  NULL for an unknown name or index, and, with mscnn_net_last_error saying why, for a
+ * blob released by activation reuse. */
+MSCNN_API float* mscnn_net_blob_cpu_data(void* net, const char* blob);
+MSCNN_API float* mscnn_net_param_cpu_data(void* net, const char* layer, int i);
+/* The blob indices (mscnn_net_blob_name order) layer i reads and writes (Net::bottom_ids / top_ids, pycaffe's
+ * _bottom_ids / _top_ids), split blobs included: up to cap of them into ids; returns how many the layer has, or
+ * MSCNN_ERR_INVALID for a layer index out of range. */
+MSCNN_API int mscnn_net_layer_bottoms(void* net, int i, int* ids, int cap);
+MSCNN_API int mscnn_net_layer_tops(void* net, int i, int* ids, int cap);
+/* The registered layer types (LayerRegistry::LayerTypeList), in name order, one per line, into buf; returns how many
+ * there are, or MSCNN_ERR_INVALID when cap is too small. */
+MSCNN_API int mscnn_layer_type_list(char* buf, int cap);
 /* uint8 host images -> pre-processing kernels -> the input blob (N, in size and out size from the plan / blob). */
 MSCNN_API int mscnn_net_set_input_images(void* net, const char* blob, void* preprocess_plan, int N,
                                          const unsigned char* host_images);

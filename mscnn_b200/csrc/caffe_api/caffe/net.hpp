@@ -66,6 +66,17 @@ class CAFFE_API Net {
   inline Phase phase() const { return phase_; }
   inline const vector<vector<Blob<Dtype>*> >& bottom_vecs() const { return bottom_vecs_; }
   inline const vector<vector<Blob<Dtype>*> >& top_vecs() const { return top_vecs_; }
+  // the blob indices layer i writes / reads (net.hpp:154-165 of the reference)
+  inline const vector<int>& top_ids(int i) const {
+    CHECK_GE(i, 0) << "Invalid layer id";
+    CHECK_LT(i, (int)top_id_vecs_.size()) << "Invalid layer id";
+    return top_id_vecs_[i];
+  }
+  inline const vector<int>& bottom_ids(int i) const {
+    CHECK_GE(i, 0) << "Invalid layer id";
+    CHECK_LT(i, (int)bottom_id_vecs_.size()) << "Invalid layer id";
+    return bottom_id_vecs_[i];
+  }
   inline int num_inputs() const { return (int)net_input_blobs_.size(); }
   inline int num_outputs() const { return (int)net_output_blobs_.size(); }
   inline const vector<Blob<Dtype>*>& input_blobs() const { return net_input_blobs_; }

@@ -5,6 +5,7 @@
 #include <sstream>
 #include <string>
 
+#include "caffe/layer_factory.hpp"
 #include "caffe/layers/mscnn_layers.hpp"
 #include "caffe/net.hpp"
 #include "mscnn_b200.h"
@@ -143,6 +144,11 @@ int detect_inputs(NetHandle* h, const mscnn_detect_cfg* cfg, const mscnn_detect_
   in->bbox = h->net->blob_by_name(bbox)->gpu_data();
   in->geom = h->geom.empty() ? nullptr : h->geom.data();
   return MSCNN_OK;
+}
+// Whether the net's stream has finished all it was given (a net built without a device has no stream: it holds host
+// data only).
+bool drained(NetHandle* nh) {
+  return nh->net->device() < 0 || cudaStreamSynchronize(Caffe::stream()) == cudaSuccess;
 }
 int fill_shape(const std::vector<int>& s, int* shape4) {
   for (size_t d = 0; d < s.size() && d < 4; ++d) shape4[d] = s[d];
@@ -423,6 +429,46 @@ const float* mscnn_net_blob_device(void* h, const char* name) {
   H(h)->net->ResolveRowsFor(name);
   if (!H(h)->net->has_blob(name) || released(H(h), "mscnn_net_blob_device", name)) return nullptr;
   return H(h)->net->blob_by_name(name)->gpu_data();
+}
+// pycaffe's Blob.data.  The stream is drained first: the view may be written as soon as it is returned, and an upload
+// of its previous contents may still be queued (SyncedMemory uploads from the pinned host side asynchronously).
+float* mscnn_net_blob_cpu_data(void* h, const char* name) {
+  NetHandle* nh = H(h);
+  nh->net->ResolveRowsFor(name);
+  nh->last_error.clear();
+  if (!nh->net->has_blob(name) || released(nh, "mscnn_net_blob_cpu_data", name)) return nullptr;
+  if (settle_pending(nh) != MSCNN_OK) return nullptr;
+  float* p = nh->net->blob_by_name(name)->mutable_cpu_data();
+  return drained(nh) ? p : nullptr;
+}
+float* mscnn_net_param_cpu_data(void* h, const char* layer, int i) {
+  NetHandle* nh = H(h);
+  nh->last_error.clear();
+  if (!nh->net->has_layer(layer)) return nullptr;
+  auto& blobs = nh->net->layer_by_name(layer)->blobs();
+  if (i < 0 || i >= (int)blobs.size()) return nullptr;
+  float* p = blobs[i]->mutable_cpu_data();
+  return drained(nh) ? p : nullptr;
+}
+static int copy_ids(const std::vector<int>& v, int* ids, int cap) {
+  for (int k = 0; k < (int)v.size() && k < cap; ++k) ids[k] = v[k];
+  return (int)v.size();
+}
+int mscnn_net_layer_bottoms(void* h, int i, int* ids, int cap) {
+  if (i < 0 || i >= (int)H(h)->net->layers().size() || (cap > 0 && !ids)) return MSCNN_ERR_INVALID;
+  return copy_ids(H(h)->net->bottom_ids(i), ids, cap);
+}
+int mscnn_net_layer_tops(void* h, int i, int* ids, int cap) {
+  if (i < 0 || i >= (int)H(h)->net->layers().size() || (cap > 0 && !ids)) return MSCNN_ERR_INVALID;
+  return copy_ids(H(h)->net->top_ids(i), ids, cap);
+}
+int mscnn_layer_type_list(char* buf, int cap) {
+  const std::vector<std::string> types = caffe::LayerRegistry<float>::LayerTypeList();
+  std::string s;
+  for (const std::string& t : types) s += t + "\n";
+  if (!buf || (int)s.size() + 1 > cap) return MSCNN_ERR_INVALID;
+  memcpy(buf, s.c_str(), s.size() + 1);
+  return (int)types.size();
 }
 
 // layers [from, to] inclusive; to < 0 = last (Net::ForwardFromTo, net.cpp:544-555)

@@ -60,6 +60,13 @@ def _declare(L):
     L.mscnn_net_get_blob.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long]
     L.mscnn_net_blob_device.restype = C.c_void_p
     L.mscnn_net_blob_device.argtypes = [C.c_void_p, C.c_char_p]
+    L.mscnn_net_blob_cpu_data.restype = C.c_void_p
+    L.mscnn_net_blob_cpu_data.argtypes = [C.c_void_p, C.c_char_p]
+    L.mscnn_net_param_cpu_data.restype = C.c_void_p
+    L.mscnn_net_param_cpu_data.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
+    for f in ("mscnn_net_layer_bottoms", "mscnn_net_layer_tops"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_int]
+    L.mscnn_layer_type_list.argtypes = [C.c_char_p, C.c_int]
     L.mscnn_net_forward.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.mscnn_net_set_layer_timing.argtypes = [C.c_void_p, C.c_int]
     L.mscnn_net_layer_times.argtypes = [C.c_void_p, C.c_void_p]
